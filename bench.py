@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""bench.py -- ADMM iterations/sec and time-to-eps of the SCS hot path on B200 (BASELINE.json metric).
+"""bench.py -- ADMM iterations/sec and time-to-eps of the SCS hot path on H100 (BASELINE.json metric).
 
   python bench.py [--gpus N] [--steps K] [--warmup W] [--impl ours|reference] [--config C2] [--scale f]
+                  [--dump-outputs DIR]
 
 A "step" is ONE ADMM iteration (normalise v -> indirect KKT solve by device PCG -> cone projection -> dual update,
 with Anderson acceleration every 10th step and the residual / scale check every 25th) on the synthetic workload
@@ -21,13 +22,17 @@ eps = 0 (so exactly K iterations run) -- identical algorithmic work, identical `
            for this, its figure is an extrapolation from its measured iterations/s and labelled so.
   roofline: the kernels of the CG loop AS THEY RUN IN THE SOLVE (spmv_flag_kernel<POST_MUL> on the solver's own p,
            <POST_FMA_DOT>+alpha hook on its tmp, k_cg_update, k_cg_pupdate), each bracketed by CUDA events inside
-           genuine CG iterations; consecutive kernels stream 2 x 124 MB of matrix data, more than the 126 MB L2.
+           genuine CG iterations; consecutive kernels stream 2 x 124 MB of matrix data, more than the 50 MB L2.
   parity : the gate of SURVEY 8(d) measured in this very run: our first ADMM iteration against the reference's
            (run beside the cpu_baseline sample), relative differences of x, y, s and the ScsInfo residuals.
   cpu_baseline: the UNMODIFIED reference CPU-indirect solver (oracle/_ref, OpenMP build) on a bounded sample (the
            first 3 iterations) of the same workload.
 
 --impl reference times that same reference solver for the same K cold iterations as the whole arm.
+--dump-outputs DIR writes what the timed solve returned in its last step -- x, y, s of the K-th iteration -- as
+DIR/{x,y,s}.npy (float64) and its ScsInfo scalars as DIR/info.npy; the inputs are fixed by --config, --scale and
+--seed, so two builds can be compared output for output. Beyond 64 MB in all, each vector is replaced by a fixed
+seeded sample (DIR/<name>_index.npy holds the sampled positions).
 N > 1: one process per GPU, ONE cooperative solve of the same workload (strong scaling): A is row-sharded across the
 ranks; the CG runs in the sharded-x push mode over NVLink peer memory (DESIGN.md section 6) and the line carries the
 per-phase timeline of one CG iteration (`cg_phases_us`, max over ranks).
@@ -56,7 +61,7 @@ CONFIG_DESC = {
 
 
 class ClockSampler(threading.Thread):
-    """nvidia-smi clocks / throttle reasons during the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons during the timed region (read-only queries)."""
 
     def __init__(self, gpu_index):
         super().__init__(daemon=True)
@@ -105,7 +110,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "MEASURED_PEAKS.json hbm_gbs (measured)"
         except Exception:
             pass
-    return 6650.0, "B200_PROFILING.md fallback 6.65 TB/s"
+    return 3350.0, "H100 SXM data-sheet HBM3 bandwidth 3.35 TB/s (not measured)"
 
 
 def workload_config(name, scale, n, m, nnz, steps):
@@ -115,7 +120,7 @@ def workload_config(name, scale, n, m, nnz, steps):
             "settings": "SCS defaults (AA mem 10 / interval 10, adaptive scale, normalize), eps = 0 so exactly K "
                         "iterations run",
             "window": f"ADMM iterations 1..{int(steps)} of a cold-started solve",
-            "l2": "working set (A and A' = 2 x 124 MB at C2, streamed alternately, + vectors) exceeds the 126 MB L2"}
+            "l2": "working set (A and A' = 2 x 124 MB at C2, streamed alternately, + vectors) exceeds the 50 MB L2"}
 
 
 def build_problem(name, scale, seed):
@@ -203,9 +208,9 @@ def run_reference(args, iters, lib, omp_threads, blas_threads=1, dump=None):
 
 def best_reference(args, iters, probe_iters=2, dump=None):
     """The reference with 'all the host threads it can use'. Only accum_by_atrans is parallel in the
-    reference (OpenMP, linsys/scs_matrix.c:174-176); probing on this pool's hosts (profiles/README.md: 1, 8,
-    32, 128 threads) showed 32 threads fastest and all 128 hardware threads 6x SLOWER, so the default is
-    min(32, cores) without probing -- a probe costs minutes at C2 (one reference iteration takes ~10 s).
+    reference (OpenMP, linsys/scs_matrix.c:174-176); probing 1, 8, 32 and 128 threads on a 128-thread host showed
+    32 threads fastest and all 128 hardware threads 6x SLOWER, so the default is min(32, cores) without probing --
+    a probe costs minutes at C2 (one reference iteration takes ~10 s).
     SCS_BENCH_PROBE=1 repeats the probe."""
     d = os.path.join(ROOT, "oracle", "_ref")
     plain, omp = os.path.join(d, "libscsindir_ref.so"), os.path.join(d, "libscsindir_ref_omp.so")
@@ -216,7 +221,7 @@ def best_reference(args, iters, probe_iters=2, dump=None):
         lib, t = (omp, min(32, ncores)) if os.path.exists(omp) else (plain, 1)
         r = run_reference(args, iters, lib, t, 1, dump=dump)
         r["cores"] = t
-        r["probes"] = "not probed (SCS_BENCH_PROBE=1 to probe; earlier probes: profiles/README.md)"
+        r["probes"] = "not probed (SCS_BENCH_PROBE=1 to probe)"
         return r
     cands = [(plain, 1, 1)]
     if os.path.exists(omp):
@@ -239,16 +244,22 @@ def best_reference(args, iters, probe_iters=2, dump=None):
     return r
 
 
-def ncu_traffic(kernel_key):
-    """DRAM bytes per launch (dram__bytes_read.sum + dram__bytes_write.sum) of the named in-loop kernel from the
-    committed `ncu --set full` capture (profiles/spmv_ncu_traffic.json, written from gpurun_out by
-    scripts/ncu_summary.py), or None. ncu cannot run inside a timed bench: this is the one number of the line that is
-    read from a file, and the file names the capture it came from."""
-    p = os.path.join(ROOT, "profiles", "spmv_ncu_traffic.json")
-    try:
-        return float(json.load(open(p))[kernel_key]["dram_bytes_per_launch"])
-    except Exception:
-        return None
+DUMP_BYTES = 64 << 20
+
+
+def dump_outputs(d, arrays, info):
+    """the timed solve's outputs as float64 .npy files; over DUMP_BYTES, a fixed seeded sample of each vector"""
+    os.makedirs(d, exist_ok=True)
+    total = sum(a.nbytes for a in arrays.values())
+    for name, a in arrays.items():
+        if total > DUMP_BYTES:
+            k = max(1, int(a.size * (DUMP_BYTES // 2) / total))
+            idx = np.sort(np.random.default_rng(len(name)).choice(a.size, min(k, a.size), replace=False))
+            np.save(os.path.join(d, f"{name}_index.npy"), idx.astype(np.float64))
+            a = a[idx]
+        np.save(os.path.join(d, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float64))
+    np.save(os.path.join(d, "info.npy"), np.array([info.iter, info.pobj, info.dobj, info.res_pri, info.res_dual,
+                                                   info.gap, info.scale], dtype=np.float64))
 
 
 def rel_err(a, b):
@@ -266,6 +277,7 @@ def main():
     ap.add_argument("--seed", type=int, default=1234)
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-tte", action="store_true", help="skip the time-to-eps solve")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="write x, y, s of the timed solve's last step to DIR/*.npy")
     args = ap.parse_args()
     if args.warmup < 3:
         args.warmup = 3
@@ -321,7 +333,7 @@ def main():
         dist.init_process_group("nccl", device_id=torch.device("cuda", local_rank))
     lib = capi.load()
     if not lib.scs_b200_device_ok():
-        raise RuntimeError("scs_b200: no usable sm_100 device (there is no CPU fallback)")
+        raise RuntimeError("scs_b200: no usable sm_90 device (there is no CPU fallback)")
     if world > 1:
         # row-sharded KKT solve: rank 0 creates the NCCL id, torch.distributed carries it
         idbuf = torch.zeros(128, dtype=torch.uint8, device="cuda")
@@ -390,6 +402,8 @@ def main():
     solve_s = info.solve_time / 1e3
     iters = int(info.iter)
     lib.scs_finish(w)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, {"x": sols[0], "y": sols[1], "s": sols[2]}, info)
 
     # ---- time to the default stopping criterion eps_abs = eps_rel = 1e-4 (second half of BASELINE's metric):
     # a separate full solve so that the K-step timing above is untouched
@@ -477,15 +491,12 @@ def main():
             rows = [{"kernel": names[k], "ms": ms[k], "alg_bytes": by[k], "achieved": by[k] / ms[k] / 1e6,
                      "frac": by[k] / ms[k] / 1e6 / peak} for k in range(5)]
             dom = max(rows[:4], key=lambda r: r["ms"])
-            key = "K1" if dom is rows[0] else ("K2" if dom is rows[1] else None)
             roof = {"bound": "hbm", "achieved": dom["achieved"], "peak": peak, "unit": "GB/s", "frac": dom["frac"],
-                    "traffic": ncu_traffic(key) if (key and args.config == "C2" and args.scale == 1.0) else None,
-                    "traffic_source": "profiles/spmv_ncu_traffic.json (ncu --set full capture of the same kernel)",
                     "kernel": dom["kernel"], "ms_per_launch": dom["ms"], "alg_bytes_per_launch": dom["alg_bytes"],
                     "peak_source": peak_src,
                     "timing": "CUDA events around every launch inside 50 genuine CG iterations on the solver's own "
                               "vectors (rhs = [c; b]); K1 / K2 alternate, so each streams its 124 MB matrix after "
-                              "the other's 124 MB passed through the 126 MB L2",
+                              "the other's 124 MB passed through the 50 MB L2",
                     "share_of_cg_iteration": dom["ms"] / ms[4]}
             extra["roofline_all"] = rows
         if not args.no_cpu_baseline:

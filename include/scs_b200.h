@@ -20,7 +20,7 @@
  *      (include/cones.h:80-90, include/aa.h:66-143, linsys/scs_matrix.h); they are
  *      exported here so the parity tests can compare operator by operator.
  *
- * All compute happens in hand-written sm_100a CUDA kernels; there is no CPU
+ * All compute happens in hand-written sm_90a CUDA kernels; there is no CPU
  * fallback: every entry point fails (NULL / nonzero / SCS_FAILED) when no CUDA
  * device is usable.
  *

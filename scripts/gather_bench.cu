@@ -1,13 +1,13 @@
 // gather_bench.cu -- what does ONE random 8-byte gather cost on B200?  (measurement tool, not product)
 //
 // The SpMV of a uniformly random sparse matrix does exactly one random fp64 gather per nonzero,
-// and that gather -- not the 12 B/nnz matrix stream -- is what bounds it (profiles/README.md).
+// and that gather -- not the 12 B/nnz matrix stream -- is what bounds it (DESIGN.md section 3.1).
 // This binary measures the ceiling: a kernel that does nothing but read a coalesced int32 index
 // stream and gather x[idx] (no shared memory, no row logic), for several load flavours, loads in
 // flight per thread, occupancies and gather-vector sizes. Output: one line per variant with the
 // time for N gathers and the rate in gathers / clock / SM.
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/bin/gather_bench scripts/gather_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/bin/gather_bench scripts/gather_bench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>
@@ -135,7 +135,7 @@ int main(int argc, char **argv) {
   const double ghz = khz / 1e6;
   printf("device %s, %d SMs, %.3f GHz (max), N = %lld gathers per launch\n", prop.name, nsm, ghz, total);
   const long long vec_lens[3] = {1000000LL, 3000000LL, 4096LL};
-  const long long flush_total = 40000000LL;  // 160 MB of int32 > 126 MB L2
+  const long long flush_total = 40000000LL;  // 160 MB of int32 > 50 MB L2
   int *d_idx, *d_flush;
   double *d_x, *d_out;
   CK(cudaMalloc(&d_idx, (size_t)total * 4));

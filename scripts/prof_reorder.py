@@ -1,5 +1,5 @@
 """Experiment: how much does an m-space / n-space REORDERING of the C2 matrix buy the SpMV?
-The SpMV is bound by L2->SM sector traffic (32 B per random 8-byte gather, profiles/README.md); the
+The SpMV is bound by L2->SM sector traffic (32 B per random 8-byte gather, DESIGN.md section 3.1); the
 m-space ordering inside the CG operator is free (tmp = R_y^-1 A p never leaves it), so rows can be
 sorted to make one gather per row sequential. Times the unchanged kernels on permuted copies."""
 import ctypes as C

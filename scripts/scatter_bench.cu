@@ -1,4 +1,4 @@
-// scatter_bench.cu -- what does ONE random fp64 `red.global.add` cost on B200, alone and next to a gather?
+// scatter_bench.cu -- what does ONE random fp64 `red.global.add` cost on H100, alone and next to a gather?
 // (measurement tool, not product; companion of gather_bench.cu)
 //
 // Question (VERDICT r01, next-round item 4-iv): the CG operator G p = R_x p + A' R_y^-1 A p is applied today as
@@ -12,7 +12,7 @@
 //   scatter4  : per row read t, 4 x red.add               (the scatter ceiling)
 //   onepass4  : per row 4 gathers, t = sum/R, 4 x red.add (the fused candidate) + block-reduced dot
 //
-//   nvcc -gencode arch=compute_100a,code=sm_100a -O3 -o scripts/bin/scatter_bench scripts/scatter_bench.cu
+//   nvcc -gencode arch=compute_90a,code=sm_90a -O3 -o scripts/bin/scatter_bench scripts/scatter_bench.cu
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdio.h>

@@ -1,4 +1,4 @@
-"""scs_b200 -- B200-native (sm_100a) ADMM hot path for SCS behind SCS's own C ABI.
+"""scs_b200 -- H100-native (sm_90a) ADMM hot path for SCS behind SCS's own C ABI.
 
 The product is the shared library ``scs_b200/libscs_b200.so`` (C ABI declared in
 ``include/scs_b200.h``). This Python package only holds the ctypes mirror used

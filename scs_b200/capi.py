@@ -1,9 +1,9 @@
 """ctypes mirror of include/scs_b200.h (and of the reference's include/scs.h layout).
 
 This is plumbing for tests/ and bench.py: it loads the in-tree
-``scs_b200/libscs_b200.so`` (hand-written sm_100a kernels behind a C ABI) and
+``scs_b200/libscs_b200.so`` (hand-written sm_90a kernels behind a C ABI) and
 declares argument types for every exported symbol.  There is no fallback: if the
-shared library is missing, or no sm_100 device is usable, calls fail loudly.
+shared library is missing, or no sm_90 device is usable, calls fail loudly.
 
 The same struct classes are used to drive the reference build
 (``oracle/_ref/libscsindir_ref.so``) in the parity tests, because the layouts

@@ -1,10 +1,10 @@
-// common.cuh -- device-side helpers shared by all kernels of the B200 SCS hot path.
+// common.cuh -- device-side helpers shared by all kernels of the SCS hot path.
 //
 // * deterministic block reductions (fixed shuffle tree + fixed smem order)
 // * "last block finishes" grid reductions: every block writes its partial to a
 //   fixed slot, the last block to arrive sums the slots in index order, so a
 //   launch with a fixed grid is bit-reproducible (no fp64 atomics anywhere)
-// * sm_100a TMA 1-D bulk copy + mbarrier wrappers (cp.async.bulk -> SASS UBLKCP)
+// * sm_90a TMA 1-D bulk copy + mbarrier wrappers (cp.async.bulk -> SASS UBLKCP)
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>
@@ -129,7 +129,7 @@ __device__ __forceinline__ bool grid_finish(double (&mine)[NV], double *partials
   return true;
 }
 
-// ---------------------------------------------------------------- TMA / mbarrier (sm_100a)
+// ---------------------------------------------------------------- TMA / mbarrier (sm_90a)
 __device__ __forceinline__ uint32_t smem_u32(const void *p) {
   return static_cast<uint32_t>(__cvta_generic_to_shared(p));
 }

@@ -1,5 +1,5 @@
 /* dev_api.h -- INTERNAL thin C layer between the C host code (host/ *.c) and the
- * hand-written sm_100a kernels (kernels/ *.cu).  All pointers named d_* are
+ * hand-written sm_90a kernels (kernels/ *.cu).  All pointers named d_* are
  * device pointers; everything is enqueued on the library stream and is
  * asynchronous unless stated otherwise.  Return value: 0 ok, <0 error
  * (message via b200_last_error()). */
@@ -65,7 +65,7 @@ double b200_spmv_alg_bytes(const B200Spmv *M, int extra_row_vectors);
 enum { B200_POST_NONE = 0, B200_POST_DIV = 1, B200_POST_FMA_DOT = 2, B200_POST_FMA = 3, B200_POST_MUL = 4 };
 /* B200_POST_MUL: y = s * d[r] with d = R_y^-1 precomputed -- what the reference's own GPU backend does
  * (linsys/gpu/indirect/private.c:78,164: inv_r_y, scale_by_diag); used by K1 inside the CG loop, where the fp64
- * division chain of POST_DIV held the warps out of the gather pipeline (profiles/README.md, round 2). */
+ * division chain of POST_DIV holds the warps out of the gather pipeline. */
 enum { B200_HOOK_NONE = 0, B200_HOOK_CG_ALPHA = 1, B200_HOOK_P2P_SIGNAL = 2, B200_HOOK_P2P_ROUTE = 3 };
 /* B200_HOOK_P2P_SIGNAL: when the LAST block of the launch has stored its rows, it publishes
  * hook_val into slot `rank` of every peer's flag line (d_hook_arg -> B200P2pSignal). */

@@ -375,8 +375,8 @@ static int build_both_ops(int m, int n, const int *Ap, const int *Ai, const doub
 /* The reordered pair used inside the CG operator (kernels/spmv.cu "Reordered copies"): built once, values and R_y
  * refreshed whenever the resident operators may have been rescaled (b200_linsys_update_diag_r_dev). */
 static int cg_ops_build(ScsLinSysWork *w) {
-  /* OFF by default: measured on C2 (profiles/README.md, round 2 call C) the reordered pair makes K2 1.6 us faster
-   * (62.1 -> 60.5 us) but K1 25 us SLOWER (64.9 -> 90.1 us); SCS_B200_REORDER=1 enables it for experiments */
+  /* OFF by default: on C2 the reordered pair makes K2 slightly faster but K1 much slower (the sort piles the empty
+   * and the longest rows onto a few CTAs, DESIGN.md section 3.1); SCS_B200_REORDER=1 enables it for experiments */
   const char *e = getenv("SCS_B200_REORDER");
   if (w->nranks > 1 || !(e && atoi(e) != 0)) return 0;
   if (!b200_spmv_can_route(w->A) || !b200_spmv_can_route(w->At)) return 0; /* one-pass flagged streams only */
@@ -405,7 +405,7 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
   double *Lx = NULL;
   const int n = A->n, m = A->m;
   if (b200_runtime_init() != 0) {
-    fprintf(stderr, "scs_b200: no usable sm_100 device: %s\n", b200_last_error());
+    fprintf(stderr, "scs_b200: no usable sm_90 device: %s\n", b200_last_error());
     return SCS_NULL;
   }
   w = (ScsLinSysWork *)calloc(1, sizeof(ScsLinSysWork));

@@ -1,4 +1,4 @@
-/* linsys_b200.h -- private definition of struct SCS_LIN_SYS_WORK for the B200
+/* linsys_b200.h -- private definition of struct SCS_LIN_SYS_WORK for this
  * backend (the reference keeps one such private.h per backend, e.g.
  * linsys/cpu/indirect/private.h:16-31). */
 #ifndef LINSYS_B200_H

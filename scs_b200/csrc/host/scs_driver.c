@@ -3,7 +3,7 @@
  * DEVICE-RESIDENT ADMM loop.
  *
  * Host C orchestrates; every O(n+m) or O(nnz) operation of the iteration is a
- * hand-written sm_100a kernel (kernels/ *.cu) reached through the thin C layer
+ * hand-written sm_90a kernel (kernels/ *.cu) reached through the thin C layer
  * of dev_api.h / admm_api.h.  The host sees only scalars (CG flags every
  * iteration, 18 residual scalars every CONVERGED_INTERVAL iterations) and the
  * solution vectors once at the end.
@@ -331,7 +331,7 @@ static void print_header(const ScsWork *w) {
   const ScsCone *k = w->k;
   int i;
   for (i = 0; i < 78; ++i) printf("-");
-  printf("\n\t       SCS hot path on B200 (scs_b200 %s, API of SCS 3.2.11)\n", SCS_VERSION_STR);
+  printf("\n\t       SCS hot path on H100 (scs_b200 %s, API of SCS 3.2.11)\n", SCS_VERSION_STR);
   for (i = 0; i < 78; ++i) printf("-");
   printf("\nproblem:  variables n: %i, constraints m: %i\n", w->n, w->m);
   printf("cones: \t  z: %i, l: %i, b: %i, q: %i cones, s: %i cones, exp: %i + %i dual, pow: %i\n", k->z, k->l,
@@ -362,7 +362,7 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
     return SCS_NULL;
   }
   if (b200_runtime_init() != 0) {
-    printf("ERROR: scs_b200 needs an sm_100 (B200) CUDA device: %s\n", b200_last_error());
+    printf("ERROR: scs_b200 needs an sm_90 (H100) CUDA device: %s\n", b200_last_error());
     return SCS_NULL;
   }
   if (stgs->write_data_filename) { /* reference scs.c:1270-1273 */

@@ -888,8 +888,8 @@ static int mat_vec(B200Cg *cg, const double *d_x, double *d_y, int with_dot, con
   return b200_spmv(At, &a);
 }
 
-// sharded-x push mode (see k_cgx_iteration): -1 = read SCS_B200_SHARD_X once (default ON since its hardware runs at 2
-// and 4 GPUs, profiles/README.md "multi-GPU"; =0 selects the replicated modes), 0 = off, 1 = on
+// sharded-x push mode (see k_cgx_iteration): -1 = read SCS_B200_SHARD_X once (default ON; =0 selects the replicated
+// modes), 0 = off, 1 = on
 static int g_shard_x = -1;
 extern "C" void scs_b200_set_shard_x(int on) { g_shard_x = on ? 1 : 0; }
 static int shard_x_active(const B200Cg *cg) {

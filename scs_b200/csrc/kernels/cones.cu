@@ -335,7 +335,7 @@ k_psd_reconstruct(int k, int count, const int *__restrict__ off, const double *_
   }
 }
 // Same contraction on the fp64 TENSOR-CORE path: mma.sync.aligned.m8n8k4.row.col.f64 (DMMA; SASS "DMMA").
-// tcgen05 has no fp64 MMA kind, so this is the tensor pipe an fp64 contraction at 1e-13 parity can use on sm_100a
+// wgmma has no fp64 kind, so this is the tensor pipe an fp64 contraction at 1e-13 parity can use on sm_90a
 // (north_star: "tensor-core GEMM for the dense Z+ Z+' contraction", reference cones.c:1058-1062 dsyrk).
 // CTA = 4 warps = one 32x32 output tile (ti >= tj) of one block; warp w owns the 16x16 quadrant (w >> 1, w & 1)
 // = 2 x 2 mma tiles. Fragments (PTX ISA, m8n8k4 .f64): A[g][t], B[t][g], C[g][2t], C[g][2t+1] with g = lane >> 2,

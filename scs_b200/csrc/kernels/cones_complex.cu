@@ -1,8 +1,8 @@
 // cones_complex.cu -- projection onto the complex (Hermitian) PSD cone, batched by order.
 //
 // Replaces reference src/cones.c:1072-1156 (proj_complex_semi_definite_cone: zheevr + zherk per block).
-// First hardware run: round 2 (profiles/r02a_first_call.log: operator parity vs the reference's zheevr projection
-// <= 5e-13); enabled by default since. The index arithmetic is also checked on the CPU against the reference
+// Operator parity vs the reference's zheevr projection <= 5e-13 (tests/test_zz_reference_fixtures_gpu.py); enabled by
+// default. The index arithmetic is also checked on the CPU against the reference
 // (numpy restatement in tests/test_complex_psd_cpu.py, <= 3e-14).
 //
 // Vectorisation (docs/src/api/cones.rst, cones.c:1095-1103): a block of order k occupies k^2 doubles;

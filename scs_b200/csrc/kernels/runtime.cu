@@ -57,8 +57,8 @@ extern "C" int b200_runtime_init(void) {
   CUDA_OK(cudaSetDevice(g_dev));
   cudaDeviceProp prop;
   CUDA_OK(cudaGetDeviceProperties(&prop, g_dev));
-  if (prop.major != 10) {
-    snprintf(g_err, sizeof(g_err), "device %d is sm_%d%d; this library is built for sm_100a only",
+  if (prop.major != 9 || prop.minor != 0) {
+    snprintf(g_err, sizeof(g_err), "device %d is sm_%d%d; this library is built for sm_90a only",
              g_dev, prop.major, prop.minor);
     return -1;
   }

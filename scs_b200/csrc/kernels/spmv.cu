@@ -1,10 +1,10 @@
-// spmv.cu -- fp64 / int32 sparse mat-vec for the SCS indirect KKT solve, sm_100a.
+// spmv.cu -- fp64 / int32 sparse mat-vec for the SCS indirect KKT solve, sm_90a.
 //
 // Replaces reference linsys/scs_matrix.c:161-186 (accum_by_atrans, used for both
 // A'x on the CSC arrays and A x on the explicit transpose) and the cuSPARSE
 // calls of linsys/gpu/gpu.c:3-58.
 //
-// Two kernels (history and sweeps: profiles/README.md):
+// Two kernels:
 //   * v3 "flagged stream" (spmv_flag_kernel, the default): nonzero-per-lane on a TMA ring, rows recovered from
 //     END flags with ballots and a segmented warp scan -- see the block comment above the kernel. Rows longer
 //     than a warp-tile are cut into "virtual rows" whose partial sums a second, tiny pass adds in order
@@ -30,7 +30,7 @@
 
 extern "C" int b200_host_threads(long long work_items);  // host/linsys_b200.c
 
-// tuning knobs (overridable with -D for sweeps; see profiles/README.md for the measurements)
+// tuning knobs (overridable with -D for sweeps)
 #ifndef SPMV_DEFAULT_VERSION
 #define SPMV_DEFAULT_VERSION 3  // flagged stream (SCS_B200_SPMV=2 forces the warp-specialised row-per-lane kernel)
 #endif
@@ -122,9 +122,9 @@ __device__ __forceinline__ double spmv_epilogue(double s, int row, double *__res
 // independent loads in flight per thread, and adds the products in storage order (bit-identical
 // to the sequential CPU loop).  Stages are handed over with full/empty mbarriers only -- there
 // is no __syncthreads in the main loop, so a fast warp runs ahead into the next tile.
-// defaults from the sweep in profiles/README.md (C2, B200): 512 threads (1 producer + 15 consumer
-// warps), 1536-entry tiles, 3 stages, 2 CTAs/SM = 148 kB of shared memory per SM, which leaves
-// ~80 kB of L1 for the gathers (bigger tiles / more stages shrink L1 and lose more than they gain)
+// defaults: 512 threads (1 producer + 15 consumer warps), 1536-entry tiles, 3 stages, 2 CTAs/SM =
+// 148 kB of shared memory per SM, which leaves ~100 kB of the H100's 256 kB L1/shared array for the
+// gathers (bigger tiles / more stages shrink L1, which the random gathers need)
 #ifndef SPMV2_THREADS
 #define SPMV2_THREADS 512
 #endif
@@ -366,8 +366,8 @@ spmv_ws_kernel(const int *__restrict__ rowptr, const int *__restrict__ colidx,
 //     return, so the ring runs ahead of the gather latency.
 // Rows longer than SPMV3_MAXROW entries do not fit a warp-tile: such operators keep the plain
 // CSR and the v2 kernel.
-// defaults from the sweep in profiles/README.md (C2, B200): ONE CTA of 768 threads per SM (1 producer
-// + 23 consumer warps), 3 stages = 130 kB of shared memory, which leaves ~98 kB of L1 to the gathers
+// defaults: ONE CTA of 768 threads per SM (1 producer + 23 consumer warps), 3 stages = 130 kB of shared
+// memory (within the H100's 227 kB per block), which leaves ~125 kB of the 256 kB L1/shared array to the gathers
 #ifndef SPMV3_THREADS
 #define SPMV3_THREADS 768
 #endif
@@ -1031,12 +1031,12 @@ extern "C" B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr,
     const char *g = getenv("SCS_B200_SPMV_GRID");  // tests: force many groups per CTA on small matrices
     if (g && atoi(g) > 0 && atoi(g) < cap) cap = atoi(g);
     // operators with very short rows (avg below SCS_B200_SPMV_MINAVG, default 0 = never) can be sent to
-    // the row-per-lane kernel instead (tuning knob, see profiles/README.md)
+    // the row-per-lane kernel instead (tuning knob)
     const char *ma = getenv("SCS_B200_SPMV_MINAVG");
     const bool too_short = ma && nrows > 0 && (double)nnz / nrows < atof(ma);
     Spmv3Plan P;
     // rows longer than a warp-tile: virtual rows + combine pass (SCS_B200_SPMV_LONGROWS=0 sends such operators
-    // to the v2 kernel instead; first hardware run: profiles/r02a_first_call.log)
+    // to the v2 kernel instead)
     const char *lr = getenv("SCS_B200_SPMV_LONGROWS");
     const bool split_long = !(lr && atoi(lr) == 0);
     if (nrows > 0 && !too_short && spmv3_build_plan(nrows, ncols, h_rowptr, h_colidx, h_vals, cap, P, split_long)) {
@@ -1101,8 +1101,8 @@ extern "C" B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr,
     if (M->version == 2) {
       // v2: lg 0/1/2 = 1/2/4 lanes per row with ORDERED combine (bit-exact), 5 = warp per row (tree)
       const int nr = r1 - r, cons = SPMV2_NCW * 32;
-      // measured on C2 (profiles/README.md): sharing a 10-entry row between 2 lanes costs 7 %
-      // (65.1 vs 60.6 us), so the ordered multi-lane mode is off unless asked for
+      // sharing a 10-entry row between 2 lanes was slower on C2, so the ordered multi-lane mode is off unless
+      // asked for
       lgv = 0;
       if (mx > 64) lgv = 5;
 #ifdef SPMV2_ORDERED_LANES
@@ -1357,7 +1357,7 @@ extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, c
 }
 
 // ---------------------------------------------------------------------------------------------
-// Reordered copies for the CG operator (VERDICT r01 item 4-ii; measurements: profiles/README.md "reordering").
+// Reordered copies for the CG operator (off by default, DESIGN.md section 3.1 "Reordering").
 // The m-space ordering INSIDE G = R_x + A' R_y^-1 A is free (tmp = R_y^-1 A p never leaves the operator), so the rows
 // of A can be sorted by their smallest column index: one gather per row of K1 becomes sequential, and the matching
 // entries of every column of A' become adjacent for K2.

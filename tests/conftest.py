@@ -31,8 +31,8 @@ def pytest_sessionstart(session):
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a real B200 (run with -m gpu on the GPU box)")
-    config.addinivalue_line("markers", "gpu_unverified: needs a real B200 and has NOT been run on one yet; promote to `gpu` "
+    config.addinivalue_line("markers", "gpu: needs a real H100 (run with -m gpu)")
+    config.addinivalue_line("markers", "gpu_unverified: needs a real H100 and has NOT been run on one yet; promote to `gpu` "
                             "after the first green run (none at present: round 1's were promoted in round 2)")
 
 
@@ -44,8 +44,12 @@ def lib():
 
 @pytest.fixture(scope="session")
 def reflib():
-    """The UNMODIFIED reference CPU-indirect build (oracle/_ref). Checker only."""
-    from scs_b200 import capi
-    if not os.path.exists(REF_LIB):
-        pytest.skip("oracle/_ref not built (run `make -C oracle ref` where /root/reference exists)")
-    return capi.load_reference(REF_LIB)
+    """The UNMODIFIED reference CPU-indirect build: its answers recorded under tests/golden/reference/ (see
+    tests/reference_replay.py; SCS_RECORD_REFERENCE=<dir> records them anew from oracle/_ref). Checker only."""
+    import reference_replay
+    return reference_replay.Reference("ref")
+
+
+def pytest_sessionfinish(session, exitstatus):
+    import reference_replay
+    reference_replay.SESSION.save()

@@ -1,6 +1,6 @@
 """CPU tests (no GPU): the C-ABI library loads and exports every symbol that
 include/scs_b200.h declares; struct layouts match the reference's; the library
-fails loudly (no CPU fallback) when there is no sm_100 device."""
+fails loudly (no CPU fallback) when there is no sm_90 device."""
 import ctypes as C
 import os
 import re

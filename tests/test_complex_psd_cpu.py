@@ -1,17 +1,15 @@
 """CPU: the index arithmetic of the complex-PSD kernels (scs_b200/csrc/kernels/cones_complex.cu:
 k_cpsd_unpack / k_cpsd_reconstruct -- packed Hermitian block <-> real embedding [[A, -B], [B, A]] of order 2k),
 restated in numpy line by line and checked against the reference's zheevr-based projection
-(oracle/_ref: src/cones.c:1072-1156 through _scs_proj_dual_cone)."""
+(src/cones.c:1072-1156 through _scs_proj_dual_cone; its answer recorded under tests/golden/reference/)."""
 import ctypes as C
-import os
 
 import numpy as np
 import pytest
 
-from conftest import REF_LIB
 from scs_b200 import capi
+import reference_replay
 
-pytestmark = pytest.mark.skipif(not os.path.exists(REF_LIB), reason="oracle/_ref not built")
 SQRT2 = 1.4142135623730951
 
 
@@ -68,6 +66,12 @@ def reference_projection(reflib, orders, x):
     assert reflib._scs_proj_dual_cone(capi.dptr(v), cw, None, None) == 0
     reflib._scs_finish_cone(cw)
     return v + x        # Pi_K(x) = Pi_K*(-x) + x  (the cone is self-dual)
+
+
+@pytest.fixture(scope="module")
+def reflib():
+    """the reference's answers stored whole: every block of the projection is compared"""
+    return reference_replay.Reference("ref", whole=True)
 
 
 def test_embedding_reproduces_the_reference(reflib):

@@ -13,8 +13,8 @@ from conftest import ROOT, REF_LIB
 from scs_b200 import capi
 
 HOST_LIB = os.path.join(ROOT, "oracle", "libtriples_host.so")
-pytestmark = pytest.mark.skipif(not (os.path.exists(HOST_LIB) and os.path.exists(REF_LIB)),
-                                reason="oracle/libtriples_host.so or oracle/_ref not built")
+pytestmark = pytest.mark.skipif(not os.path.exists(HOST_LIB), reason="oracle/libtriples_host.so not built")
+needs_reference = pytest.mark.skipif(not os.path.exists(REF_LIB), reason="oracle/_ref not built")
 
 
 def triples(rng, n):
@@ -27,6 +27,7 @@ def triples(rng, n):
     return x
 
 
+@needs_reference
 def test_exp_cone_host_restatement_matches_reference():
     host = C.CDLL(HOST_LIB)
     host.b200_triples_host_exp.argtypes = [capi.c_double_p, C.c_int]
@@ -44,6 +45,7 @@ def test_exp_cone_host_restatement_matches_reference():
     assert worst <= 1e-13, worst
 
 
+@needs_reference
 def test_power_cone_host_restatement_matches_reference():
     host = C.CDLL(HOST_LIB)
     host.b200_triples_host_pow.argtypes = [capi.c_double_p, C.c_double]

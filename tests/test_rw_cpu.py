@@ -14,6 +14,12 @@ pytestmark = pytest.mark.skipif(not os.path.exists(REF_LIB), reason="oracle/_ref
 PP = C.POINTER
 
 
+@pytest.fixture(scope="module")
+def reflib():
+    """the reference build itself: files are compared byte for byte and its reader allocates the problem"""
+    return capi.load_reference(REF_LIB)
+
+
 def bind(lib, read, write, free=None):
     r, w = getattr(lib, read), getattr(lib, write)
     r.restype = C.c_int

@@ -1,12 +1,13 @@
 """Whole-solver parity on the GPU: the device-resident scs_init/scs_solve/
-scs_finish against the reference CPU-indirect solver (oracle/_ref) on the same
-problems, plus the known optimum the generator builds in."""
+scs_finish against the reference CPU-indirect solver (its answers recorded under
+tests/golden/reference/) on the same problems, plus the known optimum the generator builds in."""
 import ctypes as C
 
 import numpy as np
 import pytest
 
 from scs_b200 import capi, problems
+from reference_replay import rel
 
 pytestmark = pytest.mark.gpu
 
@@ -87,7 +88,7 @@ def test_one_iteration_matches_reference(lib, reflib, kind):
     assert st_m == st_r and info_m.iter == info_r.iter == 1
     errs = {}
     for a, b, nm in ((x, xr, "x"), (y, yr, "y"), (s, sr, "s")):
-        errs[nm] = np.abs(a - b).max() / max(1.0, np.abs(b).max())
+        errs[nm] = rel(a, b)
     for fld in ("pobj", "dobj", "res_pri", "res_dual", "gap"):
         a, b = getattr(info_m, fld), getattr(info_r, fld)
         errs[fld] = abs(a - b) / max(1.0, abs(b))
@@ -121,7 +122,7 @@ def test_qp_matches_reference(lib, reflib):
     st_r, info_r, xr, yr, sr = solve_with(reflib, prob, max_iters=1)
     assert st_m == st_r and info_m.iter == info_r.iter == 1
     for a, b, nm in ((x, xr, "x"), (y, yr, "y"), (s, sr, "s")):
-        err = np.abs(a - b).max() / max(1.0, np.abs(b).max())
+        err = rel(a, b)
         assert err <= 1e-10, (nm, err)
     for fld in ("pobj", "dobj", "res_pri", "res_dual", "gap"):
         a, b = getattr(info_m, fld), getattr(info_r, fld)
@@ -132,7 +133,7 @@ def test_qp_matches_reference(lib, reflib):
     print(f"\n[qp] mine it={info_m.iter} pobj={info_m.pobj:.10e} | ref it={info_r.iter} pobj={info_r.pobj:.10e}")
     assert st_m == st_r == 1
     assert abs(info_m.pobj - info_r.pobj) <= 100 * eps * max(1.0, abs(info_r.pobj))
-    assert np.abs(x - xr).max() <= 1e-4 * max(1.0, np.abs(xr).max())   # strictly convex in x: unique minimiser
+    assert rel(x, xr) <= 1e-4   # strictly convex in x: unique minimiser
 
 
 def exp_pow_problem(seed, n=60):
@@ -197,7 +198,7 @@ def test_exp_and_power_cones_match_reference(lib, reflib):
     st_r, info_r, xr, yr, sr = solve_with(reflib, prob, max_iters=1)
     assert st_m == st_r and info_m.iter == info_r.iter == 1
     for a, b, nm in ((x, xr, "x"), (y, yr, "y"), (s, sr, "s")):
-        err = np.abs(a - b).max() / max(1.0, np.abs(b).max())
+        err = rel(a, b)
         assert err <= 1e-9, (nm, err)
     eps = 1e-6
     st_m, info_m, x, y, s = solve_with(lib, prob, eps_abs=eps, eps_rel=eps, max_iters=50000)
@@ -285,7 +286,7 @@ def test_complex_psd_cone_matches_reference(lib, reflib):
     st_r, info_r, xr, yr, sr = solve_with(reflib, prob, max_iters=1)
     assert st_m == st_r and info_m.iter == info_r.iter == 1
     for a, b, nm in ((x, xr, "x"), (yy, yr, "y"), (s, sr, "s")):
-        err = np.abs(a - b).max() / max(1.0, np.abs(b).max())
+        err = rel(a, b)
         assert err <= 1e-10, (nm, err)
     eps = 1e-7
     st_m, info_m, x, yy, s = solve_with(lib, prob, eps_abs=eps, eps_rel=eps, max_iters=50000)
@@ -310,6 +311,7 @@ def test_csv_trace_matches_reference(lib, reflib, tmp_path):
     over = dict(max_iters=30, acceleration_lookback=0, eps_abs=1e-12, eps_rel=1e-12)
     st_m, info_m, *_ = solve_with(lib, prob, log_csv_filename=mine.encode(), **over)
     st_r, info_r, *_ = solve_with(reflib, prob, log_csv_filename=ref.encode(), **over)
+    reflib.written_file(ref)
     assert st_m == st_r
     hm, rm = csv_trace_diff.read(mine)
     hr, rr = csv_trace_diff.read(ref)

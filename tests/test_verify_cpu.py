@@ -1,12 +1,20 @@
 """CPU: tests/verify.py (numpy restatement of the reference's verify_solution_correct,
-/root/reference/test/problem_utils.h:107-249) accepts what the UNMODIFIED reference produces -- solved,
+test/problem_utils.h:107-249) accepts what the UNMODIFIED reference produces (recorded under tests/golden/reference/) -- solved,
 infeasible and unbounded outcomes -- and rejects a corrupted solution. Pins the checker the GPU tests use."""
 import ctypes as C
 
 import numpy as np
+import pytest
 
 from scs_b200 import capi, problems
+import reference_replay
 import verify
+
+
+@pytest.fixture(scope="module")
+def reflib():
+    """the reference's answers stored whole: the checker reads every entry of the solution"""
+    return reference_replay.Reference("ref", whole=True)
 
 
 def ref_solve(reflib, prob, **over):

@@ -1,29 +1,25 @@
-"""The reference's own binary fixtures (test/problems/{random_prob, max_ent, mpc_bug1..3}; known optima in
-random_prob.h:6, max_ent.h:6, mpc_bug.h:7-9) read with scs_b200_read_data and solved by the device-resident
+"""The reference's own binary fixtures (test/problems/{random_prob, mpc_bug1..3}, copied to tests/golden/problems/;
+known optima in random_prob.h:6, mpc_bug.h:7-9) read with scs_b200_read_data and solved by the device-resident
 driver, checked the way the reference checks them (test/problems/test_prob_from_data_file.h:31-60:
 eps 1e-6, status solved, primal and dual objective within 1e-4 of the known optimum).
 
 random_prob exercises every supported cone at once (zero, LP, SOC incl. sizes 0 and 1, PSD incl. orders 0 and
-1, primal/dual exponential, primal/dual power); max_ent has 450 exponential cones; mpc_bug1..3 are QPs.
-
-First green run on a B200: round 2, gpurun call A (profiles/r02a_first_call.log): 11 passed -- promoted from
-`gpu_unverified` to `gpu` (the file reader itself is verified on the CPU against the reference's reader in
-tests/test_rw_cpu.py)."""
+1, primal/dual exponential, primal/dual power); mpc_bug1..3 are QPs. (The file reader itself is verified on the CPU
+against the reference's reader in tests/test_rw_cpu.py.)"""
 import ctypes as C
 import os
 
 import numpy as np
 import pytest
 
-from conftest import REF_DIR
 from scs_b200 import capi
+from reference_replay import rel
 
 pytestmark = pytest.mark.gpu
 PP = C.POINTER
 
 FIXTURES = {
     "random_prob": 5.751458006385587,
-    "max_ent": -6.067087663361563,
     "mpc_bug1": -0.473957794500,
     "mpc_bug2": -0.029336830816,
     "mpc_bug3": -0.002215217478,
@@ -32,9 +28,7 @@ FIXTURES = {
 
 @pytest.mark.parametrize("name", sorted(FIXTURES))
 def test_reference_fixture_known_optimum(lib, name):
-    path = os.path.join(REF_DIR, "test", "problems", name)
-    if not os.path.exists(path):
-        pytest.skip("fixture not present (oracle/Makefile copies it where /root/reference exists)")
+    path = os.path.join(os.path.dirname(os.path.abspath(__file__)), "golden", "problems", name)
     lib.scs_b200_read_data.restype = C.c_int
     lib.scs_b200_read_data.argtypes = [C.c_char_p, PP(PP(capi.ScsData)), PP(PP(capi.ScsCone)), PP(PP(capi.ScsSettings))]
     lib.scs_b200_free_data.argtypes = [PP(capi.ScsData), PP(capi.ScsCone), PP(capi.ScsSettings)]
@@ -112,7 +106,7 @@ def test_complex_psd_operator_matches_reference(lib, reflib, monkeypatch):
             out = x.copy()
             assert lib.scs_b200_proj_dual_cone(mw, capi.dptr(out), capi.dptr(None if ry is None else ry.copy())) == 0
             lib.scs_b200_finish_cone(mw)
-            err = np.abs(out - ref).max() / max(np.abs(ref).max(), 1.0)
+            err = rel(out, ref)
             assert err <= (1e-8 if cone.get("p") else 5e-13), (cone, err)
 
 
@@ -167,17 +161,17 @@ def test_long_row_mode_matches_reference(lib, reflib, monkeypatch):
             mine, ref = np.zeros(m), np.zeros(m)
             assert lib.scs_b200_accum_by_a(w, capi.dptr(x), capi.dptr(mine), 0) == 0
             reflib._scs_accum_by_a(C.byref(hp.A), capi.dptr(x), capi.dptr(ref))
-            assert np.abs(mine - ref).max() / np.abs(ref).max() <= 1e-13
+            assert rel(mine, ref, 0.0) <= 1e-13
             mine, ref = np.ones(n), np.ones(n)
             assert lib.scs_b200_accum_by_atrans(w, capi.dptr(yv), capi.dptr(mine), 1) == 0
             reflib._scs_accum_by_atrans(C.byref(hp.A), capi.dptr(yv), capi.dptr(ref))
-            assert np.abs(mine - ref).max() / np.abs(ref).max() <= 1e-13
+            assert rel(mine, ref, 0.0) <= 1e-13
             rhs = rng.standard_normal(n + m)
             wr = reflib.scs_init_lin_sys_work(C.byref(hp.A), None, capi.dptr(dr))
             a, b = rhs.copy(), rhs.copy()
             assert lib.scs_solve_lin_sys(w, capi.dptr(a), None, 1e-12) == 0
             assert reflib.scs_solve_lin_sys(wr, capi.dptr(b), None, 1e-12) == 0
             reflib.scs_free_lin_sys_work(wr)
-            assert np.abs(a - b).max() / np.abs(b).max() <= 1e-10
+            assert rel(a, b, 0.0) <= 1e-10
         finally:
             lib.scs_free_lin_sys_work(w)

@@ -1,5 +1,5 @@
 """numpy restatement of the reference's universal solution checker `verify_solution_correct`
-(/root/reference/test/problem_utils.h:107-249) -- every clause, same tolerances.  Test infrastructure.
+(the reference's test/problem_utils.h:107-249) -- every clause, same tolerances.  Test infrastructure.
 
 All norms are infinity norms (NORM = SCS(norm_inf), problem_utils.h:16).  The cone distances are
 ||s - Pi_K(s)||_inf = ||Pi_K*(-s)||_inf and ||y - Pi_K*(y)||_inf (problem_utils.h:83-105); they are computed with
