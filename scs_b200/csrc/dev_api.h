@@ -56,6 +56,7 @@ int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, cons
 int b200_spmv_nrows(const B200Spmv *M);
 int b200_spmv_ncols(const B200Spmv *M);
 long long b200_spmv_nnz(const B200Spmv *M);
+long long b200_spmv_stored(const B200Spmv *M);     /* entries in the stream: flagged streams add one per empty row */
 const double *b200_spmv_vals(const B200Spmv *M);   /* device */
 const int *b200_spmv_colidx(const B200Spmv *M);    /* device */
 const int *b200_spmv_rowptr(const B200Spmv *M);    /* device */
@@ -106,7 +107,7 @@ typedef struct {
 } B200SpmvArgs;
 
 /* reordered copies for the CG operator (kernels/spmv.cu, kernels/setup.cu): rows of A by smallest column index */
-B200Spmv *b200_spmv_permuted_rows(const B200Spmv *M, const int *d_perm /* new -> old */);
+B200Spmv *b200_spmv_permuted_rows(const B200Spmv *M, const int *d_perm /* new -> old */, int nrows /* kept: perm[0..nrows) */);
 int b200_spmv_refresh_permuted(B200Spmv *Mp, const B200Spmv *M, const int *d_perm); /* values only */
 B200Spmv *b200_spmv_renumbered_cols(const B200Spmv *M, const int *d_inv /* old -> new */); /* view: borrows M's arrays */
 int b200_perm_rows_by_min_col(const B200Spmv *A, int *d_perm, int *d_inv);
@@ -135,8 +136,8 @@ typedef struct {
   const B200Spmv *A;   /* CSR of A  (m x n): rows of A   -> used for z = A p      */
   const B200Spmv *At;  /* CSR of A' (n x m): cols of A   -> used for y = A' z     */
   const B200Spmv *P;   /* full symmetric P as CSR (n x n) or NULL                 */
-  /* optional m-space-reordered pair used ONLY inside mat_vec (tmp lives in the permuted order): A_cg = rows of A
-   * sorted by smallest column, At_cg = A' with its column indices renumbered, d_ry_cg = R_y in that order */
+  /* m-space-reordered pair used ONLY inside mat_vec when set (tmp lives in the permuted order): A_cg = the non-empty
+   * rows of A sorted by smallest column, At_cg = A' with its column indices renumbered, d_ry_cg = R_y in that order */
   const B200Spmv *A_cg, *At_cg;
   const double *d_ry_cg;
   const double *d_rx;  /* R_x (n) */

@@ -372,20 +372,28 @@ static int build_both_ops(int m, int n, const int *Ap, const int *Ai, const doub
   return *A_out ? 0 : -1;
 }
 
-/* The reordered pair used inside the CG operator (kernels/spmv.cu "Reordered copies"): built once, values and R_y
- * refreshed whenever the resident operators may have been rescaled (b200_linsys_update_diag_r_dev). */
+/* The reordered pair used inside the CG operator (kernels/spmv.cu "Reordered copies", DESIGN.md section 3.1): the rows
+ * of A sorted by their smallest column make one gather per row of K1 and of K2 sequential, and every row keeps the
+ * lane split it has in A, so the pair computes what the plain pair computes. Built once on a single GPU whenever both
+ * operators are one-pass flagged streams (the only form the permuted copy and the renumbered view are built for);
+ * other inputs keep the plain pair. Values and R_y are refreshed whenever the resident operators may have been
+ * rescaled (b200_linsys_update_diag_r_dev). */
 static int cg_ops_build(ScsLinSysWork *w) {
-  /* OFF by default: on C2 the reordered pair makes K2 slightly faster but K1 much slower (the sort piles the empty
-   * and the longest rows onto a few CTAs, DESIGN.md section 3.1); SCS_B200_REORDER=1 enables it for experiments */
-  const char *e = getenv("SCS_B200_REORDER");
-  if (w->nranks > 1 || !(e && atoi(e) != 0)) return 0;
+  long long empty;
+  int kept;
+  if (w->nranks > 1) return 0;
   if (!b200_spmv_can_route(w->A) || !b200_spmv_can_route(w->At)) return 0; /* one-pass flagged streams only */
+  /* empty rows (one stored SKIP entry each) sort last and no column of A references them: A_cg leaves them out, their
+   * entries of the permuted tmp are never written and never read */
+  empty = b200_spmv_stored(w->A) - b200_spmv_nnz(w->A);
+  kept = w->m - (int)empty;
+  if (kept <= 0) return 0;
   w->d_perm = (int *)b200_malloc((size_t)w->m * 4);
   w->d_inv = (int *)b200_malloc((size_t)w->m * 4);
   w->d_ry_cg = (double *)b200_malloc((size_t)w->m * 8);
   if (!w->d_perm || !w->d_inv || !w->d_ry_cg) return -1;
   if (b200_perm_rows_by_min_col(w->A, w->d_perm, w->d_inv) != 0) return -1;
-  w->A_cg = b200_spmv_permuted_rows(w->A, w->d_perm);
+  w->A_cg = b200_spmv_permuted_rows(w->A, w->d_perm, kept);
   w->At_cg = b200_spmv_renumbered_cols(w->At, w->d_inv);
   if (!w->A_cg || !w->At_cg) return -1;
   w->cg.A_cg = w->A_cg; w->cg.At_cg = w->At_cg; w->cg.d_ry_cg = w->d_ry_cg;

@@ -20,8 +20,9 @@ struct SCS_LIN_SYS_WORK {
   B200Cg cg;
   /* row-sharded mode: this rank owns rows [row0, row0+mloc); offsets has nranks+1 entries */
   int nranks, rank, row0, mloc;
-  /* m-space-reordered pair for the CG operator (single GPU; SCS_B200_REORDER=0 turns it off): A_cg = rows of A by
-   * smallest column index, At_cg = view of At with renumbered columns, d_ry_cg = R_y in that order */
+  /* m-space-reordered pair for the CG operator (single GPU, flagged-stream operators; else NULL): A_cg = the
+   * non-empty rows of A by smallest column index, each with A's lane split, At_cg = view of At with renumbered
+   * columns, d_ry_cg = R_y in that order */
   B200Spmv *A_cg, *At_cg;
   double *d_ry_cg;
   int *d_perm, *d_inv;

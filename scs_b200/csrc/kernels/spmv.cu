@@ -739,7 +739,11 @@ struct Spmv3Plan {
 };
 
 // warp-tiles (whole (virtual) rows whose aligned span (k0 & ~3 .. end) is <= 128 entries) and the static CTA
-// partition, from the stored (virtual) row pointers alone -- shared by the host plan builder and the device one
+// partition, from the stored (virtual) row pointers alone -- shared by every plan builder (host, device, permuted).
+// CTAs own equal counts of warp-tiles. A warp-tile holds up to 128 entries whatever its rows, so this balances the
+// gathers; on the row-sorted CG copy of A it leaves 2.8x more rows on the last CTAs than on the first, but rows are
+// cheap next to gathers: balancing on entries + rows (or 2 entries + rows) was 1.3 % (0.2 %) slower per CG iteration
+// on C2 (H100 SXM, DESIGN.md section 3.1).
 static void spmv3_tiles_from_rowptr(int nv, const int *vrp, long long stored, int grid_cap, Spmv3Plan &P) {
   std::vector<int4> real;
   real.reserve((size_t)(stored / 100 + 16));
@@ -1357,20 +1361,29 @@ extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, c
 }
 
 // ---------------------------------------------------------------------------------------------
-// Reordered copies for the CG operator (off by default, DESIGN.md section 3.1 "Reordering").
+// Reordered copies for the CG operator (DESIGN.md section 3.1 "Reordering").
 // The m-space ordering INSIDE G = R_x + A' R_y^-1 A is free (tmp = R_y^-1 A p never leaves the operator), so the rows
 // of A can be sorted by their smallest column index: one gather per row of K1 becomes sequential, and the matching
 // entries of every column of A' become adjacent for K2.
-//   b200_spmv_permuted_rows : row-permuted copy of a flagged-stream operator (row `new` = row perm[new] of M);
-//                             segments are copied with their flags, the warp-tiles are recomputed;
+//   b200_spmv_permuted_rows : row-permuted copy of the first `nrows` rows of the permutation of a flagged-stream
+//                             operator (row `new` = row perm[new] of M); segments are copied with their flags, the
+//                             warp-tiles are recomputed. Rows left out are never written (the caller leaves out
+//                             empty rows only, so the entry count stays M's). Every row keeps the LANE SPLIT it has
+//                             in M, so that the copy computes bit-for-bit the row sums M computes (see below);
 //   b200_spmv_refresh_permuted : values only (after the resident operators were rescaled in place);
 //   b200_spmv_renumbered_cols  : a VIEW of M whose stored column indices are mapped through inv[] (flags kept);
 //                             row pointers, values and warp-tiles are M's own (borrowed, not copied).
-__global__ void k_perm_len(int nrows, const int *__restrict__ sp, const int *__restrict__ perm, int *__restrict__ out) {
-  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += gridDim.x * blockDim.x) {
-    const int o = perm[r];
-    out[r] = sp[o + 1] - sp[o];
-  }
+//
+// Lane split. The flag kernel sums a row inside one lane sequentially and combines the pieces of a row that spans lanes
+// with a scan whose tree depends only on the pieces (lanes own the entries [4l, 4l+4) of the 16-byte-aligned stream;
+// a leading lane that holds only explicit zeros adds exact zeros). The pieces are set by the position of the row's
+// first entry modulo 4 and its length. The permuted copy therefore places every row so that it is cut into the same
+// pieces as in M: a row that spans lanes in M starts at the same position modulo 4, a row that fits one lane in M fits
+// one lane here. Up to 3 explicit zeros (SKIP, no END) lead a row's segment to get there. With the row sums equal, the
+// CG operator computes what the plain pair computes, only faster.
+__global__ void k_fill_skip(long long count, int *__restrict__ oi) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < count; k += (long long)gridDim.x * blockDim.x)
+    oi[k] = (int)SPMV3_SKIP;
 }
 __global__ void k_perm_copy(int nrows, const int *__restrict__ sp_old, const int *__restrict__ sp_new,
                             const int *__restrict__ perm, const int *__restrict__ ci, const double *__restrict__ va,
@@ -1378,7 +1391,7 @@ __global__ void k_perm_copy(int nrows, const int *__restrict__ sp_old, const int
   for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += gridDim.x * blockDim.x) {
     const int o = perm[r];
     const int a = sp_old[o], len = sp_old[o + 1] - a;
-    const int b = sp_new[r];
+    const int b = sp_new[r + 1] - len;  // the entries close the segment; explicit zeros lead it
     for (int k = 0; k < len; ++k) {
       if (oi != nullptr) oi[b + k] = ci[a + k];
       ov[b + k] = va[a + k];
@@ -1393,41 +1406,52 @@ __global__ void k_renumber_cols(long long stored, const int *__restrict__ ci, co
   }
 }
 
-extern "C" B200Spmv *b200_spmv_permuted_rows(const B200Spmv *S, const int *d_perm) {
-  if (!S || S->version != 3 || S->d_vptr != nullptr) return nullptr;
+extern "C" B200Spmv *b200_spmv_permuted_rows(const B200Spmv *S, const int *d_perm, int nrows) {
+  if (!S || S->version != 3 || S->d_vptr != nullptr || nrows <= 0 || nrows > S->nrows) return nullptr;
   cudaStream_t st = (cudaStream_t)b200_stream();
-  const int nrows = S->nrows;
   B200Spmv *M = (B200Spmv *)calloc(1, sizeof(B200Spmv));
   if (!M) return nullptr;
-  M->nrows = nrows; M->ncols = S->ncols; M->nnz = S->nnz; M->version = 3; M->stored = S->stored; M->nvrows = nrows;
-  const size_t pad = (((size_t)S->stored + 3) & ~(size_t)3) + 8;
-  int *d_len = (int *)b200_malloc((size_t)(nrows + 1) * 4);
+  M->nrows = nrows; M->ncols = S->ncols; M->nnz = S->nnz; M->version = 3; M->nvrows = nrows;
+  // segment layout on the host (sequential, O(rows)): stored row pointers of M and the permutation come back once
+  std::vector<int> h_old((size_t)S->nrows + 1), h_perm((size_t)nrows), h_sp((size_t)nrows + 1);
+  bool ok = b200_d2h(h_old.data(), S->d_rowptr, h_old.size() * 4) == 0 &&
+            b200_d2h(h_perm.data(), d_perm, h_perm.size() * 4) == 0 && b200_sync() == 0;
+  long long pos = 0;
+  for (int r = 0; ok && r < nrows; ++r) {
+    const int a = h_old[(size_t)h_perm[(size_t)r]], len = h_old[(size_t)h_perm[(size_t)r] + 1] - a;
+    const int phase = a & 3, c = (int)(pos & 3);
+    int lead;
+    if (phase + len <= 4) lead = c + len <= 4 ? 0 : 4 - c;  // one lane in M: one lane here
+    else lead = (phase - c) & 3;                              // spans lanes in M: the same first position modulo 4
+    if (c + lead + len > SPMV3_WT) lead = 0;  // a row of more than 121 entries: its warp-tile could not hold the zeros
+    h_sp[(size_t)r] = (int)pos;
+    pos += lead + len;
+  }
+  h_sp[(size_t)nrows] = (int)pos;
+  if (pos > 2000000000LL) ok = false;
+  M->stored = pos;
+  const size_t pad = (((size_t)pos + 3) & ~(size_t)3) + 8;
   M->d_rowptr = (int *)b200_malloc((size_t)(nrows + 1 + 8) * 4);
   M->d_colidx = (int *)b200_malloc(pad * 4);
   M->d_vals = (double *)b200_malloc(pad * 8);
   M->d_partials = (double *)b200_malloc((size_t)B200_MAX_PARTIALS * 8);
   M->d_counter = (unsigned int *)b200_malloc(64);
-  std::vector<int> h_sp((size_t)nrows + 1);
   Spmv3Plan P;
   int g = (nrows + 255) / 256;
   if (g > 16 * b200_num_sms()) g = 16 * b200_num_sms();
-  bool ok = d_len && M->d_rowptr && M->d_colidx && M->d_vals && M->d_partials && M->d_counter;
-  ok = ok && b200_memset0(d_len + nrows, 4) == 0 && b200_memset0(M->d_rowptr, (size_t)(nrows + 1 + 8) * 4) == 0 &&
-       b200_memset0(M->d_colidx, pad * 4) == 0 && b200_memset0(M->d_vals, pad * 8) == 0 &&
-       b200_memset0(M->d_counter, 64) == 0;
+  ok = ok && M->d_rowptr && M->d_colidx && M->d_vals && M->d_partials && M->d_counter;
+  ok = ok && b200_memset0(M->d_rowptr, (size_t)(nrows + 1 + 8) * 4) == 0 && b200_memset0(M->d_vals, pad * 8) == 0 &&
+       b200_memset0(M->d_counter, 64) == 0 && b200_h2d(M->d_rowptr, h_sp.data(), h_sp.size() * 4) == 0;
   if (ok) {
-    k_perm_len<<<g, 256, 0, st>>>(nrows, S->d_rowptr, d_perm, d_len);
-    ok = b200_dev_exclusive_scan_int(d_len, M->d_rowptr, nrows + 1) == 0;
-  }
-  if (ok) {
+    k_fill_skip<<<8 * b200_num_sms(), 256, 0, st>>>((long long)pad, M->d_colidx);
     k_perm_copy<<<g, 256, 0, st>>>(nrows, S->d_rowptr, M->d_rowptr, d_perm, S->d_colidx, S->d_vals, M->d_colidx,
                                    M->d_vals);
     b200_count_launch(2);
-    ok = b200_d2h(h_sp.data(), M->d_rowptr, (size_t)(nrows + 1) * 4) == 0 && b200_sync() == 0;
+    ok = cudaGetLastError() == cudaSuccess;
   }
   if (ok) {
     P.nvrows = nrows;
-    spmv3_tiles_from_rowptr(nrows, h_sp.data(), S->stored, S->grid > 0 ? SPMV3_CTAS_PER_SM * b200_num_sms() : 1, P);
+    spmv3_tiles_from_rowptr(nrows, h_sp.data(), M->stored, S->grid > 0 ? SPMV3_CTAS_PER_SM * b200_num_sms() : 1, P);
     M->grid = P.grid; M->ntiles = P.nwt; M->tile_nnz = SPMV3_WT;
     M->d_wt3 = (int4 *)b200_malloc(P.wt.size() * sizeof(int4));
     M->d_cta_begin3 = (int *)b200_malloc(P.cta_begin.size() * 4);
@@ -1435,7 +1459,6 @@ extern "C" B200Spmv *b200_spmv_permuted_rows(const B200Spmv *S, const int *d_per
          b200_h2d(M->d_cta_begin3, P.cta_begin.data(), P.cta_begin.size() * 4) == 0 && b200_sync() == 0 &&
          cudaGetLastError() == cudaSuccess;
   }
-  b200_free(d_len);
   if (!ok) {
     b200_spmv_destroy(M);
     return nullptr;
