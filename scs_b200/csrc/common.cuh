@@ -13,6 +13,8 @@
 #define B200_RED_THREADS 512  // threads per block of every reduction-carrying vector kernel
 #define B200_MAX_PARTIALS 2048
 // stored column indices carry flags in bits 30/31 (kernels/spmv.cu, flagged stream); every reader masks
+#define B200_FLAG_END 0x80000000u   // last stored entry of its (virtual) row
+#define B200_FLAG_SKIP 0x40000000u  // explicit zero, not gathered: an empty row's one entry, or layout padding
 #define B200_COLMASK 0x3fffffff
 
 #define CUDA_OK(call)                                                        \
@@ -143,6 +145,9 @@ __device__ __forceinline__ void mbar_expect_tx(uint64_t *bar, unsigned bytes) {
   asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)),
                "r"(bytes)
                : "memory");
+}
+__device__ __forceinline__ void mbar_arrive(uint64_t *bar) {
+  asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
 }
 __device__ __forceinline__ void mbar_wait(uint64_t *bar, unsigned parity) {
   asm volatile(

@@ -50,7 +50,7 @@ B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr, const int 
                            const double *h_vals);
 void b200_spmv_destroy(B200Spmv *M);
 /* both resident orientations built ON THE DEVICE from the host CSC of A (kernels/setup.cu): 0 ok, 1 declined (use the
- * host builders: rows longer than a warp-tile, forced v2, SCS_B200_HOST_SETUP=1), < 0 CUDA error */
+ * host builders: SCS_B200_HOST_SETUP=1, an empty A, sizes beyond the device path), < 0 CUDA error */
 int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax, B200Spmv **A_out,
                             B200Spmv **At_out);
 int b200_spmv_nrows(const B200Spmv *M);

@@ -156,7 +156,7 @@ __global__ void k_min_col_key(int nrows, int ncols, const int *__restrict__ sp, 
                               int *__restrict__ key) {
   for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += gridDim.x * blockDim.x) {
     const unsigned v = (unsigned)ci[sp[r]];  // first stored entry of the row: its smallest column (rows are sorted)
-    key[r] = (v & 0x40000000u) ? ncols : (int)(v & 0x3fffffffu);
+    key[r] = (v & B200_FLAG_SKIP) ? ncols : (int)(v & B200_COLMASK);
   }
 }
 __global__ void k_invert_perm(int n, const int *__restrict__ perm, int *__restrict__ inv) {

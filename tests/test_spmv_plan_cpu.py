@@ -213,15 +213,6 @@ def test_plan_and_lane_algorithm(lib, case):
     assert np.abs(y - ref).max() / scale <= 1e-14
 
 
-def test_long_rows_are_refused_when_the_split_is_switched_off(lib, monkeypatch):
-    """SCS_B200_SPMV_LONGROWS=0: an operator with a row longer than a warp-tile gets no v3 plan (-> v2 kernel)"""
-    monkeypatch.setenv("SCS_B200_SPMV_LONGROWS", "0")
-    rng = np.random.default_rng(0)
-    lens = np.array([3, MAXROW + 1, 2])
-    rp, ci, va = random_csr(3, 500, rng, lens)
-    assert build_plan(lib, 3, 500, rp, ci, va, 8) is None
-
-
 @pytest.mark.parametrize("threads", ["1", "3", "8"])
 def test_plan_is_identical_for_any_host_thread_count(lib, threads, monkeypatch):
     """the setup-time passes are split over host threads (disjoint output ranges): same plan for any count"""
@@ -299,11 +290,10 @@ def test_plan_property_random_shapes(lib):
     check()
 
 
-def test_long_rows_as_virtual_rows(lib, monkeypatch):
+def test_long_rows_as_virtual_rows(lib):
     """long-row mode (the default): rows longer than 124 entries are cut into balanced pieces
     (an END flag per piece = one "virtual row"); the lane algorithm produces one sum per virtual row and the combine
     pass (spmv_combine_kernel) adds the pieces of each true row in order."""
-    monkeypatch.delenv("SCS_B200_SPMV_LONGROWS", raising=False)
     lib.b200_spmv3_plan_nvrows.restype = C.c_int
     lib.b200_spmv3_plan_nvrows.argtypes = [C.c_void_p]
     lib.b200_spmv3_plan_vptr.restype = C.POINTER(C.c_int)
@@ -378,11 +368,10 @@ def device_fill_restated(rp, ci, va):
     return np.array(idx, dtype=np.uint32), np.array(vals)
 
 
-def test_device_fill_rule_equals_host_plan_stream(lib, monkeypatch):
+def test_device_fill_rule_equals_host_plan_stream(lib):
     """The device builder (b200_spmv_create_dev) cuts long rows with its own kernel; the rule restated above must give
     exactly the stream of the host plan builder (the hardware test of the real kernel:
     tests/test_linsys_gpu.py::test_device_built_operators_equal_host_built)."""
-    monkeypatch.delenv("SCS_B200_SPMV_LONGROWS", raising=False)
     rng = np.random.default_rng(77)
     for nrows, ncols, sampler in [
         (40, 3000, lambda: rng.choice([0, 1, 3, 124, 125, 200, 248, 249, 373, 700, 1500], 40)),

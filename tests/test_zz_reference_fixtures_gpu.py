@@ -141,10 +141,9 @@ def test_full_size_configs_are_self_consistent(lib, cfg, steps):
     assert np.abs(problems.proj_dual_cone(y, prob["cone"]) - y).max() <= 1e-9 * ymax
 
 
-def test_long_row_mode_matches_reference(lib, reflib, monkeypatch):
+def test_long_row_mode_matches_reference(lib, reflib):
     """v3 long-row mode (virtual rows + combine pass, the default since round 2): both operators and a KKT
     solve on matrices with 700-entry columns and 40-entry rows / very long rows."""
-    monkeypatch.delenv("SCS_B200_SPMV_LONGROWS", raising=False)
     from scs_b200 import problems
     reflib._scs_accum_by_a.argtypes = [PP(capi.ScsMatrix), capi.c_double_p, capi.c_double_p]
     reflib._scs_accum_by_atrans.argtypes = [PP(capi.ScsMatrix), capi.c_double_p, capi.c_double_p]
