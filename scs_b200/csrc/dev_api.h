@@ -107,10 +107,14 @@ typedef struct {
 } B200SpmvArgs;
 
 /* reordered copies for the CG operator (kernels/spmv.cu, kernels/setup.cu): rows of A by smallest column index */
-B200Spmv *b200_spmv_permuted_rows(const B200Spmv *M, const int *d_perm /* new -> old */, int nrows /* kept: perm[0..nrows) */);
+int b200_perm_rows_by_min_col(const B200Spmv *A, int *d_perm /* new -> old */);
+/* d_perm: in sorted, out placed (its first nrows entries, the kept rows, move by less than 32 slots); d_inv: out,
+ * old -> new for all of M's rows */
+B200Spmv *b200_spmv_permuted_rows(const B200Spmv *M, int *d_perm, int *d_inv, int nrows /* kept: perm[0..nrows) */);
 int b200_spmv_refresh_permuted(B200Spmv *Mp, const B200Spmv *M, const int *d_perm); /* values only */
 B200Spmv *b200_spmv_renumbered_cols(const B200Spmv *M, const int *d_inv /* old -> new */); /* view: borrows M's arrays */
-int b200_perm_rows_by_min_col(const B200Spmv *A, int *d_perm, int *d_inv);
+/* host placement behind b200_spmv_permuted_rows (pure host code): returns the copy's stored count */
+long long b200_spmv_place_rows(int nrows, const int *sp_old, int *perm, int *sp_new);
 int b200_gather_vec(int n, const int *d_perm, const double *d_src, double *d_dst); /* dst[i] = src[perm[i]] */
 
 int b200_spmv(const B200Spmv *M, const B200SpmvArgs *a);

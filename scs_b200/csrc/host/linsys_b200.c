@@ -373,8 +373,8 @@ static int build_both_ops(int m, int n, const int *Ap, const int *Ai, const doub
 }
 
 /* The reordered pair used inside the CG operator (kernels/spmv.cu "Reordered copies", DESIGN.md section 3.1): the rows
- * of A sorted by their smallest column make one gather per row of K1 and of K2 sequential, and every row keeps the
- * lane split it has in A, so the pair computes what the plain pair computes. Built once on a single GPU whenever both
+ * of A sorted by their smallest column make one gather per row of K1 and of K2 sequential, and every row is placed
+ * where the kernel sums it as in A, so the pair computes what the plain pair computes. Built once on a single GPU whenever both
  * operators are one-pass flagged streams (the only form the permuted copy and the renumbered view are built for);
  * other inputs keep the plain pair. Values and R_y are refreshed whenever the resident operators may have been
  * rescaled (b200_linsys_update_diag_r_dev). */
@@ -392,10 +392,12 @@ static int cg_ops_build(ScsLinSysWork *w) {
   w->d_inv = (int *)b200_malloc((size_t)w->m * 4);
   w->d_ry_cg = (double *)b200_malloc((size_t)w->m * 8);
   if (!w->d_perm || !w->d_inv || !w->d_ry_cg) return -1;
-  if (b200_perm_rows_by_min_col(w->A, w->d_perm, w->d_inv) != 0) return -1;
-  w->A_cg = b200_spmv_permuted_rows(w->A, w->d_perm, kept);
+  if (b200_perm_rows_by_min_col(w->A, w->d_perm) != 0) return -1;
+  /* the placement reorders the sorted rows slightly: d_perm is final, and d_inv computed from it, only after this */
+  w->A_cg = b200_spmv_permuted_rows(w->A, w->d_perm, w->d_inv, kept);
+  if (!w->A_cg) return -1;
   w->At_cg = b200_spmv_renumbered_cols(w->At, w->d_inv);
-  if (!w->A_cg || !w->At_cg) return -1;
+  if (!w->At_cg) return -1;
   w->cg.A_cg = w->A_cg; w->cg.At_cg = w->At_cg; w->cg.d_ry_cg = w->d_ry_cg;
   return 0;
 }

@@ -151,7 +151,7 @@ extern "C" int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int 
 
 // ---------------------------------------------------------------------------------------------
 // Row order for the CG-internal copy of A: rows by their smallest column index (stable, so equal keys keep the
-// original order; empty rows go last). perm[new] = old row, inv[old] = new row.
+// original order; empty rows go last). perm[new] = old row; b200_spmv_permuted_rows refines the order and inverts it.
 __global__ void k_min_col_key(int nrows, int ncols, const int *__restrict__ sp, const int *__restrict__ ci,
                               int *__restrict__ key) {
   for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += gridDim.x * blockDim.x) {
@@ -159,10 +159,7 @@ __global__ void k_min_col_key(int nrows, int ncols, const int *__restrict__ sp, 
     key[r] = (v & B200_FLAG_SKIP) ? ncols : (int)(v & B200_COLMASK);
   }
 }
-__global__ void k_invert_perm(int n, const int *__restrict__ perm, int *__restrict__ inv) {
-  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) inv[perm[i]] = i;
-}
-extern "C" int b200_perm_rows_by_min_col(const B200Spmv *A, int *d_perm, int *d_inv) {
+extern "C" int b200_perm_rows_by_min_col(const B200Spmv *A, int *d_perm) {
   cudaStream_t st = (cudaStream_t)b200_stream();
   const int nrows = b200_spmv_nrows(A), ncols = b200_spmv_ncols(A);
   int *d_key = (int *)b200_malloc((size_t)nrows * 4), *d_key2 = (int *)b200_malloc((size_t)nrows * 4);
@@ -183,8 +180,7 @@ extern "C" int b200_perm_rows_by_min_col(const B200Spmv *A, int *d_perm, int *d_
     if (!d_tmp) break;
     if (cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_key, d_key2, d_iota, d_perm, nrows, 0, bits, st) != cudaSuccess)
       break;
-    k_invert_perm<<<g, 256, 0, st>>>(nrows, d_perm, d_inv);
-    b200_count_launch(4);
+    b200_count_launch(3);
     if (cudaGetLastError() != cudaSuccess || b200_sync() != 0) break;
     rc = 0;
   } while (0);

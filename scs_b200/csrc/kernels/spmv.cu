@@ -168,6 +168,20 @@ __host__ __device__ __forceinline__ int spmv3_piece_end(int len, int q) {
   return (q + 1) * small + (q + 1 < big ? q + 1 : big);
 }
 
+// The phases (first stored position modulo 4, bit q = phase q) at which the flag kernel sums a row of `len` <= 124
+// entries exactly as it does at `phase`. The kernel cuts a row at phase q into lane pieces of 4 - q, 4, 4, ..., and
+// the remainder, sums each piece sequentially in its lane and joins the pieces with the segmented scan. The result is
+// the plain sequential chain ((p0 + p1) + p2) + ... in two cases only:
+//   * q + len <= 4: one piece, summed in one lane (what is open from the lanes before adds an exact 0);
+//   * q + len == 5: two pieces, the second holds the last entry alone: (chain of the first piece) + p[len-1].
+// So a row that is plain sequential at `phase` is plain sequential at every q <= 5 - len (len 1, 2: all four phases;
+// 3: 0..2; 4: 0, 1; 5: 0). Any other cut has a tree that depends on q (the scan joins two or more pieces of at least
+// two entries, or three or more pieces), and such a row keeps its phase.
+__host__ __device__ __forceinline__ unsigned spmv3_same_sum_phases(int len, int phase) {
+  if (phase + len > 5) return 1u << phase;
+  return (1u << (6 - len < 4 ? 6 - len : 4)) - 1u;
+}
+
 
 template <int POST>
 __global__ void __launch_bounds__(SPMV3_THREADS, SPMV3_CTAS_PER_SM)
@@ -813,8 +827,10 @@ extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, c
 //   b200_spmv_permuted_rows : row-permuted copy of the first `nrows` rows of the permutation of a flagged-stream
 //                             operator (row `new` = row perm[new] of M); segments are copied with their flags, the
 //                             warp-tiles are recomputed. Rows left out are never written (the caller leaves out
-//                             empty rows only, so the entry count stays M's). Every row keeps the LANE SPLIT it has
-//                             in M, so that the copy computes bit-for-bit the row sums M computes (see below);
+//                             empty rows only, so the entry count stays M's). Every row is placed where the kernel
+//                             sums it as in M, so the copy computes bit-for-bit the row sums M computes (see below).
+//                             The placement reorders rows slightly: the final order is written back to perm, and inv
+//                             is computed from it;
 //   b200_spmv_refresh_permuted : values only (after the resident operators were rescaled in place);
 //   b200_spmv_renumbered_cols  : a VIEW of M whose stored column indices are mapped through inv[] (flags kept);
 //                             row pointers, values and warp-tiles are M's own (borrowed, not copied).
@@ -822,10 +838,82 @@ extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, c
 // Lane split. The flag kernel sums a row inside one lane sequentially and combines the pieces of a row that spans lanes
 // with a scan whose tree depends only on the pieces (lanes own the entries [4l, 4l+4) of the 16-byte-aligned stream;
 // a leading lane that holds only explicit zeros adds exact zeros). The pieces are set by the position of the row's
-// first entry modulo 4 and its length. The permuted copy therefore places every row so that it is cut into the same
-// pieces as in M: a row that spans lanes in M starts at the same position modulo 4, a row that fits one lane in M fits
-// one lane here. Up to 3 explicit zeros (SKIP, no END) lead a row's segment to get there. With the row sums equal, the
-// CG operator computes what the plain pair computes, only faster.
+// first entry modulo 4 (its phase) and its length, and spmv3_same_sum_phases gives the phases at which a row sums as it
+// does in M: any phase where it is still one plain sequential chain if it is one in M, else its phase in M.
+// b200_spmv_place_rows lays the rows out in their sorted order, except that at every position it takes the earliest
+// of the next SPMV3_PLACE_WINDOW rows that may start there. Only when none may, up to 3 explicit zeros (SKIP, no END)
+// lead a row's segment to a phase it may take. On C2-shaped matrices the zeros are 0.14 % of nnz (a window of 16: 0.9 %,
+// 64: 0.01 %; keeping every row's lane pieces as in M took 30 %), and a row's smallest column moves by 0.75 columns on
+// average. With the row sums equal, the CG operator computes what the plain pair computes, only faster.
+#define SPMV3_PLACE_WINDOW 32
+
+// Pure host code, exported with the phase masks for the CPU tests (tests/test_spmv_place_rows_cpu.py). sp_old: M's
+// stored row pointers; perm[0..nrows): rows of M in sorted order, every one non-empty and at most SPMV3_MAXROW long. On
+// return perm[0..nrows) holds the rows in the order they are laid out, each less than SPMV3_PLACE_WINDOW slots from
+// where it came in, and sp_new[0..nrows] the copy's stored row pointers (a segment is its leading zeros, then the row's
+// entries). Returns the copy's stored count; sp_new is valid only if that passes spmv3_fits. The result depends only
+// on sp_old and the incoming perm.
+extern "C" long long b200_spmv_place_rows(int nrows, const int *sp_old, int *perm, int *sp_new) {
+  // The pending rows live in a ring indexed by slot % 64, with one bit mask per phase of the rows that may start there.
+  // A row is placed at the latest when it is SPMV3_PLACE_WINDOW - 1 slots late, so the pending slots span less than
+  // 2 * SPMV3_PLACE_WINDOW. Selecting by bit scans instead of walking a list keeps the loop nearly free of branches
+  // that depend on the data: at C2 size it runs in a few tens of ms.
+  static_assert(2 * SPMV3_PLACE_WINDOW <= 64, "the pending rows must fit a 64-slot ring");
+  // length and phase in M of every row in sorted order, first: independent random reads of sp_old that overlap
+  std::vector<int> lp((size_t)nrows);
+  for (int i = 0; i < nrows; ++i) lp[(size_t)i] = (sp_old[perm[i] + 1] - sp_old[perm[i]]) << 2 | (sp_old[perm[i]] & 3);
+  int ring_row[64], ring_len[64];
+  unsigned char ring_mask[64];
+  unsigned long long adm[4] = {0, 0, 0, 0};  // bit slot % 64: that pending row may start at phase q
+  unsigned long long longm = 0;  // rows of more than SPMV3_WT - 6 entries: leading zeros may not fit their warp-tile
+  auto rotr = [](unsigned long long v, int s) { return (v >> s) | (v << ((64 - s) & 63)); };
+  int pending = 0, next = 0, s0 = 0;  // s0: the oldest pending slot
+  long long pos = 0;
+  for (int t = 0; t < nrows; ++t) {
+    // perm[t] is overwritten below: every slot up to t + SPMV3_PLACE_WINDOW - 1 has been read by then
+    for (; pending < SPMV3_PLACE_WINDOW && next < nrows; ++next, ++pending) {
+      const int len = lp[(size_t)next] >> 2, b = next & 63;
+      const unsigned m = spmv3_same_sum_phases(len, lp[(size_t)next] & 3);
+      ring_row[b] = perm[next];
+      ring_len[b] = len;
+      ring_mask[b] = (unsigned char)m;
+      for (int q = 0; q < 4; ++q) adm[q] |= (unsigned long long)(m >> q & 1u) << b;
+      longm |= (unsigned long long)(len > SPMV3_WT - 6) << b;
+    }
+    const int c = (int)(pos & 3), sh = s0 & 63;
+    int slot = -1, lead = 0;
+    if (t - s0 < SPMV3_PLACE_WINDOW - 1) {
+      // the earliest row that may start at c; else the earliest with the fewest leading zeros
+      unsigned long long r = rotr(adm[c], sh);
+      if (r) slot = s0 + __builtin_ctzll(r);
+      for (int z = 1; slot < 0 && z < 4; ++z) {
+        r = rotr(adm[(c + z) & 3] & ~longm, sh);
+        if (r) { slot = s0 + __builtin_ctzll(r); lead = z; }
+      }
+    }
+    if (slot < 0) {
+      // the oldest row is due (or only long rows are pending): it goes now, with the zeros it needs unless they would
+      // push its segment out of one warp-tile
+      slot = s0;
+      while (!(ring_mask[s0 & 63] >> ((c + lead) & 3) & 1u)) ++lead;
+      if (c + lead + ring_len[s0 & 63] > SPMV3_WT) lead = 0;
+    }
+    const int b = slot & 63;
+    const unsigned long long keep = ~(1ull << b);
+    for (int q = 0; q < 4; ++q) adm[q] &= keep;
+    longm &= keep;
+    --pending;
+    perm[t] = ring_row[b];
+    sp_new[t] = (int)pos;
+    pos += lead + ring_len[b];
+    const unsigned long long left = adm[0] | adm[1] | adm[2] | adm[3];  // every row may start at some phase
+    if (left) s0 += __builtin_ctzll(rotr(left, s0 & 63));
+  }
+  sp_new[nrows] = (int)pos;
+  return pos;
+}
+extern "C" unsigned b200_spmv3_phase_mask(int len, int phase) { return spmv3_same_sum_phases(len, phase); }
+
 __global__ void k_fill_skip(long long count, int *__restrict__ oi) {
   for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < count; k += (long long)gridDim.x * blockDim.x)
     oi[k] = (int)B200_FLAG_SKIP;
@@ -851,13 +939,18 @@ __global__ void k_renumber_cols(long long stored, const int *__restrict__ ci, co
   }
 }
 
-extern "C" B200Spmv *b200_spmv_permuted_rows(const B200Spmv *S, const int *d_perm, int nrows) {
+__global__ void k_invert_perm(int n, const int *__restrict__ perm, int *__restrict__ inv) {
+  for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n; i += gridDim.x * blockDim.x) inv[perm[i]] = i;
+}
+
+extern "C" B200Spmv *b200_spmv_permuted_rows(const B200Spmv *S, int *d_perm, int *d_inv, int nrows) {
   if (!S || S->d_vptr != nullptr || nrows <= 0 || nrows > S->nrows) return nullptr;
   cudaStream_t st = (cudaStream_t)b200_stream();
   B200Spmv *M = (B200Spmv *)calloc(1, sizeof(B200Spmv));
   if (!M) return nullptr;
   M->nrows = nrows; M->ncols = S->ncols; M->nnz = S->nnz;
-  // segment layout on the host (sequential, O(rows)): stored row pointers of M and the permutation come back once
+  // placement on the host (sequential, O(rows)): stored row pointers of S and the sorted rows come back once, the
+  // placed order goes up before anything reads d_perm
   std::vector<int> h_old((size_t)S->nrows + 1), h_perm((size_t)nrows);
   Spmv3Plan P;
   P.rowptr.resize((size_t)nrows + 1);
@@ -865,19 +958,12 @@ extern "C" B200Spmv *b200_spmv_permuted_rows(const B200Spmv *S, const int *d_per
   P.nvrows = nrows;
   bool ok = b200_d2h(h_old.data(), S->d_rowptr, h_old.size() * 4) == 0 &&
             b200_d2h(h_perm.data(), d_perm, h_perm.size() * 4) == 0 && b200_sync() == 0;
-  long long pos = 0;
-  for (int r = 0; ok && r < nrows; ++r) {
-    const int a = h_old[(size_t)h_perm[(size_t)r]], len = h_old[(size_t)h_perm[(size_t)r] + 1] - a;
-    const int phase = a & 3, c = (int)(pos & 3);
-    int lead;
-    if (phase + len <= 4) lead = c + len <= 4 ? 0 : 4 - c;  // one lane in M: one lane here
-    else lead = (phase - c) & 3;                              // spans lanes in M: the same first position modulo 4
-    if (c + lead + len > SPMV3_WT) lead = 0;  // a row of more than 121 entries: its warp-tile could not hold the zeros
-    P.rowptr[(size_t)r] = (int)pos;
-    pos += lead + len;
+  const long long pos = ok ? b200_spmv_place_rows(nrows, h_old.data(), h_perm.data(), P.rowptr.data()) : 0;
+  ok = ok && spmv3_fits(pos) && b200_h2d(d_perm, h_perm.data(), h_perm.size() * 4) == 0;
+  if (ok) {
+    k_invert_perm<<<8 * b200_num_sms(), 256, 0, st>>>(S->nrows, d_perm, d_inv);
+    b200_count_launch(1);
   }
-  P.rowptr[(size_t)nrows] = (int)pos;
-  ok = ok && spmv3_fits(pos);
   if (ok) {
     const size_t pad = (((size_t)pos + 3) & ~(size_t)3) + 8;
     M->stored = pos;
