@@ -60,13 +60,17 @@ long long b200_spmv_stored(const B200Spmv *M);     /* entries in the stream: fla
 const double *b200_spmv_vals(const B200Spmv *M);   /* device */
 const int *b200_spmv_colidx(const B200Spmv *M);    /* device */
 const int *b200_spmv_rowptr(const B200Spmv *M);    /* device */
-/* algorithmic bytes of one launch: 12 nnz + 4 (R+1) + 8 C + 8 R (+ 8 R per extra row vector) */
+/* algorithmic bytes of one launch: 12 nnz (11 nnz packed) + 4 (R+1) + 8 C + 8 R (+ 8 R per extra row vector) */
 double b200_spmv_alg_bytes(const B200Spmv *M, int extra_row_vectors);
 
 enum { B200_POST_NONE = 0, B200_POST_DIV = 1, B200_POST_FMA_DOT = 2, B200_POST_FMA = 3, B200_POST_MUL = 4 };
 /* B200_POST_MUL: y = s * d[r] with d = R_y^-1 precomputed -- what the reference's own GPU backend does
  * (linsys/gpu/indirect/private.c:78,164: inv_r_y, scale_by_diag); used by K1 inside the CG loop, where the fp64
  * division chain of POST_DIV holds the warps out of the gather pipeline. */
+/* The row operand d[r] of the epilogue: a vector (B200_D_VEC), one value d[0] for every row (B200_D_ONE), or a
+ * two-value table d[0..1] indexed by bit r of d_dmask (B200_D_TWO). The table forms stream no row vector; the one-pass
+ * flagged-stream kernel only (no virtual rows). */
+enum { B200_D_VEC = 0, B200_D_ONE = 1, B200_D_TWO = 2 };
 enum { B200_HOOK_NONE = 0, B200_HOOK_CG_ALPHA = 1, B200_HOOK_P2P_SIGNAL = 2, B200_HOOK_P2P_ROUTE = 3 };
 /* B200_HOOK_P2P_SIGNAL: when the LAST block of the launch has stored its rows, it publishes
  * hook_val into slot `rank` of every peer's flag line (d_hook_arg -> B200P2pSignal). */
@@ -96,6 +100,8 @@ typedef struct {
   double init_sign;
   int post;              /* B200_POST_*: y = s | s / d[r] | fma(d[r], v[r], s) with dot(v, y) | same, no dot | s * d[r] */
   const double *d_d;
+  int dform;             /* B200_D_*: how d[r] is read (the post-operations other than NONE) */
+  const unsigned *d_dmask; /* B200_D_TWO: bit r selects d_d[0] or d_d[1] for row r */
   const double *d_v;
   double *d_dot;         /* B200_POST_FMA_DOT: receives sum_r v[r]*y[r] */
   int hook;              /* B200_HOOK_*: run by the last block after the dot is final */
@@ -113,6 +119,10 @@ int b200_perm_rows_by_min_col(const B200Spmv *A, int *d_perm /* new -> old */);
 B200Spmv *b200_spmv_permuted_rows(const B200Spmv *M, int *d_perm, int *d_inv, int nrows /* kept: perm[0..nrows) */);
 int b200_spmv_refresh_permuted(B200Spmv *Mp, const B200Spmv *M, const int *d_perm); /* values only */
 B200Spmv *b200_spmv_renumbered_cols(const B200Spmv *M, const int *d_inv /* old -> new */); /* view: borrows M's arrays */
+/* for the CG loop's operators: store the index stream at 3 bytes per entry when M has at most 2^22 columns (else
+ * nothing changes); M then serves POST_MUL / POST_FMA_DOT / POST_FMA only and b200_spmv_colidx(M) is NULL */
+int b200_spmv_pack_indices(B200Spmv *M);
+int b200_spmv_entry_bytes(const B200Spmv *M); /* bytes per stored entry the kernel streams: 12, or 11 when packed */
 /* host placement behind b200_spmv_permuted_rows (pure host code): returns the copy's stored count */
 long long b200_spmv_place_rows(int nrows, const int *sp_old, int *perm, int *sp_new);
 int b200_gather_vec(int n, const int *d_perm, const double *d_src, double *d_dst); /* dst[i] = src[perm[i]] */
@@ -144,6 +154,13 @@ typedef struct {
    * rows of A sorted by smallest column, At_cg = A' with its column indices renumbered, d_ry_cg = R_y in that order */
   const B200Spmv *A_cg, *At_cg;
   const double *d_ry_cg;
+  /* the same row operands as tables (b200_cg_classify_diag): d_diag_tab = {the two values of 1/R_y over the rows of
+   * A_cg, R_x[0]}, bit r of d_ry_mask picks the value of row r of A_cg; ry_form = B200_D_TWO when 1/R_y takes at most
+   * two values there, rx_form = B200_D_ONE when R_x is uniform, else B200_D_VEC (d_ry_cg, d_rx) */
+  double *d_diag_tab;
+  unsigned *d_diag_mixed;
+  unsigned *d_ry_mask;
+  int ry_form, rx_form;
   const double *d_rx;  /* R_x (n) */
   const double *d_ry;  /* R_y (m) */
   double *d_ry_inv;    /* 1 / R_y (m), refreshed by b200_cg_set_preconditioner */
@@ -165,6 +182,9 @@ typedef struct {
 
 /* M_j = 1 / (R_x,j + P_jj + sum_k A_kj^2 / R_y,k)   (private.c:50-82) */
 int b200_cg_set_preconditioner(const B200Cg *cg, const double *d_Pdiag);
+/* after b200_cg_set_preconditioner, with the reordered pair and d_perm (its rows) in place: fills d_diag_tab and
+ * d_ry_mask and sets ry_form / rx_form (one 4-byte read-back) */
+int b200_cg_classify_diag(B200Cg *cg, const int *d_perm);
 /* Full device solve of [[R_x+P, A'],[A, -R_y]] [x;y] = b in place on d_b (n+m),
  * warm start d_s (n) or NULL; returns CG iterations (>=0) or <0 on error.
  * Synchronises with the host only to poll the done flag. (private.c:284-324) */
@@ -172,7 +192,8 @@ int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double tol, int ma
                   int its_hint, const double *d_tol /* optional device tol */);
 /* one CG iteration (4 kernels), for timing */
 int b200_cg_one_iteration(B200Cg *cg, double *d_x);
-double b200_cg_iter_alg_bytes(const B200Cg *cg);
+/* algorithmic bytes of one CG iteration; per_kernel (optional): K1, K2, K3, K4 (DESIGN.md section 3) */
+double b200_cg_iter_alg_bytes(const B200Cg *cg, double *per_kernel);
 /* per-kernel device times (ms per launch) of `reps` genuine CG iterations: K1, K2, K3, K4, whole iteration */
 int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *out_ms);
 

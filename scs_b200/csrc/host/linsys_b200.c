@@ -391,20 +391,29 @@ static int cg_ops_build(ScsLinSysWork *w) {
   w->d_perm = (int *)b200_malloc((size_t)w->m * 4);
   w->d_inv = (int *)b200_malloc((size_t)w->m * 4);
   w->d_ry_cg = (double *)b200_malloc((size_t)w->m * 8);
-  if (!w->d_perm || !w->d_inv || !w->d_ry_cg) return -1;
+  w->cg.d_diag_tab = (double *)b200_malloc(3 * 8);
+  w->cg.d_diag_mixed = (unsigned *)b200_malloc(4);
+  w->cg.d_ry_mask = (unsigned *)b200_malloc(((size_t)kept + 31) / 32 * 4);
+  if (!w->d_perm || !w->d_inv || !w->d_ry_cg || !w->cg.d_diag_tab || !w->cg.d_diag_mixed || !w->cg.d_ry_mask)
+    return -1;
   if (b200_perm_rows_by_min_col(w->A, w->d_perm) != 0) return -1;
   /* the placement reorders the sorted rows slightly: d_perm is final, and d_inv computed from it, only after this */
   w->A_cg = b200_spmv_permuted_rows(w->A, w->d_perm, w->d_inv, kept);
   if (!w->A_cg) return -1;
   w->At_cg = b200_spmv_renumbered_cols(w->At, w->d_inv);
   if (!w->At_cg) return -1;
+  /* only the CG loop reads these two: their index streams go to 3 bytes per entry where the columns allow it */
+  if (b200_spmv_pack_indices(w->A_cg) != 0 || b200_spmv_pack_indices(w->At_cg) != 0) return -1;
   w->cg.A_cg = w->A_cg; w->cg.At_cg = w->At_cg; w->cg.d_ry_cg = w->d_ry_cg;
   return 0;
 }
+/* R_y and R_x as tables when SCS's form of diag_r holds (two values of R_y, one of R_x; any other diag_r, e.g. through
+ * scs_update_lin_sys_diag_r, takes the vectors): K1 and K2 then stream no row vector for them */
 static int cg_ops_refresh(ScsLinSysWork *w) {
   if (!w->A_cg) return 0;
   if (b200_spmv_refresh_permuted(w->A_cg, w->A, w->d_perm) != 0) return -1;
-  return b200_gather_vec(w->m, w->d_perm, w->cg.d_ry_inv, w->d_ry_cg); /* 1 / R_y in the permuted order */
+  if (b200_gather_vec(w->m, w->d_perm, w->cg.d_ry_inv, w->d_ry_cg) != 0) return -1; /* 1 / R_y, permuted order */
+  return b200_cg_classify_diag(&w->cg, w->d_perm);
 }
 
 ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
@@ -537,6 +546,9 @@ void scs_free_lin_sys_work(ScsLinSysWork *w) {
   b200_spmv_destroy(w->At_cg); /* a view of At: before At itself */
   b200_spmv_destroy(w->A_cg);
   b200_free(w->d_ry_cg);
+  b200_free(w->cg.d_diag_tab);
+  b200_free(w->cg.d_diag_mixed);
+  b200_free(w->cg.d_ry_mask);
   b200_free(w->d_perm);
   b200_free(w->d_inv);
   b200_spmv_destroy(w->A);
@@ -671,11 +683,10 @@ double scs_b200_time_spmv(ScsLinSysWork *w, scs_int op, scs_int reps, double *al
 /* bench.py roofline: the kernels of the CG loop as they run inside a solve (the solver's own p / tmp / r after
  * a genuine start on the right-hand side b, which the caller provides: length n + m, host). out_ms[0..4] = ms
  * per launch of K1, K2, K3, K4 and of the whole iteration; out_bytes[0..4] = the algorithmic bytes of each
- * (DESIGN.md section 3: K1 12 nnz + 4(m+1) + 8n + 16m, K2 12 nnz + 4(n+1) + 8m + 24n, K3 64n, K4 24n). */
+ * (b200_cg_iter_alg_bytes, DESIGN.md section 3). */
 scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms,
                                  double *out_bytes) {
   const size_t nm = (size_t)w->n + w->m;
-  const double nnz = (double)b200_spmv_nnz(w->A), n = (double)w->n, m = (double)w->m;
   int k;
   if (w->P) return -1;
   if (b200_h2d(w->d_b, b, nm * 8) != 0) return -1;
@@ -686,13 +697,7 @@ scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int r
   for (k = 0; k < 3; ++k) if (b200_cg_one_iteration(&w->cg, w->d_b) != 0) return -1;
   if (b200_sync() != 0) return -1;
   if (b200_cg_time_kernels(&w->cg, w->d_b, (int)reps, out_ms) != 0) return -1;
-  if (out_bytes) {
-    out_bytes[0] = 12.0 * nnz + 4.0 * (m + 1.0) + 8.0 * n + 16.0 * m;
-    out_bytes[1] = 12.0 * nnz + 4.0 * (n + 1.0) + 8.0 * m + 24.0 * n;
-    out_bytes[2] = 64.0 * n;
-    out_bytes[3] = 24.0 * n;
-    out_bytes[4] = b200_cg_iter_alg_bytes(&w->cg);
-  }
+  if (out_bytes) out_bytes[4] = b200_cg_iter_alg_bytes(&w->cg, out_bytes);
   return 0;
 }
 
@@ -718,7 +723,7 @@ double scs_b200_time_cg_iter(ScsLinSysWork *w, scs_int reps, double *alg_bytes) 
   for (k = 0; k < reps; ++k) if (b200_cg_one_iteration(&w->cg, w->d_b) != 0) goto out;
   ms = b200_timer_stop_ms();
   if (ms >= 0) ms /= (double)reps;
-  if (alg_bytes) *alg_bytes = b200_cg_iter_alg_bytes(&w->cg);
+  if (alg_bytes) *alg_bytes = b200_cg_iter_alg_bytes(&w->cg, NULL);
 out:
   free(hb);
   return ms;

@@ -757,6 +757,65 @@ __global__ void k_recip(long long len, const double *__restrict__ v, double *__r
   for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < len; i += (long long)gridDim.x * blockDim.x)
     out[i] = 1.0 / v[i];
 }
+// Row operands of the reordered pair as tables. SCS sets R_y to two values (zero-cone rows and the rest) and R_x to
+// one, so K1 and K2 need not stream a row vector for them. The table holds k_recip's own results, so the products
+// are the same bits as with d_ry_cg / d_rx. Values are compared by their bits.
+__global__ void k_diag_tab_init(const int *__restrict__ perm, const double *__restrict__ ry_inv,
+                                const double *__restrict__ rx, double *__restrict__ tab, unsigned *mixed) {
+  tab[0] = tab[1] = ry_inv[perm[0]];
+  tab[2] = rx[0];
+  *mixed = 0u;
+}
+// bit r of mask: 1/R_y of row r of A_cg is not tab[0]. The first other value claims tab[1]; a third one sets bit 0 of
+// *mixed, an R_x that is not tab[2] bit 1.
+__global__ void k_diag_tab_classify(int kept, int n, const int *__restrict__ perm, const double *__restrict__ ry_inv,
+                                    const double *__restrict__ rx, double *tab, unsigned *mask, unsigned *mixed) {
+  const unsigned FULL = 0xffffffffu;
+  const unsigned long long b0 = (unsigned long long)__double_as_longlong(tab[0]);
+  const unsigned long long x0 = (unsigned long long)__double_as_longlong(tab[2]);
+  unsigned long long *b1 = reinterpret_cast<unsigned long long *>(tab + 1);
+  const int lane = threadIdx.x & 31;
+  const long long warp = ((long long)blockIdx.x * blockDim.x + threadIdx.x) >> 5;
+  const long long nwarps = ((long long)gridDim.x * blockDim.x) >> 5;
+  unsigned mx = 0u;
+  for (long long base = warp * 32; base < kept; base += nwarps * 32) {  // warp-uniform
+    const long long r = base + lane;
+    const unsigned long long b = r < kept ? (unsigned long long)__double_as_longlong(ry_inv[perm[r]]) : b0;
+    const unsigned w = __ballot_sync(FULL, b != b0);
+    if (lane == 0) mask[base >> 5] = w;
+    if (w != 0u) {
+      const unsigned long long bl = __shfl_sync(FULL, b, __ffs(w) - 1);
+      if (b != b0 && b != bl) mx |= 1u;
+      if (lane == 0) {
+        unsigned long long cur = *(volatile unsigned long long *)b1;
+        if (cur == b0) {
+          cur = atomicCAS(b1, b0, bl);
+          if (cur == b0) cur = bl;
+        }
+        if (cur != bl) mx |= 1u;
+      }
+    }
+  }
+  for (long long j = (long long)blockIdx.x * blockDim.x + threadIdx.x; j < n; j += (long long)gridDim.x * blockDim.x)
+    if ((unsigned long long)__double_as_longlong(rx[j]) != x0) mx |= 2u;
+  if (mx) atomicOr(mixed, mx);
+}
+
+extern "C" int b200_cg_classify_diag(B200Cg *cg, const int *d_perm) {
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  const int kept = b200_spmv_nrows(cg->A_cg);
+  unsigned mixed = 3u;
+  k_diag_tab_init<<<1, 1, 0, st>>>(d_perm, cg->d_ry_inv, cg->d_rx, cg->d_diag_tab, cg->d_diag_mixed);
+  k_diag_tab_classify<<<vec_grid((long long)kept + cg->n), 256, 0, st>>>(kept, cg->n, d_perm, cg->d_ry_inv, cg->d_rx,
+                                                                        cg->d_diag_tab, cg->d_ry_mask,
+                                                                        cg->d_diag_mixed);
+  b200_count_launch(2);
+  if (b200_d2h(&mixed, cg->d_diag_mixed, 4) != 0 || b200_sync() != 0) return -1;
+  cg->ry_form = (mixed & 1u) ? B200_D_VEC : B200_D_TWO;
+  cg->rx_form = (mixed & 2u) ? B200_D_VEC : B200_D_ONE;
+  return 0;
+}
+
 // ---------------------------------------------------------------------------
 extern "C" int b200_cg_set_preconditioner(const B200Cg *cg, const double *d_Pdiag) {
   cudaStream_t st = (cudaStream_t)b200_stream();
@@ -858,6 +917,19 @@ static int mat_vec_sharded(B200Cg *cg, const double *d_x, double *d_y, int with_
   return 0;
 }
 
+// K1's and K2's row operands: 1 / R_y and R_x, from the tables when the reordered pair has them (the plain pair: the
+// vectors). Sets d_d / dform / d_dmask.
+static void k1_operand(const B200Cg *cg, bool re, B200SpmvArgs &a) {
+  a.dform = re ? cg->ry_form : B200_D_VEC;
+  a.d_d = a.dform == B200_D_TWO ? cg->d_diag_tab : re ? cg->d_ry_cg : cg->d_ry_inv;
+  a.d_dmask = a.dform == B200_D_TWO ? cg->d_ry_mask : nullptr;
+}
+static void k2_operand(const B200Cg *cg, bool re, B200SpmvArgs &a) {
+  a.dform = re ? cg->rx_form : B200_D_VEC;
+  a.d_d = a.dform == B200_D_ONE ? cg->d_diag_tab + 2 : cg->d_rx;
+  a.d_dmask = nullptr;
+}
+
 static int mat_vec(B200Cg *cg, const double *d_x, double *d_y, int with_dot, const int *d_skip) {
   if (cg->nranks > 1) return mat_vec_sharded(cg, d_x, d_y, with_dot, d_skip);
   // the m-space-reordered pair when present: tmp is internal to the operator, so its ordering is free
@@ -868,21 +940,23 @@ static int mat_vec(B200Cg *cg, const double *d_x, double *d_y, int with_dot, con
   // K1: tmp = (A x) ./ R_y
   a.pdl = cg_pdl_enabled() ? 1 : 0;
   a.d_x = d_x; a.d_y = cg->d_tmp; a.d_init = nullptr; a.init_sign = 1.0;
-  a.post = B200_POST_MUL; a.d_d = re ? cg->d_ry_cg : cg->d_ry_inv; a.d_v = nullptr; a.d_dot = nullptr;
+  a.post = B200_POST_MUL; a.d_v = nullptr; a.d_dot = nullptr;
+  k1_operand(cg, re, a);
   a.hook = B200_HOOK_NONE; a.d_hook_arg = nullptr; a.d_skip = d_skip;
   if (b200_spmv(A, &a) != 0) return -1;
   const double *init = nullptr;
   if (cg->P) {
     // y = P x first (reference accumulates P x before A' z)
     a.d_x = d_x; a.d_y = d_y; a.d_init = nullptr; a.post = B200_POST_NONE;
-    a.d_d = nullptr; a.d_v = nullptr;
+    a.d_d = nullptr; a.dform = B200_D_VEC; a.d_dmask = nullptr; a.d_v = nullptr;
     if (b200_spmv(cg->P, &a) != 0) return -1;
     init = d_y;
   }
   // K2: y = fma(R_x, x, init + A' tmp)
   a.d_x = cg->d_tmp; a.d_y = d_y; a.d_init = init; a.init_sign = 1.0;
   a.post = with_dot ? B200_POST_FMA_DOT : B200_POST_FMA;
-  a.d_d = cg->d_rx; a.d_v = d_x; a.d_dot = with_dot ? &cg->d_ctl->pGp : nullptr;
+  k2_operand(cg, re, a);
+  a.d_v = d_x; a.d_dot = with_dot ? &cg->d_ctl->pGp : nullptr;
   a.hook = with_dot ? B200_HOOK_CG_ALPHA : B200_HOOK_NONE;
   a.d_hook_arg = cg->d_ctl; a.d_skip = d_skip;
   return b200_spmv(At, &a);
@@ -1022,11 +1096,12 @@ extern "C" int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *o
       cudaEventRecord(ev[(size_t)r * 5 + 0], st);
       const bool re = cg->A_cg != nullptr && cg->At_cg != nullptr && cg->d_ry_cg != nullptr;
       a.d_x = cg->d_p; a.d_y = cg->d_tmp; a.init_sign = 1.0; a.post = B200_POST_MUL;
-      a.d_d = re ? cg->d_ry_cg : cg->d_ry_inv;
+      k1_operand(cg, re, a);
       a.d_skip = d_skip;
       if (b200_spmv(re ? cg->A_cg : cg->A, &a) != 0) ok = false;
       cudaEventRecord(ev[(size_t)r * 5 + 1], st);
-      a.d_x = cg->d_tmp; a.d_y = cg->d_Gp; a.post = B200_POST_FMA_DOT; a.d_d = cg->d_rx; a.d_v = cg->d_p;
+      a.d_x = cg->d_tmp; a.d_y = cg->d_Gp; a.post = B200_POST_FMA_DOT; a.d_v = cg->d_p;
+      k2_operand(cg, re, a);
       a.d_dot = &cg->d_ctl->pGp; a.hook = B200_HOOK_CG_ALPHA; a.d_hook_arg = cg->d_ctl;
       if (b200_spmv(re ? cg->At_cg : cg->At, &a) != 0) ok = false;
       cudaEventRecord(ev[(size_t)r * 5 + 2], st);
@@ -1059,9 +1134,22 @@ extern "C" int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *o
   return rc;
 }
 
-extern "C" double b200_cg_iter_alg_bytes(const B200Cg *cg) {
-  const double nnz = (double)b200_spmv_nnz(cg->A);
-  return 24.0 * nnz + 4.0 * (cg->m + cg->n + 2.0) + 24.0 * cg->m + 120.0 * cg->n;
+extern "C" double b200_cg_iter_alg_bytes(const B200Cg *cg, double *per_kernel) {
+  const double nnz = (double)b200_spmv_nnz(cg->A), n = cg->n, m = cg->m;
+  const bool re = cg->A_cg != nullptr && cg->At_cg != nullptr && cg->d_ry_cg != nullptr;
+  // the row operand of K1 (1 / R_y) and of K2 (R_x): a vector, or a table (K1: one mask bit per row)
+  const double ry = re && cg->ry_form == B200_D_TWO ? m / 8.0 : 8.0 * m;
+  const double rx = re && cg->rx_form == B200_D_ONE ? 0.0 : 8.0 * n;
+  // bytes per stored entry: 12, or 11 with a packed index stream
+  const double e1 = b200_spmv_entry_bytes(re ? cg->A_cg : cg->A), e2 = b200_spmv_entry_bytes(re ? cg->At_cg : cg->At);
+  double k[4];
+  k[0] = e1 * nnz + 4.0 * (m + 1.0) + 8.0 * n + 8.0 * m + ry;
+  k[1] = e2 * nnz + 4.0 * (n + 1.0) + 8.0 * m + 16.0 * n + rx;
+  k[2] = 64.0 * n;
+  k[3] = 24.0 * n;
+  if (per_kernel)
+    for (int i = 0; i < 4; ++i) per_kernel[i] = k[i];
+  return k[0] + k[1] + k[2] + k[3];
 }
 
 extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double tol, int max_its,

@@ -11,11 +11,12 @@
 // (cp.async.bulk, L2 evict_first) of the value / index slices into shared memory with mbarrier completion,
 // products rounded separately from the adds (__dmul_rn / __dadd_rn: the reference's scalar loop
 // `yj += Ax[p] * x[Ai[p]]` is not contracted to fma in the oracle build), fused epilogues
-// y = s | s / d[r] | fma(d[r], v[r], s) plus the dot product v'y with a deterministic last-block reduction and
+// y = s | s / d[r] | fma(d[r], v[r], s) (d[r] from a vector, or from a one- or two-value table: B200_D_*)
+// plus the dot product v'y with a deterministic last-block reduction and
 // an optional hook that turns the dot into the CG step length on the device.
 //
-// Algorithmic bytes per launch (DESIGN.md): 12*nnz + 4*(R+1) + 8*C + 8*R (+8*R per
-// extra row vector read by the epilogue).
+// Algorithmic bytes per launch (DESIGN.md): 12*nnz (11*nnz with a packed index stream) + 4*(R+1) + 8*C + 8*R (+8*R
+// per extra row vector read by the epilogue).
 #include "../common.cuh"
 #include "../dev_api.h"
 #include <stdlib.h>
@@ -43,6 +44,7 @@ struct B200Spmv {
   int *d_vptr;       // nrows+1, or NULL
   double *d_vscratch;  // nvrows partial sums
   int borrows;       // 1: d_rowptr / d_vals / d_wt3 / d_cta_begin3 belong to another operator (renumbered-columns view)
+  unsigned char *d_idx24;  // the packed index stream (b200_spmv_pack_indices; d_colidx is then NULL), or NULL
 };
 
 // random 8-byte gather of the dense vector: read-only path, optionally without L1 allocation
@@ -182,18 +184,37 @@ __host__ __device__ __forceinline__ unsigned spmv3_same_sum_phases(int len, int 
   return (1u << (6 - len < 4 ? 6 - len : 4)) - 1u;
 }
 
+// Packed index stream of the CG loop's operators (an operator with at most 2^22 columns): 3 bytes per entry, the
+// column in bits 0..21, END in bit 22, SKIP in bit 23. The one encode / decode of that format; decode gives back the
+// int32 entry (flags in bits 31 / 30) bit for bit.
+#define SPMV3_IDX24_MAXCOLS (1 << 22)
+__host__ __device__ __forceinline__ unsigned spmv3_idx24_encode(int v) {
+  const unsigned u = (unsigned)v;
+  return (u & 0x3fffffu) | ((u >> 31) & 1u) << 22 | ((u >> 30) & 1u) << 23;
+}
+__host__ __device__ __forceinline__ int spmv3_idx24_decode(unsigned e) {
+  return (int)((e & 0x3fffffu) | ((e >> 22) & 1u) << 31 | ((e >> 23) & 1u) << 30);
+}
+// The packed slice of a stage's entries [ka, ka + cnt) (ka a multiple of 4): a 1-D bulk copy needs a 16-byte aligned
+// address and a length that is a multiple of 16, so it starts at entry ka & ~15 (byte 3 * (ka & ~15)) and its length
+// is rounded up. At most 12 + 5 entries more than the int32 slice, which is still less than 4 * cnt bytes.
+__host__ __device__ __forceinline__ unsigned spmv3_idx24_slice_bytes(int ka, int cnt) {
+  return (unsigned)((3 * (ka + cnt - (ka & ~15)) + 15) & ~15);
+}
 
-template <int POST>
+
+// IDX24: the index stream is packed (spmv3_idx24_*), else int32
+template <int POST, bool IDX24>
 __global__ void __launch_bounds__(SPMV3_THREADS, SPMV3_CTAS_PER_SM)
-spmv_flag_kernel(const int *__restrict__ colidx, const double *__restrict__ vals,
+spmv_flag_kernel(const void *__restrict__ colidx, const double *__restrict__ vals,
                  const int4 *__restrict__ wt, const int *__restrict__ cta_begin,
                  const double *__restrict__ x, double *__restrict__ y, const double *init,
-                 double init_sign, const double *__restrict__ d, const double *__restrict__ v,
-                 double *dot_out, int hook, void *hook_arg, const int *skip, double *partials,
-                 unsigned int *counter, unsigned long long hook_val) {
+                 double init_sign, const double *__restrict__ d, const unsigned *__restrict__ dmask, int dform,
+                 const double *__restrict__ v, double *dot_out, int hook, void *hook_arg, const int *skip,
+                 double *partials, unsigned int *counter, unsigned long long hook_val) {
   // Programmatic dependent launch: nothing above pdl_wait() reads data a predecessor kernel writes -- the
   // descriptors and the matrix stream are immutable -- so barrier init and the first ring stages overlap the
-  // predecessor's tail. `skip`, x, d, v, init are read only after the wait.
+  // predecessor's tail. `skip`, x, d, dmask, v, init are read only after the wait.
   extern __shared__ __align__(128) unsigned char smem_raw[];
   double *s_vals = reinterpret_cast<double *>(smem_raw);
   int *s_idx = reinterpret_cast<int *>(s_vals + SPMV3_STAGES * SPMV3_CAP);
@@ -256,10 +277,15 @@ spmv_flag_kernel(const int *__restrict__ colidx, const double *__restrict__ vals
           }
           mbar_wait(&s_empty[st], (unsigned)((use - 1) & 1));
         }
-        mbar_expect_tx(&s_full[st], (unsigned)cnt * 12u + (unsigned)(SPMV3_NCW * 16));
+        const unsigned ib = IDX24 ? spmv3_idx24_slice_bytes(ka, cnt) : (unsigned)cnt * 4u;
+        mbar_expect_tx(&s_full[st], (unsigned)cnt * 8u + ib + (unsigned)(SPMV3_NCW * 16));
         tma_load_1d(s_desc + (size_t)st * SPMV3_NCW, g + (size_t)i * SPMV3_NCW, SPMV3_NCW * 16,
                     &s_full[st], pol);
-        tma_load_1d(s_idx + (size_t)st * SPMV3_CAP, colidx + ka, (unsigned)cnt * 4u, &s_full[st], pol);
+        if (IDX24)
+          tma_load_1d(s_idx + (size_t)st * SPMV3_CAP,
+                      static_cast<const unsigned char *>(colidx) + 3 * (size_t)(ka & ~15), ib, &s_full[st], pol);
+        else
+          tma_load_1d(s_idx + (size_t)st * SPMV3_CAP, static_cast<const int *>(colidx) + ka, ib, &s_full[st], pol);
         tma_load_1d(s_vals + (size_t)st * SPMV3_CAP, vals + ka, (unsigned)cnt * 8u, &s_full[st], pol);
       }
       if (!waited) {
@@ -286,6 +312,13 @@ spmv_flag_kernel(const int *__restrict__ colidx, const double *__restrict__ vals
     const unsigned lt = (1u << lane) - 1u;
     const unsigned le = lt | (1u << lane);
     const int sw = (lane >> 2) & 1;
+    // the table forms of d (B200_D_ONE / B200_D_TWO): its values, once per launch
+    constexpr bool TAB = POST == B200_POST_MUL || POST == B200_POST_FMA_DOT || POST == B200_POST_FMA;
+    double dt0 = 0.0, dt1 = 0.0;
+    if (TAB && dform != B200_D_VEC) {
+      dt0 = d[0];
+      dt1 = dform == B200_D_TWO ? d[1] : dt0;
+    }
     for (int i = 0; i < (skipped ? 0 : nt); ++i) {
       const int st = i % SPMV3_STAGES;
       const unsigned par = (unsigned)((i / SPMV3_STAGES) & 1);
@@ -300,7 +333,15 @@ spmv_flag_kernel(const int *__restrict__ colidx, const double *__restrict__ vals
       const bool any = (kb < kend) && (kb + 4 > k0);
       if (any) {
         const int e = kb - ka;
-        iv = *reinterpret_cast<const int4 *>(s_idx + (size_t)st * SPMV3_CAP + e);
+        if (IDX24) {  // 12 bytes from byte 3 * (kb - (ka & ~15)), a multiple of 12: three conflict-free 32-bit LDS
+          const unsigned *wp = reinterpret_cast<const unsigned *>(
+              reinterpret_cast<const unsigned char *>(s_idx + (size_t)st * SPMV3_CAP) + 3 * (kb - (ka & ~15)));
+          const unsigned w0 = wp[0], w1 = wp[1], w2 = wp[2];
+          iv = make_int4(spmv3_idx24_decode(w0 & 0xffffffu), spmv3_idx24_decode(w0 >> 24 | (w1 & 0xffffu) << 8),
+                         spmv3_idx24_decode(w1 >> 16 | (w2 & 0xffu) << 16), spmv3_idx24_decode(w2 >> 8));
+        } else {
+          iv = *reinterpret_cast<const int4 *>(s_idx + (size_t)st * SPMV3_CAP + e);
+        }
         t0 = *reinterpret_cast<const double2 *>(s_vals + (size_t)st * SPMV3_CAP + e + 2 * sw);
         t1 = *reinterpret_cast<const double2 *>(s_vals + (size_t)st * SPMV3_CAP + e + 2 - 2 * sw);
       }
@@ -320,12 +361,19 @@ spmv_flag_kernel(const int *__restrict__ colidx, const double *__restrict__ vals
       const int nrows_w = dsc.w;
       // epilogue operands of the first two rounds (rows row0 + lane, row0 + lane + 32): in flight
       // together with the gathers
+      // (B200_D_TWO: the mask words, at most two per round; the table value is selected at the use)
       double pd0 = 0.0, pd1 = 0.0, pv0 = 0.0, pv1 = 0.0, pi0 = 0.0, pi1 = 0.0;
+      unsigned pw0 = 0u, pw1 = 0u;
       {
         const bool r0ok = lane < nrows_w, r1ok = lane + 32 < nrows_w;
         if (POST != B200_POST_NONE) {
-          if (r0ok) pd0 = d[row0 + lane];
-          if (r1ok) pd1 = d[row0 + lane + 32];
+          if (!TAB || dform == B200_D_VEC) {
+            if (r0ok) pd0 = d[row0 + lane];
+            if (r1ok) pd1 = d[row0 + lane + 32];
+          } else if (TAB && dform == B200_D_TWO) {
+            if (r0ok) pw0 = dmask[(row0 + lane) >> 5];
+            if (r1ok) pw1 = dmask[(row0 + lane + 32) >> 5];
+          }
         }
         if (POST == B200_POST_FMA_DOT || POST == B200_POST_FMA) {
           if (r0ok) pv0 = v[row0 + lane];
@@ -395,13 +443,16 @@ spmv_flag_kernel(const int *__restrict__ colidx, const double *__restrict__ vals
           const int row = row0 + rr;
           double sres = ws[rr];
           double dv, vv, iv0;
-          if (j == 0) { dv = pd0; vv = pv0; iv0 = pi0; }
-          else if (j == 1) { dv = pd1; vv = pv1; iv0 = pi1; }
+          unsigned dw;
+          if (j == 0) { dv = pd0; dw = pw0; vv = pv0; iv0 = pi0; }
+          else if (j == 1) { dv = pd1; dw = pw1; vv = pv1; iv0 = pi1; }
           else {
-            dv = (POST != B200_POST_NONE) ? d[row] : 0.0;
+            dv = (POST != B200_POST_NONE && (!TAB || dform == B200_D_VEC)) ? d[row] : 0.0;
+            dw = (TAB && dform == B200_D_TWO) ? dmask[row >> 5] : 0u;
             vv = (POST == B200_POST_FMA_DOT || POST == B200_POST_FMA) ? v[row] : 0.0;
             iv0 = (init != nullptr) ? init[row] : 0.0;
           }
+          if (TAB && dform != B200_D_VEC) dv = (dw >> (row & 31)) & 1u ? dt1 : dt0;
           if (init != nullptr) sres = __dadd_rn(sres, init_sign * iv0);
           if (routed) {  // push the row to the rank that owns it, as a self-validating 16-byte element
             int o = 0;
@@ -658,11 +709,16 @@ static void spmv_set_attrs() {
   static bool attr_done = false;
   if (attr_done) return;
   const int bytes = (int)spmv3_smem_bytes();
-  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_NONE>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_DIV>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_MUL>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA_DOT>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
-  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA>, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes);
+  const cudaFuncAttribute at = cudaFuncAttributeMaxDynamicSharedMemorySize;
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_NONE, false>, at, bytes);
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_DIV, false>, at, bytes);
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_MUL, false>, at, bytes);
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA_DOT, false>, at, bytes);
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA, false>, at, bytes);
+  // the packed index stream serves the CG loop's operators only: K1, K2 and the warm start's K2
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_MUL, true>, at, bytes);
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA_DOT, true>, at, bytes);
+  cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA, true>, at, bytes);
   attr_done = true;
 }
 
@@ -913,6 +969,10 @@ extern "C" long long b200_spmv_place_rows(int nrows, const int *sp_old, int *per
   return pos;
 }
 extern "C" unsigned b200_spmv3_phase_mask(int len, int phase) { return spmv3_same_sum_phases(len, phase); }
+// the packed index format, exported for the CPU tests (tests/test_spmv_packed_cpu.py)
+extern "C" unsigned b200_spmv3_idx24_encode(int v) { return spmv3_idx24_encode(v); }
+extern "C" int b200_spmv3_idx24_decode(unsigned e) { return spmv3_idx24_decode(e); }
+extern "C" unsigned b200_spmv3_idx24_slice_bytes(int ka, int cnt) { return spmv3_idx24_slice_bytes(ka, cnt); }
 
 __global__ void k_fill_skip(long long count, int *__restrict__ oi) {
   for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < count; k += (long long)gridDim.x * blockDim.x)
@@ -1022,10 +1082,44 @@ extern "C" B200Spmv *b200_spmv_renumbered_cols(const B200Spmv *S, const int *d_i
   return M;
 }
 
+// The CG loop's operators stream their column indices packed when they have at most 2^22 columns (3 bytes per entry
+// instead of 4): packed on the device, then the int32 stream is freed. Only the flag kernel reads the packed stream;
+// b200_spmv_colidx of such an operator is NULL.
+__global__ void k_pack_idx24(long long count, const int *__restrict__ ci, unsigned char *__restrict__ out) {
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < count; k += (long long)gridDim.x * blockDim.x) {
+    const unsigned e = spmv3_idx24_encode(ci[k]);
+    out[3 * k] = (unsigned char)e;
+    out[3 * k + 1] = (unsigned char)(e >> 8);
+    out[3 * k + 2] = (unsigned char)(e >> 16);
+  }
+}
+extern "C" int b200_spmv_pack_indices(B200Spmv *M) {
+  if (M->ncols > SPMV3_IDX24_MAXCOLS || M->d_idx24 != nullptr || M->d_vptr != nullptr) return 0;
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  // the int32 stream's padded length; the last bulk copy reads up to 15 bytes past its rounded end
+  const size_t pad = (((size_t)M->stored + 3) & ~(size_t)3) + 8;
+  unsigned char *p = (unsigned char *)b200_malloc(3 * pad + 16);
+  if (!p || b200_memset0(p + 3 * pad, 16) != 0) {
+    b200_free(p);
+    return -1;
+  }
+  k_pack_idx24<<<8 * b200_num_sms(), 256, 0, st>>>((long long)pad, M->d_colidx, p);
+  b200_count_launch(1);
+  if (cudaGetLastError() != cudaSuccess || b200_sync() != 0) {
+    b200_free(p);
+    return -1;
+  }
+  b200_free(M->d_colidx);
+  M->d_colidx = nullptr;
+  M->d_idx24 = p;
+  return 0;
+}
+
 extern "C" void b200_spmv_destroy(B200Spmv *M) {
   if (!M) return;
   if (M->borrows) {  // a view: only the column indices, the reduction slots and the ticket counter are its own
     b200_free(M->d_colidx);
+    b200_free(M->d_idx24);
     b200_free(M->d_partials);
     b200_free(M->d_counter);
     free(M);
@@ -1033,6 +1127,7 @@ extern "C" void b200_spmv_destroy(B200Spmv *M) {
   }
   b200_free(M->d_rowptr);
   b200_free(M->d_colidx);
+  b200_free(M->d_idx24);
   b200_free(M->d_vals);
   b200_free(M->d_partials);
   b200_free(M->d_counter);
@@ -1050,9 +1145,10 @@ extern "C" const double *b200_spmv_vals(const B200Spmv *M) { return M->d_vals; }
 extern "C" const int *b200_spmv_colidx(const B200Spmv *M) { return M->d_colidx; }
 extern "C" const int *b200_spmv_rowptr(const B200Spmv *M) { return M->d_rowptr; }
 extern "C" double b200_spmv_alg_bytes(const B200Spmv *M, int extra_row_vectors) {
-  return 12.0 * (double)M->nnz + 4.0 * (M->nrows + 1.0) + 8.0 * M->ncols +
+  return b200_spmv_entry_bytes(M) * (double)M->nnz + 4.0 * (M->nrows + 1.0) + 8.0 * M->ncols +
          8.0 * M->nrows * (1.0 + extra_row_vectors);
 }
+extern "C" int b200_spmv_entry_bytes(const B200Spmv *M) { return M->d_idx24 != nullptr ? 11 : 12; }
 
 extern "C" int b200_spmv(const B200Spmv *M, const B200SpmvArgs *a) {
   if (M->nrows == 0) return 0;
@@ -1064,11 +1160,16 @@ extern "C" int b200_spmv(const B200Spmv *M, const B200SpmvArgs *a) {
                    cudaErrorInvalidValue, __FILE__, __LINE__);
     return -1;
   }
+  if (a->dform != B200_D_VEC && a->post != B200_POST_NONE && !b200_spmv_can_route(M)) {
+    b200_set_error("b200_spmv: the table forms of d need the one-pass flagged-stream kernel", cudaErrorInvalidValue,
+                   __FILE__, __LINE__);
+    return -1;
+  }
   if (M->d_vptr != nullptr) {
     // long-row mode: sums per virtual row, then the combine pass with the real epilogue
-    spmv_flag_kernel<B200_POST_NONE><<<grid, block, smem, st>>>(
+    spmv_flag_kernel<B200_POST_NONE, false><<<grid, block, smem, st>>>(
         M->d_colidx, M->d_vals, M->d_wt3, M->d_cta_begin3, a->d_x, M->d_vscratch, nullptr, 1.0, nullptr, nullptr,
-        nullptr, B200_HOOK_NONE, nullptr, a->d_skip, M->d_partials, M->d_counter, 0ull);
+        B200_D_VEC, nullptr, nullptr, B200_HOOK_NONE, nullptr, a->d_skip, M->d_partials, M->d_counter, 0ull);
     int cg = (M->nrows + 255) / 256;
     const int cap = 8 * b200_num_sms();
     if (cg > cap) cg = cap;
@@ -1089,20 +1190,33 @@ extern "C" int b200_spmv(const B200Spmv *M, const B200SpmvArgs *a) {
     CUDA_OK(cudaGetLastError());
     return 0;
   }
-#define LAUNCH(POSTV)                                                                                          \
-  CUDA_OK(b200_launch(spmv_flag_kernel<POSTV>, grid, block, smem, st, a->pdl != 0, (const int *)M->d_colidx,  \
+  if (M->d_idx24 != nullptr && a->post != B200_POST_MUL && a->post != B200_POST_FMA_DOT && a->post != B200_POST_FMA) {
+    b200_set_error("b200_spmv: an operator with a packed index stream takes POST_MUL / POST_FMA_DOT / POST_FMA only",
+                   cudaErrorInvalidValue, __FILE__, __LINE__);
+    return -1;
+  }
+  const void *idx = M->d_idx24 != nullptr ? (const void *)M->d_idx24 : (const void *)M->d_colidx;
+#define LAUNCH_IDX(POSTV, PACKED)                                                                              \
+  CUDA_OK(b200_launch(spmv_flag_kernel<POSTV, PACKED>, grid, block, smem, st, a->pdl != 0, idx,               \
                       (const double *)M->d_vals, (const int4 *)M->d_wt3, (const int *)M->d_cta_begin3, a->d_x, \
-                      a->d_y, a->d_init, a->init_sign, a->d_d, a->d_v, a->d_dot, a->hook, a->d_hook_arg,       \
+                      a->d_y, a->d_init, a->init_sign, a->d_d, a->d_dmask, a->dform, a->d_v, a->d_dot, a->hook, \
+                      a->d_hook_arg,                                                                             \
                       a->d_skip, M->d_partials, M->d_counter, a->hook_val))
+#define LAUNCH(POSTV)                 \
+  if (M->d_idx24 != nullptr)          \
+    LAUNCH_IDX(POSTV, true);          \
+  else                                \
+    LAUNCH_IDX(POSTV, false)
   switch (a->post) {
-    case B200_POST_NONE: LAUNCH(B200_POST_NONE); break;
-    case B200_POST_DIV: LAUNCH(B200_POST_DIV); break;
+    case B200_POST_NONE: LAUNCH_IDX(B200_POST_NONE, false); break;
+    case B200_POST_DIV: LAUNCH_IDX(B200_POST_DIV, false); break;
     case B200_POST_MUL: LAUNCH(B200_POST_MUL); break;
     case B200_POST_FMA_DOT: LAUNCH(B200_POST_FMA_DOT); break;
     case B200_POST_FMA: LAUNCH(B200_POST_FMA); break;
     default: return -1;
   }
 #undef LAUNCH
+#undef LAUNCH_IDX
   b200_count_launch(1);
   CUDA_OK(cudaGetLastError());
   return 0;
