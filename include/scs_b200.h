@@ -9,6 +9,8 @@
  *      DLONG=0, SFLOAT=0 and no spectral cones (reference include/scs.h:47-244,
  *      include/aa_stats.h:21-42, include/scs_types.h:16-30), so a caller
  *      compiled against the reference headers can link this library instead.
+ *      Compiled with USE_SPECTRAL_CONES, ScsCone gains the reference's spectral
+ *      block; that layout is served by libscs_b200_spectral.so.
  *
  *  (2) the LINEAR-SYSTEM PLUGIN ABI -- the five link-time symbols every SCS
  *      backend defines (reference include/linsys.h:25-71).  Host pointers in and
@@ -102,6 +104,18 @@ typedef struct {
   scs_int ep, ed;      /* primal / dual exponential triples */
   scs_float *p;        /* power cone parameters in [-1, 1] [psize]; negative = dual cone */
   scs_int psize;
+#ifdef USE_SPECTRAL_CONES
+  /* spectral cones (layout of the reference's USE_SPECTRAL_CONES build, include/scs.h:154-171); only
+   * libscs_b200_spectral.so is compiled with this block. Their rows follow the power cones in this order. */
+  scs_int *d;          /* log-det cone orders [dsize]: accepted by the layout, refused by scs_init */
+  scs_int dsize;
+  scs_int *nuc_m, *nuc_n; /* nuclear-norm cones: m x n column-major, 1 <= n <= m, 1 + m n rows each */
+  scs_int nucsize;
+  scs_int *ell1;       /* l1-norm cones: 1 + ell1[i] rows each */
+  scs_int ell1_size;
+  scs_int *sl_n, *sl_k; /* sum-of-largest-eigenvalues cones: order n, 0 < k < n, 1 + n(n+1)/2 rows each */
+  scs_int sl_size;
+#endif
 } ScsCone;
 
 /* solution or certificate (layout of reference include/scs.h:180-187) */
@@ -195,7 +209,8 @@ scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int r
                                  double *out_bytes);
 
 /* Cone operator: replaces reference src/cones.c:1498-1596 (init_cone /
- * proj_dual_cone / finish_cone) for zero, LP, box, SOC, PSD, exponential and power cones.
+ * proj_dual_cone / finish_cone) for zero, LP, box, SOC, PSD, exponential and power cones,
+ * and in the spectral library also nuclear-norm, l1-norm and sum-of-largest-eigenvalues cones.
  * D is the row scaling of the equilibrated problem (length m) or NULL
  * (reference normalize_box_cone, cones.c:1160-1177).  x (length m) and r_y
  * (length m or NULL) are HOST arrays; x is projected in place onto the dual

@@ -16,6 +16,8 @@ import numpy as np
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SCS_B200_LIB", os.path.join(_HERE, "libscs_b200.so"))
+# the same kernels behind the reference's USE_SPECTRAL_CONES ScsCone layout (ScsConeSpectral below)
+SPECTRAL_LIB_PATH = os.environ.get("SCS_B200_SPECTRAL_LIB", os.path.join(_HERE, "libscs_b200_spectral.so"))
 
 c_int_p = C.POINTER(C.c_int)
 c_double_p = C.POINTER(C.c_double)
@@ -50,6 +52,18 @@ class ScsCone(C.Structure):
         ("cs", c_int_p), ("cssize", C.c_int), ("ep", C.c_int), ("ed", C.c_int),
         ("p", c_double_p), ("psize", C.c_int),
     ]
+
+
+class ScsConeSpectral(ScsCone):
+    """ScsCone of the reference's USE_SPECTRAL_CONES build (include/scs.h:154-171): 184 bytes, taken by
+    libscs_b200_spectral.so. Log-det cones (d) fit the layout but that library refuses them at scs_init."""
+    _fields_ = [
+        ("d", c_int_p), ("dsize", C.c_int), ("nuc_m", c_int_p), ("nuc_n", c_int_p), ("nucsize", C.c_int),
+        ("ell1", c_int_p), ("ell1_size", C.c_int), ("sl_n", c_int_p), ("sl_k", c_int_p), ("sl_size", C.c_int),
+    ]
+
+
+SPECTRAL_KEYS = ("d", "nuc_m", "nuc_n", "ell1", "sl_n", "sl_k")
 
 
 class ScsSolution(C.Structure):
@@ -123,9 +137,17 @@ class HostProblem:
         self.cone, self._cone_keep = make_cone(cone)
 
 
-def make_cone(cone):
+def is_spectral(cone):
+    return any(cone.get(key) is not None and len(cone.get(key)) > 0 for key in SPECTRAL_KEYS)
+
+
+def make_cone(cone, spectral=None):
+    """ctypes cone struct + the arrays it points into. The struct is a ScsConeSpectral when `spectral` is True, or
+    when it is None and the dict has spectral keys (nuc_m / nuc_n, ell1, sl_n / sl_k, d); otherwise a ScsCone."""
     keep = {}
-    k = ScsCone()
+    if spectral is None:
+        spectral = is_spectral(cone)
+    k = ScsConeSpectral() if spectral else ScsCone()
     k.z = int(cone.get("z", 0))
     k.l = int(cone.get("l", 0))
     bu = cone.get("bu")
@@ -154,6 +176,16 @@ def make_cone(cone):
     if p is not None and len(p) > 0:
         keep["p"] = np.ascontiguousarray(p, dtype=np.float64)
         k.p, k.psize = dptr(keep["p"]), len(keep["p"])
+    if spectral:
+        for key, size, names in (("d", "dsize", ("d",)), ("nuc_m", "nucsize", ("nuc_m", "nuc_n")),
+                                 ("ell1", "ell1_size", ("ell1",)), ("sl_n", "sl_size", ("sl_n", "sl_k"))):
+            v = cone.get(key)
+            if v is None or len(v) == 0:
+                continue
+            for name in names:
+                keep[name] = np.ascontiguousarray(cone[name], dtype=np.int32)
+                setattr(k, name, iptr(keep[name]))
+            setattr(k, size, len(keep[key]))
     return k, keep
 
 
@@ -164,7 +196,19 @@ def cone_rows(cone):
     return (int(cone.get("z", 0)) + int(cone.get("l", 0)) + bs + int(sum(q)) +
             int(sum(int(k) * (int(k) + 1) // 2 for k in s)) +
             int(sum(int(k) * int(k) for k in (cone.get("cs", []) or []))) +
-            3 * (int(cone.get("ep", 0)) + int(cone.get("ed", 0)) + len(cone.get("p", []) or [])))
+            3 * (int(cone.get("ep", 0)) + int(cone.get("ed", 0)) + len(cone.get("p", []) or [])) +
+            spectral_rows(cone))
+
+
+def spectral_rows(cone):
+    """rows of the spectral cones (reference cones.c:435-443); 0 for a cone without them"""
+    if not is_spectral(cone):
+        return 0
+    rows = sum(int(d) * (int(d) + 1) // 2 + 2 for d in (cone.get("d", []) or []))
+    rows += sum(int(m) * int(n) + 1 for m, n in zip(cone.get("nuc_m", []) or [], cone.get("nuc_n", []) or []))
+    rows += sum(int(n) + 1 for n in (cone.get("ell1", []) or []))
+    rows += sum(int(n) * (int(n) + 1) // 2 + 1 for n in (cone.get("sl_n", []) or []))
+    return rows
 
 
 class _Decl:
@@ -185,11 +229,11 @@ class _Decl:
             return _Decl._Sink()
 
 
-def _declare(lib, ours):
-    """Declare the signatures shared by our library and the reference build."""
+def _declare(lib, ours, cone=ScsCone):
+    """Declare the signatures shared by our library and the reference build (`cone`: its ScsCone layout)."""
     lib = _Decl(lib)
     lib.scs_init.restype = C.c_void_p
-    lib.scs_init.argtypes = [C.POINTER(ScsData), C.POINTER(ScsCone), C.POINTER(ScsSettings)]
+    lib.scs_init.argtypes = [C.POINTER(ScsData), C.POINTER(cone), C.POINTER(ScsSettings)]
     lib.scs_solve.restype = C.c_int
     lib.scs_solve.argtypes = [C.c_void_p, C.POINTER(ScsSolution), C.POINTER(ScsInfo), C.c_int]
     lib.scs_update.restype = C.c_int
@@ -197,7 +241,7 @@ def _declare(lib, ours):
     lib.scs_finish.restype = None
     lib.scs_finish.argtypes = [C.c_void_p]
     lib.scs.restype = C.c_int
-    lib.scs.argtypes = [C.POINTER(ScsData), C.POINTER(ScsCone), C.POINTER(ScsSettings),
+    lib.scs.argtypes = [C.POINTER(ScsData), C.POINTER(cone), C.POINTER(ScsSettings),
                         C.POINTER(ScsSolution), C.POINTER(ScsInfo)]
     lib.scs_set_default_settings.restype = None
     lib.scs_set_default_settings.argtypes = [C.POINTER(ScsSettings)]
@@ -227,7 +271,7 @@ def _declare(lib, ours):
     lib.scs_b200_time_cg_kernels.restype = C.c_int
     lib.scs_b200_time_cg_kernels.argtypes = [C.c_void_p, c_double_p, C.c_int, c_double_p, c_double_p]
     lib.scs_b200_init_cone.restype = C.c_void_p
-    lib.scs_b200_init_cone.argtypes = [C.POINTER(ScsCone), C.c_int, c_double_p]
+    lib.scs_b200_init_cone.argtypes = [C.POINTER(cone), C.c_int, c_double_p]
     lib.scs_b200_proj_dual_cone.restype = C.c_int
     lib.scs_b200_proj_dual_cone.argtypes = [C.c_void_p, c_double_p, c_double_p]
     lib.scs_b200_finish_cone.restype = None
@@ -261,25 +305,26 @@ def _declare(lib, ours):
     lib.scs_b200_release_memory.restype = None
 
 
-_lib = None
+_libs = {}
 
 
-def load():
-    """Load scs_b200/libscs_b200.so. Raises if it has not been built."""
-    global _lib
-    if _lib is None:
-        if not os.path.exists(LIB_PATH):
+def load(spectral=False):
+    """Load scs_b200/libscs_b200.so, or with spectral=True scs_b200/libscs_b200_spectral.so (ScsConeSpectral
+    layout, nuclear-norm / l1 / sum-of-largest cones). Raises if it has not been built."""
+    path = SPECTRAL_LIB_PATH if spectral else LIB_PATH
+    if spectral not in _libs:
+        if not os.path.exists(path):
             raise RuntimeError(
-                f"{LIB_PATH} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
+                f"{path} is missing: build it with `python -c 'import __graft_entry__ as g; g.build()'` "
                 "(make -C scs_b200/csrc). There is no CPU fallback.")
         # RTLD_LOCAL: our scs_* symbols must not interpose on the reference build loaded by the tests
-        lib = C.CDLL(LIB_PATH, mode=C.RTLD_LOCAL)
-        _declare(lib, ours=True)
-        _lib = lib
-    return _lib
+        lib = C.CDLL(path, mode=C.RTLD_LOCAL)
+        _declare(lib, ours=True, cone=ScsConeSpectral if spectral else ScsCone)
+        _libs[spectral] = lib
+    return _libs[spectral]
 
 
-def load_reference(path):
+def load_reference(path, spectral=False):
     """Load a build of the UNMODIFIED reference (oracle/_ref/*.so). Test infrastructure only."""
     # the venv's OpenBLAS (the only LAPACK in this image) needs its bundled
     # libgfortran/libquadmath, which sit next to it without an rpath
@@ -294,7 +339,7 @@ def load_reference(path):
             except OSError:
                 pass
     lib = C.CDLL(path, mode=C.RTLD_LOCAL)
-    _declare(lib, ours=False)
+    _declare(lib, ours=False, cone=ScsConeSpectral if spectral else ScsCone)
     return lib
 
 

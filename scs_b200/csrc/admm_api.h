@@ -99,6 +99,23 @@ void b200_cpsd_set_err(B200CpsdCones *c, int *d_err);
 void *b200_solver_acquire(void);
 void b200_solver_release(void *handle);
 int b200_cones_set_complex_psd(B200Cones *c, int cssize, const int *h_cs, int n_triples);
+/* nuclear-norm (nuc_m x nuc_n), l1-norm (ell1) and sum-of-largest-eigenvalues (sl_n, sl_k) cones of the spectral
+ * build: the LAST rows of the cone product, in that order (kernels/cones_spectral.cu; reference cones.c:1462-1490).
+ * Must be called before b200_cones_set_triples / b200_cones_set_complex_psd. 0 on success (also when all are empty). */
+int b200_cones_set_spectral(B200Cones *c, int nucsize, const int *h_nuc_m, const int *h_nuc_n, int ell1_size,
+                            const int *h_ell1, int sl_size, const int *h_sl_n, const int *h_sl_k);
+typedef struct B200SpecCones B200SpecCones;
+B200SpecCones *b200_spec_create(int nucsize, const int *h_nuc_m, const int *h_nuc_n, int ell1_size, const int *h_ell1,
+                                int sl_size, const int *h_sl_n, const int *h_sl_k, long long first_row, int *d_err);
+int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_s, const double *d_ry);
+void b200_spec_destroy(B200SpecCones *c);
+/* shared with kernels/cones_spectral.cu (kernels/cones.cu): the sqrt2-scaled unpack of packed lower triangles, and
+ * the DMMA contraction V diag(w) V' with signed weights (mode 1, packed lower output) or its rectangular block
+ * (mode 2, dense rows x cols output from V of order ld = rows + cols) */
+void b200_psd_info_or(int count, const int *d_info, int *d_err);
+void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_x, double *d_mats);
+void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off, const double *d_mats,
+                             const double *d_w, double *d_x, const double *d_s, const double *d_ry);
 void b200_cones_destroy(B200Cones *c);
 /* Projects the box/SOC/PSD rows. On entry d_x (length m, the y block of u) holds
  * x = -r .* u on those rows and d_s holds the saved u (k_cone_pre); on exit

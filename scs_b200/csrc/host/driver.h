@@ -27,6 +27,19 @@
 #define MAX_BOX_VAL (1e15)
 #define DIV_EPS_TOL (1E-18)
 #define SAFEDIV_POS(X, Y) ((Y) < DIV_EPS_TOL ? ((X) / DIV_EPS_TOL) : (X) / (Y))
+
+#ifdef USE_SPECTRAL_CONES
+/* rows of the spectral cones (reference cones.c:435-443); a log-det cone of order d has d(d+1)/2 + 2 */
+static inline long long b200_spectral_rows(const ScsCone *k) {
+  long long rows = 0;
+  int i;
+  for (i = 0; i < k->dsize; ++i) rows += (long long)k->d[i] * (k->d[i] + 1) / 2 + 2;
+  for (i = 0; i < k->nucsize; ++i) rows += (long long)k->nuc_m[i] * k->nuc_n[i] + 1;
+  for (i = 0; i < k->ell1_size; ++i) rows += (long long)k->ell1[i] + 1;
+  for (i = 0; i < k->sl_size; ++i) rows += (long long)k->sl_n[i] * (k->sl_n[i] + 1) / 2 + 1;
+  return rows;
+}
+#endif
 #ifndef MAX
 #define MAX(a, b) (((a) > (b)) ? (a) : (b))
 #endif

@@ -28,6 +28,19 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float
   for (j = 0; j < k->ssize; ++j) dims += ((long long)k->s[j] * (k->s[j] + 1)) / 2;
   for (j = 0; j < k->cssize; ++j) dims += (long long)k->cs[j] * k->cs[j];
   dims += 3LL * ((long long)k->ep + k->ed + k->psize);
+#ifdef USE_SPECTRAL_CONES
+  if (k->dsize != 0 || k->nucsize < 0 || k->ell1_size < 0 || k->sl_size < 0) return SCS_NULL; /* no log-det cones */
+  if ((k->nucsize > 0 && (!k->nuc_m || !k->nuc_n)) || (k->ell1_size > 0 && !k->ell1) ||
+      (k->sl_size > 0 && (!k->sl_n || !k->sl_k)))
+    return SCS_NULL;
+  for (j = 0; j < k->nucsize; ++j)
+    if (k->nuc_m[j] < 1 || k->nuc_n[j] < 1 || k->nuc_n[j] > k->nuc_m[j]) return SCS_NULL;
+  for (j = 0; j < k->ell1_size; ++j)
+    if (k->ell1[j] < 1) return SCS_NULL;
+  for (j = 0; j < k->sl_size; ++j)
+    if (k->sl_k[j] <= 0 || k->sl_k[j] >= k->sl_n[j]) return SCS_NULL;
+  dims += b200_spectral_rows(k);
+#endif
   if (dims != m) {
     fprintf(stderr, "scs_b200: cone dims %lld != m %d\n", dims, m);
     return SCS_NULL;
@@ -57,6 +70,11 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float
   free(bu);
   bl = bu = SCS_NULL;
   if (!c->cones) goto fail;
+#ifdef USE_SPECTRAL_CONES
+  if (b200_cones_set_spectral(c->cones, k->nucsize, k->nuc_m, k->nuc_n, k->ell1_size, k->ell1, k->sl_size, k->sl_n,
+                              k->sl_k) != 0)
+    goto fail;
+#endif
   if (b200_cones_set_triples(c->cones, k->ep, k->ed, k->psize, k->p) != 0) goto fail;
   if (b200_cones_set_complex_psd(c->cones, k->cssize, k->cs, k->ep + k->ed + k->psize) != 0) goto fail;
   c->d_x = (double *)b200_malloc((size_t)m * 8);

@@ -16,6 +16,8 @@
  *            acceleration_relaxation; I adaptive_scale       (older files: I adaptive_scale only)
  *   optional extension block: u32 magic "SCSE", u32 1; I cssize, cs[]; I dsize, d[]; I nucsize, nuc_m[],
  *            nuc_n[]; I ell1_size, ell1[]; I sl_size, sl_n[], sl_k[]; F time_limit_secs
+ * The default build skips the spectral arrays on reading and writes them empty; the spectral build
+ * (USE_SPECTRAL_CONES) reads them into ScsCone and writes them as the reference's spectral build does.
  * The writer always emits I = 4 bytes and the version string of the API it implements ("3.2.11");
  * the reader accepts I = 4 or 8 (values must fit an int) and both settings layouts. */
 #include "driver.h"
@@ -90,6 +92,7 @@ static double *get_f_array(Stream *s, int n) {
   get_raw(s, v, (size_t)n * sizeof(double));
   return v;
 }
+#ifndef USE_SPECTRAL_CONES
 static void skip_i_array(Stream *s, int n) {
   char buf[4096];
   uint64_t left;
@@ -102,6 +105,7 @@ static void skip_i_array(Stream *s, int n) {
     left -= chunk;
   }
 }
+#endif
 
 /* ------------------------------------------------------------------ writer */
 static void put_matrix(Stream *s, const ScsMatrix *M) {
@@ -156,7 +160,14 @@ scs_int scs_b200_write_data(const char *filename, const ScsData *d, const ScsCon
   /* extension block: complex PSD orders, four empty spectral-cone groups, the time limit */
   put_raw(&s, ext, sizeof(ext));
   put_i(&s, k->cssize); put_is(&s, k->cs, k->cssize);
+#ifdef USE_SPECTRAL_CONES
+  put_i(&s, k->dsize); put_is(&s, k->d, k->dsize);
+  put_i(&s, k->nucsize); put_is(&s, k->nuc_m, k->nucsize); put_is(&s, k->nuc_n, k->nucsize);
+  put_i(&s, k->ell1_size); put_is(&s, k->ell1, k->ell1_size);
+  put_i(&s, k->sl_size); put_is(&s, k->sl_n, k->sl_size); put_is(&s, k->sl_k, k->sl_size);
+#else
   put_i(&s, 0); put_i(&s, 0); put_i(&s, 0); put_i(&s, 0);
+#endif
   put_f(&s, stgs->time_limit_secs);
   if (fclose(s.f) != 0) s.bad = 1;
   if (s.bad) printf("Error: failed writing SCS data to %s\n", filename);
@@ -189,7 +200,11 @@ void scs_b200_free_data(ScsData *d, ScsCone *k, ScsSettings *stgs) {
     free(d->b); free(d->c); free(d);
   }
   if (k) {
-    free(k->bu); free(k->bl); free(k->q); free(k->s); free(k->cs); free(k->p); free(k);
+    free(k->bu); free(k->bl); free(k->q); free(k->s); free(k->cs); free(k->p);
+#ifdef USE_SPECTRAL_CONES
+    free(k->d); free(k->nuc_m); free(k->nuc_n); free(k->ell1); free(k->sl_n); free(k->sl_k);
+#endif
+    free(k);
   }
   free(stgs);
 }
@@ -267,10 +282,18 @@ scs_int scs_b200_read_data(const char *filename, ScsData **d_out, ScsCone **k_ou
       get_raw(&s, &ev, sizeof(ev));
       if (ev != 1u) { printf("Error: unsupported SCS file extension version %u\n", ev); s.bad = 1; }
       k->cssize = get_i(&s); k->cs = get_i_array(&s, k->cssize);
+#ifdef USE_SPECTRAL_CONES /* the spectral arrays (reference rw.c:540-557) */
+      (void)cnt;
+      k->dsize = get_i(&s); k->d = get_i_array(&s, k->dsize);
+      k->nucsize = get_i(&s); k->nuc_m = get_i_array(&s, k->nucsize); k->nuc_n = get_i_array(&s, k->nucsize);
+      k->ell1_size = get_i(&s); k->ell1 = get_i_array(&s, k->ell1_size);
+      k->sl_size = get_i(&s); k->sl_n = get_i_array(&s, k->sl_size); k->sl_k = get_i_array(&s, k->sl_size);
+#else
       cnt = get_i(&s); skip_i_array(&s, cnt);                              /* log-det cones */
       cnt = get_i(&s); skip_i_array(&s, cnt); skip_i_array(&s, cnt);       /* nuclear-norm cones */
       cnt = get_i(&s); skip_i_array(&s, cnt);                              /* ell-1 cones */
       cnt = get_i(&s); skip_i_array(&s, cnt); skip_i_array(&s, cnt);       /* sum-of-largest cones */
+#endif
       st->time_limit_secs = get_f(&s);
     } else if (got != 0 && got != sizeof(magic)) {
       printf("Error: incomplete extension header in %s\n", filename);

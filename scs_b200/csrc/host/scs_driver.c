@@ -144,11 +144,42 @@ static int validate_cones(const ScsData *d, const ScsCone *k) {
     for (i = 0; i < k->psize; ++i)
       if (!isfinite(k->p[i]) || k->p[i] < -1 || k->p[i] > 1) { printf("power cone error, values must be in [-1,1]\n"); return -1; }
   }
+#ifdef USE_SPECTRAL_CONES /* reference cones.c:690-754 */
+  if (k->dsize < 0 || (k->dsize > 0 && !k->d)) { printf("logdet cone dimension error\n"); return -1; }
+  for (i = 0; i < k->dsize; ++i)
+    if (k->d[i] < 1) { printf("logdet cone dimension error\n"); return -1; }
+  if (k->nucsize < 0) { printf("nuclear cone dimension error\n"); return -1; }
+  if (k->nucsize > 0 && (!k->nuc_m || !k->nuc_n)) { printf("nuclear cone arrays missing\n"); return -1; }
+  for (i = 0; i < k->nucsize; ++i)
+    if (k->nuc_m[i] < 1 || k->nuc_n[i] < 1 || k->nuc_n[i] > k->nuc_m[i]) {
+      printf("nuclear norm cone dimension error\n");
+      return -1;
+    }
+  if (k->ell1_size < 0) { printf("ell1 cone dimension error\n"); return -1; }
+  if (k->ell1_size > 0 && !k->ell1) { printf("ell1 cone array missing\n"); return -1; }
+  for (i = 0; i < k->ell1_size; ++i)
+    if (k->ell1[i] < 1) { printf("ell1 cone dimension error\n"); return -1; }
+  if (k->sl_size < 0) { printf("sum-of-largest-eigenvalues cone dimension error\n"); return -1; }
+  if (k->sl_size > 0 && (!k->sl_n || !k->sl_k)) { printf("sum-of-largest-eigenvalues cone arrays missing\n"); return -1; }
+  for (i = 0; i < k->sl_size; ++i)
+    if (k->sl_k[i] >= k->sl_n[i] || k->sl_k[i] <= 0) {
+      printf("sum-of-largest-eigenvalues cone dimension error\n");
+      return -1;
+    }
+  if (k->dsize > 0) { /* never dropped silently: its rows would go unprojected */
+    printf("log-det cones (dsize = %i) are not supported: this library projects the nuclear-norm, l1-norm and "
+           "sum-of-largest-eigenvalues spectral cones only\n", k->dsize);
+    return -1;
+  }
+#endif
   dims = (long long)k->z + k->l + k->bsize;
   for (i = 0; i < k->qsize; ++i) dims += k->q[i];
   for (i = 0; i < k->ssize; ++i) dims += sd_size(k->s[i]);
   for (i = 0; i < k->cssize; ++i) dims += (long long)k->cs[i] * k->cs[i];
   dims += 3LL * ((long long)k->ep + k->ed + k->psize);
+#ifdef USE_SPECTRAL_CONES
+  dims += b200_spectral_rows(k);
+#endif
   if (dims != d->m) {
     printf("Error: Cone dims %li != rows in A %li\n", (long)dims, (long)d->m);
     return -1;
@@ -259,7 +290,13 @@ void scs_finish(ScsWork *w) {
   if (w->d) {
     free_matrix(w->d->A); free_matrix(w->d->P); free(w->d->b); free(w->d->c); free(w->d);
   }
-  if (w->k) { free(w->k->bu); free(w->k->bl); free(w->k->q); free(w->k->s); free(w->k->p); free(w->k->cs); free(w->k); }
+  if (w->k) {
+    free(w->k->bu); free(w->k->bl); free(w->k->q); free(w->k->s); free(w->k->p); free(w->k->cs);
+#ifdef USE_SPECTRAL_CONES
+    free(w->k->d); free(w->k->nuc_m); free(w->k->nuc_n); free(w->k->ell1); free(w->k->sl_n); free(w->k->sl_k);
+#endif
+    free(w->k);
+  }
   free(w->stgs);
   free(w);
   init_mark("finish: host copies", &t_mark);
@@ -277,13 +314,23 @@ static int set_cone_boundaries(ScsWork *w) {
   const ScsCone *k = w->k;
   int i, count = 0;
   int total = k->qsize + k->ssize + k->cssize + k->ep + k->ed + k->psize;
-  int *b = (int *)calloc((size_t)total + 1, sizeof(int));
+  int *b;
+#ifdef USE_SPECTRAL_CONES
+  total += k->dsize + k->nucsize + k->ell1_size + k->sl_size;
+#endif
+  b = (int *)calloc((size_t)total + 1, sizeof(int));
   if (!b) return -1;
   b[count++] = k->z + k->l + k->bsize;
   for (i = 0; i < k->qsize; ++i) b[count++] = k->q[i];
   for (i = 0; i < k->ssize; ++i) b[count++] = sd_size(k->s[i]);
   for (i = 0; i < k->cssize; ++i) b[count++] = k->cs[i] * k->cs[i];
   for (i = 0; i < k->ep + k->ed + k->psize; ++i) b[count++] = 3; /* every triple shares one D (cones.c:405-408) */
+#ifdef USE_SPECTRAL_CONES /* one D value per spectral cone (cones.c:411-419) */
+  for (i = 0; i < k->dsize; ++i) b[count++] = sd_size(k->d[i]) + 2;
+  for (i = 0; i < k->nucsize; ++i) b[count++] = k->nuc_m[i] * k->nuc_n[i] + 1;
+  for (i = 0; i < k->ell1_size; ++i) b[count++] = k->ell1[i] + 1;
+  for (i = 0; i < k->sl_size; ++i) b[count++] = sd_size(k->sl_n[i]) + 1;
+#endif
   w->cone_boundaries = b;
   w->cone_boundaries_len = total + 1;
   return 0;
@@ -394,6 +441,9 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   *w->k = *k;
   w->k->bu = w->k->bl = SCS_NULL; w->k->q = SCS_NULL; w->k->s = SCS_NULL;
   w->k->cs = SCS_NULL; w->k->p = SCS_NULL;
+#ifdef USE_SPECTRAL_CONES
+  w->k->d = SCS_NULL; w->k->nuc_m = w->k->nuc_n = SCS_NULL; w->k->ell1 = SCS_NULL; w->k->sl_n = w->k->sl_k = SCS_NULL;
+#endif
   if (k->bsize > 1) {
     w->k->bu = (double *)dup_mem(k->bu, (size_t)(k->bsize - 1) * 8);
     w->k->bl = (double *)dup_mem(k->bl, (size_t)(k->bsize - 1) * 8);
@@ -403,6 +453,19 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   if (k->psize > 0) { w->k->p = (double *)dup_mem(k->p, (size_t)k->psize * 8); if (!w->k->p) goto fail; }
   if (k->cssize > 0) { w->k->cs = (int *)dup_mem(k->cs, (size_t)k->cssize * 4); if (!w->k->cs) goto fail; }
   if (k->ssize > 0) { w->k->s = (int *)dup_mem(k->s, (size_t)k->ssize * 4); if (!w->k->s) goto fail; }
+#ifdef USE_SPECTRAL_CONES
+  if (k->nucsize > 0) {
+    w->k->nuc_m = (int *)dup_mem(k->nuc_m, (size_t)k->nucsize * 4);
+    w->k->nuc_n = (int *)dup_mem(k->nuc_n, (size_t)k->nucsize * 4);
+    if (!w->k->nuc_m || !w->k->nuc_n) goto fail;
+  }
+  if (k->ell1_size > 0) { w->k->ell1 = (int *)dup_mem(k->ell1, (size_t)k->ell1_size * 4); if (!w->k->ell1) goto fail; }
+  if (k->sl_size > 0) {
+    w->k->sl_n = (int *)dup_mem(k->sl_n, (size_t)k->sl_size * 4);
+    w->k->sl_k = (int *)dup_mem(k->sl_k, (size_t)k->sl_size * 4);
+    if (!w->k->sl_n || !w->k->sl_k) goto fail;
+  }
+#endif
   *w->stgs = *stgs;
   w->stgs->write_data_filename = SCS_NULL;
   w->stgs->log_csv_filename = SCS_NULL;
@@ -513,6 +576,13 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
 
   w->cones = b200_cones_create(m, w->k->z, w->k->l, w->k->bsize, w->k->bl, w->k->bu, w->k->qsize,
                                w->k->q, w->k->ssize, w->k->s);
+#ifdef USE_SPECTRAL_CONES
+  if (w->cones && b200_cones_set_spectral(w->cones, w->k->nucsize, w->k->nuc_m, w->k->nuc_n, w->k->ell1_size,
+                                          w->k->ell1, w->k->sl_size, w->k->sl_n, w->k->sl_k) != 0) {
+    printf("ERROR: init_cone failure (spectral cones)\n");
+    goto fail;
+  }
+#endif
   if (!w->cones || b200_cones_set_triples(w->cones, w->k->ep, w->k->ed, w->k->psize, w->k->p) != 0 ||
       b200_cones_set_complex_psd(w->cones, w->k->cssize, w->k->cs, w->k->ep + w->k->ed + w->k->psize) != 0) {
     printf("ERROR: init_cone failure\n");

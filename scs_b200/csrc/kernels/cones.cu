@@ -78,6 +78,8 @@ struct B200Cones {
   long long tri_off;  // first row of the exponential triples
   double *d_pow;      // power cone parameters (sign = primal / dual), psize
   B200CpsdCones *cpsd;  // complex PSD blocks (kernels/cones_complex.cu), or NULL
+  B200SpecCones *spec;  // nuclear / l1 / sum-of-largest cones (kernels/cones_spectral.cu), or NULL
+  long long spec_rows;  // rows of the spectral cones: the last rows of the m-vector
   // sticky device flag: OR of every per-matrix `info` the batched eigen-solver has returned (reference
   // cones.c:1048-1052 propagates a failed syevr as "error in project_cones"); read by b200_cones_check
   int *d_err;
@@ -342,23 +344,33 @@ k_psd_reconstruct(int k, int count, const int *__restrict__ off, const double *_
 // t = lane & 3. The shared tiles are padded to a row stride of 36 doubles: the 16 lanes of a half-warp then read 16
 // distinct 8-byte banks. Eigenvalues arrive in ascending order (syevd): column chunks whose largest eigenvalue is
 // <= 0 contribute nothing and are skipped.
+//
+// The spectral cones (kernels/cones_spectral.cu) run the same contraction with other weights and outputs:
+//  REC_PSD     weights max(lambda, 0), packed lower triangle of V diag(w) V' (the PSD cone);
+//  REC_SIGNED  weights of either sign, every column chunk contributes (sum-of-largest-eigenvalues cone);
+//  REC_RECT    V of order ld = rows + cols, output the dense column-major rows x cols block
+//              V[0:rows, :] diag(w) V[rows:ld, :]' (nuclear-norm cone, from the symmetric embedding); only the
+//              last `cols` columns of V carry weight, so the chunk loop starts at the chunk holding column ld - cols.
 #define PTD 36
+enum { REC_PSD = 0, REC_SIGNED = 1, REC_RECT = 2 };
 __device__ __forceinline__ void dmma_m8n8k4(double &c0, double &c1, double a, double b) {
   asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
                : "+d"(c0), "+d"(c1)
                : "d"(a), "d"(b));
 }
+template <int MODE>
 __global__ void __launch_bounds__(128)
-k_psd_reconstruct_dmma(int k, int count, const int *__restrict__ off, const double *__restrict__ mats,
-                       const double *__restrict__ evals, double *__restrict__ x, const double *sv,
-                       const double *ry) {
-  __shared__ double sA[PT][PTD];  // V[i0+ii, c0+cc] * max(lambda_c, 0)
-  __shared__ double sB[PT][PTD];  // V[j0+jj, c0+cc]
+k_reconstruct_dmma(int ld, int rows, int cols, int count, const int *__restrict__ off,
+                   const double *__restrict__ mats, const double *__restrict__ evals, double *__restrict__ x,
+                   const double *sv, const double *ry) {
+  __shared__ double sA[PT][PTD];  // V[i0+ii, c0+cc] * w_c
+  __shared__ double sB[PT][PTD];  // V[bro+j0+jj, c0+cc]
   const int b = blockIdx.z;
   const int ti = blockIdx.y, tj = blockIdx.x;
-  if (tj > ti) return;
-  const double *V = mats + (size_t)b * k * k;
-  const double *lam = evals + (size_t)b * k;
+  if (MODE != REC_RECT && tj > ti) return;
+  const double *V = mats + (size_t)b * ld * ld;
+  const double *lam = evals + (size_t)b * ld;
+  const int bro = (MODE == REC_RECT) ? rows : 0;  // first row of the right factor inside V
   const int i0 = ti * PT, j0 = tj * PT;
   const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
   const int g = lane >> 2, t = lane & 3;
@@ -368,18 +380,21 @@ k_psd_reconstruct_dmma(int k, int count, const int *__restrict__ off, const doub
   for (int a = 0; a < 2; ++a)
 #pragma unroll
     for (int c = 0; c < 2; ++c) acc[a][c][0] = acc[a][c][1] = 0.0;
-  for (int c0 = 0; c0 < k; c0 += PT) {
-    const int clast = (c0 + PT - 1 < k) ? c0 + PT - 1 : k - 1;
-    if (lam[clast] <= 0.0) continue;  // block-uniform: nothing positive in this chunk
+  const int cstart = (MODE == REC_RECT) ? ((ld - cols) / PT) * PT : 0;
+  for (int c0 = cstart; c0 < ld; c0 += PT) {
+    if (MODE == REC_PSD) {
+      const int clast = (c0 + PT - 1 < ld) ? c0 + PT - 1 : ld - 1;
+      if (lam[clast] <= 0.0) continue;  // block-uniform: nothing positive in this chunk
+    }
     for (int e = threadIdx.x; e < PT * PT; e += blockDim.x) {
       const int rr = e % PT, cc = e / PT;
       const int c = c0 + cc;
       double la = 0.0, va = 0.0, vb = 0.0;
-      if (c < k) {
+      if (c < ld) {
         la = lam[c];
-        la = la > 0.0 ? la : 0.0;
-        if (i0 + rr < k) va = V[(size_t)(i0 + rr) + (size_t)c * k];
-        if (j0 + rr < k) vb = V[(size_t)(j0 + rr) + (size_t)c * k];
+        if (MODE == REC_PSD) la = la > 0.0 ? la : 0.0;
+        if (i0 + rr < rows) va = V[(size_t)(i0 + rr) + (size_t)c * ld];
+        if (j0 + rr < cols) vb = V[(size_t)(bro + j0 + rr) + (size_t)c * ld];
       }
       sA[rr][cc] = va * la;
       sB[rr][cc] = vb;
@@ -405,12 +420,35 @@ k_psd_reconstruct_dmma(int k, int count, const int *__restrict__ off, const doub
 #pragma unroll
       for (int q = 0; q < 2; ++q) {
         const int i = i0 + wr + 8 * a + g, j = j0 + wc + 8 * c + 2 * t + q;
-        if (i < k && j < k && i >= j) {
+        if (MODE == REC_RECT) {
+          if (i < rows && j < cols) {
+            const long long row = base + i + (long long)j * rows;
+            x[row] = post_scale(acc[a][c][q], ry, sv, row);
+          }
+        } else if (i < rows && j < rows && i >= j) {
           const double val = (i == j) ? acc[a][c][q] * inv_sqrt2 : acc[a][c][q];
-          const long long row = base + packed_idx(i, j, k);
+          const long long row = base + packed_idx(i, j, rows);
           x[row] = post_scale(val, ry, sv, row);
         }
       }
+}
+// Launchers for kernels/cones_spectral.cu (count blocks; off[b] = first row of block b's matrix)
+extern "C" void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_x, double *d_mats) {
+  dim3 ug((k * k + 255) / 256, count);
+  k_psd_unpack<<<ug, 256, 0, (cudaStream_t)b200_stream()>>>(k, count, d_off, d_x, d_mats);
+  b200_count_launch(1);
+}
+extern "C" void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off,
+                                        const double *d_mats, const double *d_w, double *d_x, const double *d_s,
+                                        const double *d_ry) {
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  const int ntr = (rows + PT - 1) / PT, ntc = (cols + PT - 1) / PT;
+  dim3 rg(ntc, ntr, count);
+  if (mode == REC_RECT)
+    k_reconstruct_dmma<REC_RECT><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
+  else
+    k_reconstruct_dmma<REC_SIGNED><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
+  b200_count_launch(1);
 }
 __global__ void k_psd_order1(int count, const int *__restrict__ off, double *__restrict__ x,
                              const double *sv, const double *ry) {
@@ -658,6 +696,7 @@ extern "C" void b200_cones_destroy(B200Cones *c) {
   b200_free(c->d_pow);
   b200_free(c->d_err);
   b200_cpsd_destroy(c->cpsd);
+  b200_spec_destroy(c->spec);
   if (c->groups) {
     for (auto &g : *c->groups) {
       b200_free(g.d_off); b200_free(g.d_mats); b200_free(g.d_evals); b200_free(g.d_info);
@@ -672,11 +711,32 @@ extern "C" void b200_cones_destroy(B200Cones *c) {
 
 extern "C" double *b200_cones_scratch(B200Cones *c) { return c->d_scratch; }
 
-// exponential / power cones occupy the LAST 3 (ep + ed + psize) rows (scs.h cone order; the complex
-// PSD cone that would sit between PSD and exp is not supported)
+// nuclear-norm, l1-norm and sum-of-largest-eigenvalues cones occupy the last rows, in that order (reference
+// cones.c:1462-1490). Called before b200_cones_set_triples / _set_complex_psd, whose rows sit just before them.
+extern "C" int b200_cones_set_spectral(B200Cones *c, int nucsize, const int *h_nuc_m, const int *h_nuc_n,
+                                       int ell1_size, const int *h_ell1, int sl_size, const int *h_sl_n,
+                                       const int *h_sl_k) {
+  long long rows = 0;
+  for (int i = 0; i < nucsize; ++i) rows += 1 + (long long)h_nuc_m[i] * h_nuc_n[i];
+  for (int i = 0; i < ell1_size; ++i) rows += 1 + (long long)h_ell1[i];
+  for (int i = 0; i < sl_size; ++i) rows += 1 + (long long)h_sl_n[i] * (h_sl_n[i] + 1) / 2;
+  if (rows == 0) return 0;
+  if (rows > c->m) return -1;
+  if (!c->d_err) {
+    c->d_err = (int *)b200_malloc(64);
+    if (!c->d_err || b200_memset0(c->d_err, 64) != 0) return -1;
+  }
+  c->spec_rows = rows;
+  c->spec = b200_spec_create(nucsize, h_nuc_m, h_nuc_n, ell1_size, h_ell1, sl_size, h_sl_n, h_sl_k,
+                             (long long)c->m - rows, c->d_err);
+  return c->spec ? 0 : -1;
+}
+
+// exponential / power cones occupy the 3 (ep + ed + psize) rows before the spectral cones, i.e. the LAST rows when
+// there are none (scs.h cone order)
 extern "C" int b200_cones_set_triples(B200Cones *c, int ep, int ed, int psize, const double *h_p) {
   c->n_ep = ep; c->n_ed = ed; c->n_pow = psize;
-  c->tri_off = (long long)c->m - 3LL * ((long long)ep + ed + psize);
+  c->tri_off = (long long)c->m - c->spec_rows - 3LL * ((long long)ep + ed + psize);
   if (c->tri_off < 0) return -1;
   if (psize > 0) {
     c->d_pow = (double *)b200_malloc((size_t)psize * 8);
@@ -690,7 +750,7 @@ extern "C" int b200_cones_set_complex_psd(B200Cones *c, int cssize, const int *h
   long long rows = 0;
   for (int i = 0; i < cssize; ++i) rows += (long long)h_cs[i] * h_cs[i];
   if (rows == 0) return 0;
-  const long long first = (long long)c->m - 3LL * n_triples - rows;
+  const long long first = (long long)c->m - c->spec_rows - 3LL * n_triples - rows;
   if (first < 0) return -1;
   if (!c->d_err) {
     c->d_err = (int *)b200_malloc(64);
@@ -763,7 +823,8 @@ extern "C" int b200_cones_project_rest(B200Cones *c, double *d_x, const double *
       if (psd_fma)
         k_psd_reconstruct<<<rg, PT * 8, 0, st>>>(k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
       else
-        k_psd_reconstruct_dmma<<<rg, 128, 0, st>>>(k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
+        k_reconstruct_dmma<REC_PSD><<<rg, 128, 0, st>>>(k, k, k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s,
+                                                         d_ry);
       b200_count_launch(1);
     }
   }
@@ -774,6 +835,8 @@ extern "C" int b200_cones_project_rest(B200Cones *c, double *d_x, const double *
     if (b200_cone_triples_project(c->n_ep, c->n_ed, c->n_pow, c->tri_off, c->d_pow, d_x, d_s, d_ry) != 0)
       return -1;
   }
+  // ---- nuclear / l1 / sum-of-largest
+  if (c->spec && b200_spec_project(c->spec, d_x, d_s, d_ry) != 0) return -1;
   CUDA_OK(cudaGetLastError());
   return 0;
 }
@@ -784,8 +847,8 @@ extern "C" int b200_cones_check(B200Cones *c) {
   int h = 0;
   if (b200_d2h(&h, c->d_err, sizeof(int)) != 0 || b200_sync() != 0) return -1;
   if (h != 0) {
-    b200_set_error("batched syevd reported a failure (info != 0) in the PSD projection", cudaErrorUnknown, __FILE__,
-                   __LINE__);
+    b200_set_error("batched syevd reported a failure (info != 0) in a PSD or spectral cone projection",
+                   cudaErrorUnknown, __FILE__, __LINE__);
     return -1;
   }
   return 0;
