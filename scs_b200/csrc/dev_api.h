@@ -46,11 +46,13 @@ double b200_section_ms(int section);
  * transpose At gives the CSR of A (reference cpu/indirect/private.c:7-46). */
 typedef struct B200Spmv B200Spmv;
 
+/* an operator from a host CSR: the arrays are uploaded and the operator is built on the device like every other
+ * (b200_spmv_create_dev, kernels/spmv.cu); nrows and nnz may be 0. NULL on failure */
 B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr, const int *h_colidx,
                            const double *h_vals);
 void b200_spmv_destroy(B200Spmv *M);
-/* both resident orientations built ON THE DEVICE from the host CSC of A (kernels/setup.cu): 0 ok, 1 declined (use the
- * host builders: SCS_B200_HOST_SETUP=1, an empty A, sizes beyond the device path), < 0 CUDA error */
+/* both resident orientations built ON THE DEVICE from the host CSC of A (kernels/setup.cu); m, n or nnz may be 0:
+ * 0 ok, < 0 error */
 int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax, B200Spmv **A_out,
                             B200Spmv **At_out);
 int b200_spmv_nrows(const B200Spmv *M);

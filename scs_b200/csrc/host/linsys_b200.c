@@ -21,13 +21,9 @@
 
 const char *scs_get_lin_sys_method(void) { return "sparse-indirect-b200-cuda"; }
 
-/* counting-sort transpose of a CSC matrix (m x n) into the CSC of its transpose
- * (= CSR of the original). Entries of each output column keep ascending source
- * column order, exactly like reference private.c:7-46, so that the per-row
- * summation order of A x matches the reference's accum_by_atrans(At, ...). */
-/* Host threads for the setup-time passes over nnz (transpose here, the SpMV plan in kernels/spmv.cu):
+/* Host threads for the setup-time passes over nnz of the multi-GPU path (row counts, row-block cut, below):
  * SCS_B200_HOST_THREADS, else min(16, online CPUs); 1 for small inputs. */
-int b200_host_threads(long long work_items) {
+static int b200_host_threads(long long work_items) {
   const char *e = getenv("SCS_B200_HOST_THREADS");
   long t = e ? atol(e) : sysconf(_SC_NPROCESSORS_ONLN);
   if (!e && t > 16) t = 16;
@@ -35,118 +31,6 @@ int b200_host_threads(long long work_items) {
   if (t < 1) t = 1;
   if (t > 64) t = 64;
   return (int)t;
-}
-
-/* The transpose is a stable counting sort. Parallel version: the OUTPUT rows are split into T contiguous
- * ranges; every thread scans the whole input in column order and handles only the entries whose row falls
- * in its range, so writes never collide, no atomics are needed and the result is identical to the serial
- * loop (entries of an output row keep ascending source-column order). The extra cost is T sequential reads
- * of the index array, which is cheap next to the random writes that dominate the serial version. */
-typedef struct {
-  int m, n, r0, r1;
-  const int *Ap, *Ai;
-  const double *Ax;
-  int *cursor, *Ci;
-  double *Cx;
-  int phase; /* 0: count, 1: fill */
-} TrJob;
-
-static void *tr_worker(void *arg) {
-  TrJob *jb = (TrJob *)arg;
-  const int r0 = jb->r0, r1 = jb->r1;
-  const int *Ai = jb->Ai;
-  if (jb->phase == 0) {
-    /* count: this thread's SLICE OF THE INPUT [r0, r1) (entry indices), relaxed atomic increments --
-     * integer counts do not depend on the order, so the result is still deterministic */
-    long long k;
-    int *cnt = jb->cursor;
-    for (k = r0; k < r1; ++k) __atomic_fetch_add(&cnt[Ai[k]], 1, __ATOMIC_RELAXED);
-  } else {
-    int j, k;
-    int *z = jb->cursor;
-    for (j = 0; j < jb->n; ++j) {
-      for (k = jb->Ap[j]; k < jb->Ap[j + 1]; ++k) {
-        const int r = Ai[k];
-        if (r >= r0 && r < r1) {
-          const int q = z[r]++;
-          jb->Ci[q] = j;
-          jb->Cx[q] = jb->Ax[k];
-        }
-      }
-    }
-  }
-  return NULL;
-}
-
-static void tr_run(TrJob *jobs, int T) {
-  pthread_t th[64];
-  int t, started = 0;
-  for (t = 1; t < T; ++t) {
-    if (pthread_create(&th[t], NULL, tr_worker, &jobs[t]) != 0) break;
-    started = t;
-  }
-  tr_worker(&jobs[0]);
-  for (t = started + 1; t < T; ++t) tr_worker(&jobs[t]); /* threads that could not be created: run inline */
-  for (t = 1; t <= started; ++t) pthread_join(th[t], NULL);
-}
-
-int scs_b200_transpose_csc(int m, int n, const int *Ap, const int *Ai, const double *Ax, int **Cp_out,
-                           int **Ci_out, double **Cx_out) {
-  const int nnz = Ap[n];
-  int *Cp = (int *)calloc((size_t)m + 1, sizeof(int));
-  int *Ci = (int *)malloc(((size_t)nnz + 1) * sizeof(int));
-  double *Cx = (double *)malloc(((size_t)nnz + 1) * sizeof(double));
-  int *z = (int *)calloc((size_t)m + 1, sizeof(int));
-  TrJob jobs[64];
-  int i, t;
-  int T = b200_host_threads(nnz);
-  if (T > m) T = m > 0 ? m : 1;
-  if (!Cp || !Ci || !Cx || !z) {
-    free(Cp); free(Ci); free(Cx); free(z);
-    return -1;
-  }
-  for (t = 0; t < T; ++t) {
-    jobs[t].m = m; jobs[t].n = n; jobs[t].Ap = Ap; jobs[t].Ai = Ai; jobs[t].Ax = Ax;
-    jobs[t].cursor = z; jobs[t].Ci = Ci; jobs[t].Cx = Cx;
-  }
-  /* count: equal slices of the input entries */
-  for (t = 0; t < T; ++t) {
-    jobs[t].phase = 0;
-    jobs[t].r0 = (int)((long long)nnz * t / T);
-    jobs[t].r1 = (int)((long long)nnz * (t + 1) / T);
-  }
-  tr_run(jobs, T);
-  Cp[0] = 0;
-  for (i = 0; i < m; ++i) Cp[i + 1] = Cp[i] + z[i];
-  for (i = 0; i < m; ++i) z[i] = Cp[i];
-  /* fill: row ranges balanced by their number of entries */
-  {
-    int r = 0;
-    for (t = 0; t < T; ++t) {
-      const long long target = (long long)nnz * (t + 1) / T;
-      jobs[t].phase = 1;
-      jobs[t].r0 = r;
-      if (t == T - 1) {
-        r = m;
-      } else {
-        int lo = r, hi = m; /* first row index whose prefix reaches the target */
-        while (lo < hi) {
-          const int mid = lo + (hi - lo) / 2;
-          if (Cp[mid] < target) lo = mid + 1; else hi = mid;
-        }
-        r = lo;
-      }
-      jobs[t].r1 = r;
-    }
-  }
-  tr_run(jobs, T);
-  free(z);
-  *Cp_out = Cp; *Ci_out = Ci; *Cx_out = Cx;
-  return 0;
-}
-static int transpose_csc(int m, int n, const int *Ap, const int *Ai, const double *Ax, int **Cp_out,
-                         int **Ci_out, double **Cx_out) {
-  return scs_b200_transpose_csc(m, n, Ap, Ai, Ax, Cp_out, Ci_out, Cx_out);
 }
 
 /* expand upper-triangular CSC P into the full symmetric matrix in CSR
@@ -198,7 +82,7 @@ static int expand_sym_upper(int n, const int *Pp, const int *Pi, const double *P
 
 /* Row partition for the sharded KKT solve (SURVEY 8e): contiguous blocks with (nearly) equal
  * numbers of nonzeros. */
-/* generic fork-join over an array of job records (same policy as tr_run: threads that cannot be created run inline) */
+/* generic fork-join over an array of job records (threads that cannot be created run inline) */
 static void run_jobs(void *(*fn)(void *), void *jobs, size_t stride, int T) {
   pthread_t th[64];
   int t, started = 0;
@@ -348,28 +232,13 @@ static void setup_mark(const char *what, double *t_last) {
   }
 }
 
-/* Both resident orientations of a CSC matrix: on the device when the builder takes it (kernels/setup.cu -- upload once,
- * stable radix-sort transpose, flagged streams filled in HBM; bit-identical to the host builders), else by the host
- * builders. *A_out = the m x n operator (rows of A), *At_out = the n x m one (rows of A' = columns of A). */
+/* Both resident orientations of a CSC matrix, built on the device (kernels/setup.cu): *A_out = the m x n operator
+ * (rows of A), *At_out = the n x m one (rows of A' = columns of A). */
 static int build_both_ops(int m, int n, const int *Ap, const int *Ai, const double *Ax, B200Spmv **A_out,
                           B200Spmv **At_out, double *t_mark) {
-  int *Tp = NULL, *Ti = NULL;
-  double *Tx = NULL;
-  const int rc_dev = b200_setup_ops_from_csc(m, n, Ap, Ai, Ax, A_out, At_out);
-  if (rc_dev < 0) return -1;
-  if (rc_dev == 0) {
-    setup_mark("linsys: both operators built on the device", t_mark);
-    return 0;
-  }
-  /* host builders: the CSR of A' is the CSC of A as given */
-  *At_out = b200_spmv_create(n, m, Ap, Ai, Ax);
-  setup_mark("linsys: operator A' (host plan + upload)", t_mark);
-  if (!*At_out || transpose_csc(m, n, Ap, Ai, Ax, &Tp, &Ti, &Tx) != 0) return -1;
-  setup_mark("linsys: host transpose", t_mark);
-  *A_out = b200_spmv_create(m, n, Tp, Ti, Tx);
-  setup_mark("linsys: operator A (host plan + upload)", t_mark);
-  free(Tp); free(Ti); free(Tx);
-  return *A_out ? 0 : -1;
+  if (b200_setup_ops_from_csc(m, n, Ap, Ai, Ax, A_out, At_out) != 0) return -1;
+  setup_mark("linsys: both operators built on the device", t_mark);
+  return 0;
 }
 
 /* The reordered pair used inside the CG operator (kernels/spmv.cu "Reordered copies", DESIGN.md section 3.1): the rows
@@ -466,6 +335,7 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
     if (w->d_Pdiag) b200_h2d(w->d_Pdiag, diag, (size_t)n * 8);
     free(Fp); free(Fi); free(Fx); free(diag);
     if (!w->P || !w->d_Pdiag) goto fail;
+    setup_mark("linsys: operator P (host expansion, device build)", &t_mark);
   }
   w->d_diag_r = (double *)b200_malloc(((size_t)n + m + 1) * 8);
   w->d_b = (double *)b200_malloc(((size_t)n + m) * 8);

@@ -21,11 +21,7 @@
 #include "../dev_api.h"
 #include <stdlib.h>
 #include <string.h>
-#include <algorithm>
-#include <thread>
 #include <vector>
-
-extern "C" int b200_host_threads(long long work_items);  // host/linsys_b200.c
 
 struct B200Spmv {
   int nrows, ncols;
@@ -163,11 +159,29 @@ static size_t spmv3_smem_bytes() {
 
 // A row longer than SPMV3_MAXROW entries is cut into ceil(len / SPMV3_MAXROW) balanced pieces, the first
 // len % pieces of them one entry longer; a shorter row is one piece. Returns the end of piece q, counted from the
-// row's first entry. The one cut rule of the host fill, the device fill (k_fill_flagged) and the virtual rows.
+// row's first entry. The one cut rule of the fill (spmv3_fill_row) and the virtual rows.
 __host__ __device__ __forceinline__ int spmv3_piece_end(int len, int q) {
   const int pieces = len > SPMV3_MAXROW ? (len + SPMV3_MAXROW - 1) / SPMV3_MAXROW : 1;
   const int small = len / pieces, big = len % pieces;
   return (q + 1) * small + (q + 1 < big ? q + 1 : big);
+}
+
+// The stored entries of one row of `len` CSR entries (from entry a, stored from position pos): the entries, with an END
+// on the last entry of the row or of each of its pieces; an empty row stores one explicit zero, SKIP | END. The one
+// fill of the flagged stream: k_fill_flagged runs it per row on the device, the plan export of the CPU tests on the host.
+__host__ __device__ __forceinline__ void spmv3_fill_row(int len, int a, int pos, const int *__restrict__ ci,
+                                                        const double *__restrict__ va, int *__restrict__ oi,
+                                                        double *__restrict__ ov) {
+  if (len == 0) {
+    oi[pos] = (int)(B200_FLAG_END | B200_FLAG_SKIP);
+    ov[pos] = 0.0;
+  }
+  for (int k = 0, q = 0, e = spmv3_piece_end(len, 0); k < len; ++k) {
+    const bool end = k + 1 == e;
+    oi[pos + k] = end ? (int)((unsigned)ci[a + k] | B200_FLAG_END) : ci[a + k];
+    ov[pos + k] = va[a + k];
+    if (end) e = spmv3_piece_end(len, ++q);
+  }
 }
 
 // The phases (first stored position modulo 4, bit q = phase q) at which the flag kernel sums a row of `len` <= 124
@@ -494,20 +508,11 @@ spmv_combine_kernel(int nrows, const int *__restrict__ vptr, const double *__res
   spmv_tail<POST>(dot_acc, dot_out, hook, hook_arg, hook_val, partials, counter, s_red);
 }
 
-// ---- host side: the flagged stream, its warp-tiles and the static CTA partition.
-// Pure host code up to spmv3_finish (no CUDA calls): also exported for the CPU tests (tests/test_spmv_plan_cpu.py
-// re-executes the kernel's lane algorithm on this plan in numpy).
+// ---- host side: the virtual rows, warp-tiles and static CTA partition of a flagged stream, from its stored row
+// pointers. Pure host code up to spmv3_finish (no CUDA calls): also exported for the CPU tests
+// (tests/test_spmv_plan_cpu.py re-executes the kernel's lane algorithm on this plan in numpy).
 struct Spmv3Plan {
   std::vector<int> rowptr;   // stored row pointers (every row has >= 1 stored entry)
-  // column | END | SKIP and the values: raw buffers, deliberately NOT value-initialised (a 120 MB memset per
-  // operator at C2) -- every element is written by the fill below
-  struct Raw {
-    void *p = nullptr;
-    ~Raw() { free(p); }
-  } idx_mem, vals_mem;
-  size_t stored_count = 0;
-  int *idx_data() const { return static_cast<int *>(idx_mem.p); }
-  double *vals_data() const { return static_cast<double *>(vals_mem.p); }
   // long-row support: a row longer than SPMV3_MAXROW is cut into pieces ("virtual rows", an END flag at the end of
   // every piece); the kernel then produces one sum per virtual row and a combine pass adds the pieces of each true
   // row. vptr[r] = first virtual row of true row r, vrp = the virtual row pointers (both empty when no row was cut).
@@ -548,7 +553,7 @@ static void spmv3_virtual_rows(int nrows, Spmv3Plan &P) {
 }
 
 // warp-tiles (whole (virtual) rows whose aligned span (k0 & ~3 .. end) is <= 128 entries) and the static CTA
-// partition, from the stored (virtual) row pointers alone -- shared by every plan builder (host, device, permuted).
+// partition, from the stored (virtual) row pointers alone -- shared by every operator (plain and permuted).
 // CTAs own equal counts of warp-tiles. A warp-tile holds up to 128 entries whatever its rows, so this balances the
 // gathers; on the row-sorted CG copy of A it leaves 2.8x more rows on the last CTAs than on the first, but rows are
 // cheap next to gathers: balancing on entries + rows (or 2 entries + rows) was 1.3 % (0.2 %) slower per CG iteration
@@ -594,98 +599,41 @@ static void spmv3_tiles_from_rowptr(int grid_cap, Spmv3Plan &P) {
   }
 }
 
-// the flagged stream of a CSR, its stored and its virtual row pointers
-static bool spmv3_build_plan(int nrows, const int *rp, const int *ci, const double *va, Spmv3Plan &P) {
-  long long empties = 0;
-  for (int r = 0; r < nrows; ++r)
-    if (rp[r + 1] == rp[r]) ++empties;
-  const long long stored = rp[nrows] + empties;
-  if (!spmv3_fits(stored)) return false;
-  P.rowptr.resize((size_t)nrows + 1);
-  P.stored_count = (size_t)stored;
-  P.idx_mem.p = malloc(((size_t)stored + 1) * sizeof(int));
-  P.vals_mem.p = malloc(((size_t)stored + 1) * sizeof(double));
-  if (!P.idx_mem.p || !P.vals_mem.p) return false;
-  {
-    int pos = 0;
-    for (int r = 0; r < nrows; ++r) {
-      P.rowptr[r] = pos;
-      const int len = rp[r + 1] - rp[r];
-      pos += len > 0 ? len : 1;
-    }
-    P.rowptr[nrows] = pos;
-  }
-  // copy + flag the entries, rows split over host threads (disjoint output ranges)
-  {
-    int *out_i = P.idx_data();
-    double *out_v = P.vals_data();
-    const int *orp = P.rowptr.data();
-    auto fill = [=](int ra, int rb) {
-      for (int r = ra; r < rb; ++r) {
-        const int a = rp[r], len = rp[r + 1] - a, pos = orp[r];
-        if (len == 0) {
-          out_i[pos] = (int)(B200_FLAG_END | B200_FLAG_SKIP);
-          out_v[pos] = 0.0;
-          continue;
-        }
-        for (int k = 0; k < len; ++k) {
-          out_i[pos + k] = ci[a + k];
-          out_v[pos + k] = va[a + k];
-        }
-        for (int q = 0, e = 0; e < len; ++q) {  // an END after the row, or after each of its pieces
-          e = spmv3_piece_end(len, q);
-          out_i[pos + e - 1] = (int)((unsigned)out_i[pos + e - 1] | B200_FLAG_END);
-        }
-      }
-    };
-    const int T = b200_host_threads(stored);
-    if (T <= 1) {
-      fill(0, nrows);
-    } else {
-      std::vector<std::thread> th;
-      for (int t = 0; t < T; ++t) {
-        // ranges balanced by stored entries
-        auto cut = [&](int q) {
-          const long long target = stored * q / T;
-          return (int)(std::lower_bound(P.rowptr.begin(), P.rowptr.end(), (int)target) - P.rowptr.begin());
-        };
-        int ra = t == 0 ? 0 : cut(t), rb = t == T - 1 ? nrows : cut(t + 1);
-        if (ra > nrows) ra = nrows;
-        if (rb > nrows) rb = nrows;
-        if (rb > ra) {
-          try {
-            th.emplace_back(fill, ra, rb);
-          } catch (...) {  // no more threads available: do this range here
-            fill(ra, rb);
-          }
-        }
-      }
-      for (auto &x : th) x.join();
-    }
-  }
-  spmv3_virtual_rows(nrows, P);
-  return true;
-}
-
-// C view of a plan for the tests (host memory, owned by the handle)
+// C view of a plan for the tests (host memory, owned by the handle): the stream of a CSR as the device builder fills it
+// (k_stored_len and the scan, spmv3_fill_row), and what spmv3_finish computes from its stored row pointers
 struct B200Spmv3PlanHost {
   Spmv3Plan plan;
+  std::vector<int> idx;
+  std::vector<double> vals;
 };
 extern "C" B200Spmv3PlanHost *b200_spmv3_plan_build(int nrows, int ncols, const int *rp, const int *ci,
                                                     const double *va, int grid_cap) {
   if (nrows <= 0 || ncols >= (1 << 30)) return nullptr;
   B200Spmv3PlanHost *h = new B200Spmv3PlanHost();
-  if (!spmv3_build_plan(nrows, rp, ci, va, h->plan)) {
+  Spmv3Plan &P = h->plan;
+  P.rowptr.resize((size_t)nrows + 1);
+  long long stored = 0;
+  for (int r = 0; r < nrows; ++r) {
+    P.rowptr[r] = (int)stored;
+    stored += rp[r + 1] > rp[r] ? rp[r + 1] - rp[r] : 1;
+  }
+  if (!spmv3_fits(stored)) {
     delete h;
     return nullptr;
   }
-  spmv3_tiles_from_rowptr(grid_cap, h->plan);
+  P.rowptr[nrows] = (int)stored;
+  h->idx.resize((size_t)stored);
+  h->vals.resize((size_t)stored);
+  for (int r = 0; r < nrows; ++r)
+    spmv3_fill_row(rp[r + 1] - rp[r], rp[r], P.rowptr[r], ci, va, h->idx.data(), h->vals.data());
+  spmv3_virtual_rows(nrows, P);
+  spmv3_tiles_from_rowptr(grid_cap, P);
   return h;
 }
 extern "C" void b200_spmv3_plan_free(B200Spmv3PlanHost *h) { delete h; }
 extern "C" int b200_spmv3_plan_info(const B200Spmv3PlanHost *h, int *stored, int *nwt, int *ndesc, int *grid,
                                     int *ncw) {
-  *stored = (int)h->plan.stored_count;
+  *stored = h->plan.rowptr.back();
   *nwt = h->plan.nwt;
   *ndesc = (int)h->plan.wt.size();
   *grid = h->plan.grid;
@@ -693,8 +641,8 @@ extern "C" int b200_spmv3_plan_info(const B200Spmv3PlanHost *h, int *stored, int
   return 0;
 }
 extern "C" const int *b200_spmv3_plan_rowptr(const B200Spmv3PlanHost *h) { return h->plan.rowptr.data(); }
-extern "C" const int *b200_spmv3_plan_idx(const B200Spmv3PlanHost *h) { return h->plan.idx_data(); }
-extern "C" const double *b200_spmv3_plan_vals(const B200Spmv3PlanHost *h) { return h->plan.vals_data(); }
+extern "C" const int *b200_spmv3_plan_idx(const B200Spmv3PlanHost *h) { return h->idx.data(); }
+extern "C" const double *b200_spmv3_plan_vals(const B200Spmv3PlanHost *h) { return h->vals.data(); }
 extern "C" const int *b200_spmv3_plan_desc(const B200Spmv3PlanHost *h) {
   return reinterpret_cast<const int *>(h->plan.wt.data());
 }
@@ -754,47 +702,11 @@ static int spmv3_finish(B200Spmv *M, Spmv3Plan &P) {
   return 0;
 }
 
-extern "C" B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr,
-                                      const int *h_colidx, const double *h_vals) {
-  if (b200_runtime_init() != 0) return nullptr;
-  if (ncols >= (1 << 30) || nrows >= (1 << 30)) {
-    // bits 30/31 of the stored column indices are flags; every reader masks them
-    b200_set_error("b200_spmv_create: dimensions >= 2^30 are not supported", cudaErrorInvalidValue, __FILE__,
-                   __LINE__);
-    return nullptr;
-  }
-  B200Spmv *M = (B200Spmv *)calloc(1, sizeof(B200Spmv));
-  if (!M) return nullptr;
-  M->nrows = nrows;
-  M->ncols = ncols;
-  M->nnz = h_rowptr[nrows];
-  Spmv3Plan P;
-  bool ok = spmv3_build_plan(nrows, h_rowptr, h_colidx, h_vals, P);
-  if (ok) {
-    // the flagged stream IS the operator's CSR: rowptr / colidx / vals stay a valid CSR with explicit zeros
-    const size_t stored = P.stored_count, pad = ((stored + 3) & ~(size_t)3) + 8;
-    M->stored = (long long)stored;
-    M->d_rowptr = (int *)b200_malloc((size_t)(nrows + 1 + 8) * 4);
-    M->d_colidx = (int *)b200_malloc(pad * 4);
-    M->d_vals = (double *)b200_malloc(pad * 8);
-    ok = M->d_rowptr && M->d_colidx && M->d_vals && b200_memset0(M->d_rowptr, (size_t)(nrows + 1 + 8) * 4) == 0 &&
-         b200_memset0(M->d_colidx, pad * 4) == 0 && b200_memset0(M->d_vals, pad * 8) == 0 &&
-         b200_h2d(M->d_rowptr, P.rowptr.data(), (size_t)(nrows + 1) * 4) == 0 &&
-         b200_h2d(M->d_colidx, P.idx_data(), stored * 4) == 0 && b200_h2d(M->d_vals, P.vals_data(), stored * 8) == 0;
-  }
-  if (!ok || spmv3_finish(M, P) != 0) {
-    b200_spmv_destroy(M);
-    return nullptr;
-  }
-  return M;
-}
-
 // ---------------------------------------------------------------------------------------------
-// Device-side construction of a flagged-stream operator from a CSR that is ALREADY IN HBM (setup path of
-// scs_init_lin_sys_work, kernels/setup.cu): stored row pointers (every row >= 1 entry) by a scan, the flagged
-// stream by one fill kernel; only the row pointers travel back to the host for the (sequential, O(rows)) virtual-row
-// and warp-tile passes. Returns NULL on failure and for what the device path does not take (no rows, dimension and
-// size limits) -- the caller then takes the host path.
+// Construction of a flagged-stream operator from a CSR in HBM, the one builder of every operator (A and A' by
+// kernels/setup.cu, host CSRs such as P through b200_spmv_create): stored row pointers (every row >= 1 entry) by a
+// scan, the flagged stream by one fill kernel; only the row pointers travel back to the host for the (sequential,
+// O(rows)) virtual-row and warp-tile passes. Returns NULL on failure, with the reason in b200_last_error().
 __global__ void k_stored_len(int nrows, const int *__restrict__ rp, int *__restrict__ out) {
   for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < nrows; r += gridDim.x * blockDim.x) {
     const int len = rp[r + 1] - rp[r];
@@ -804,23 +716,14 @@ __global__ void k_stored_len(int nrows, const int *__restrict__ rp, int *__restr
 __global__ void k_fill_flagged(int nrows, const int *__restrict__ rp, const int *__restrict__ sp,
                                const int *__restrict__ ci, const double *__restrict__ va, int *__restrict__ oi,
                                double *__restrict__ ov) {
-  // one lane per row; an END after the row, or after each of its pieces -- the cut of spmv3_build_plan
+  // one lane per row (spmv3_fill_row)
   const int lane = threadIdx.x & 31;
   const int warp = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, nwarps = (gridDim.x * blockDim.x) >> 5;
   for (int r0 = warp * 32; r0 < nrows; r0 += nwarps * 32) {
     const int r = r0 + lane;
     if (r < nrows) {
       const int a = rp[r], len = rp[r + 1] - a, pos = sp[r];
-      if (len == 0) {
-        oi[pos] = (int)(B200_FLAG_END | B200_FLAG_SKIP);
-        ov[pos] = 0.0;
-      }
-      for (int k = 0, q = 0, e = spmv3_piece_end(len, 0); k < len; ++k) {
-        const bool end = k + 1 == e;
-        oi[pos + k] = end ? (int)((unsigned)ci[a + k] | B200_FLAG_END) : ci[a + k];
-        ov[pos + k] = va[a + k];
-        if (end) e = spmv3_piece_end(len, ++q);
-      }
+      spmv3_fill_row(len, a, pos, ci, va, oi, ov);
     }
   }
 }
@@ -829,7 +732,12 @@ extern "C" int b200_dev_exclusive_scan_int(const int *d_in, int *d_out, int coun
 extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, const int *d_rp, const int *d_ci,
                                           const double *d_va) {
   if (b200_runtime_init() != 0) return nullptr;
-  if (ncols >= (1 << 30) || nrows >= (1 << 30) || nrows <= 0) return nullptr;
+  if (nrows < 0 || ncols < 0 || ncols >= (1 << 30) || nrows >= (1 << 30)) {
+    // bits 30/31 of the stored column indices are flags; every reader masks them
+    b200_set_error("b200_spmv_create_dev: dimensions must lie in [0, 2^30)", cudaErrorInvalidValue, __FILE__,
+                   __LINE__);
+    return nullptr;
+  }
   cudaStream_t st = (cudaStream_t)b200_stream();
   B200Spmv *M = (B200Spmv *)calloc(1, sizeof(B200Spmv));
   if (!M) return nullptr;
@@ -843,24 +751,25 @@ extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, c
   if (ok) {
     int g = (nrows + 255) / 256;
     if (g > 8 * b200_num_sms()) g = 8 * b200_num_sms();
-    k_stored_len<<<g, 256, 0, st>>>(nrows, d_rp, d_len);
+    if (g > 0) k_stored_len<<<g, 256, 0, st>>>(nrows, d_rp, d_len);
     // exclusive scan over nrows + 1 items: element nrows receives the total
     ok = b200_dev_exclusive_scan_int(d_len, M->d_rowptr, nrows + 1) == 0 &&
          b200_d2h(P.rowptr.data(), M->d_rowptr, (size_t)(nrows + 1) * 4) == 0 && b200_sync() == 0;
-    b200_count_launch(2);
+    b200_count_launch(g > 0 ? 2 : 1);
   }
-  // the int scan wraps a total of 2^31 or more to a negative number (nnz <= 2e9 and nrows < 2^30 keep it below 2^32)
-  const int stored = ok ? P.rowptr[(size_t)nrows] : -1;
-  ok = ok && stored >= 0 && spmv3_fits(stored);
+  // the int scan wraps a total of 2^31 or more; read as unsigned it is exact, since int row pointers (nnz < 2^31) and
+  // nrows < 2^30 keep it below 2^32, and spmv3_fits rejects it
+  const long long stored = ok ? (long long)(unsigned)P.rowptr[(size_t)nrows] : 0;
+  ok = ok && spmv3_fits(stored);
   if (ok) {
     const size_t pad = (((size_t)stored + 3) & ~(size_t)3) + 8;
     M->stored = stored;
     M->d_colidx = (int *)b200_malloc(pad * 4);
     M->d_vals = (double *)b200_malloc(pad * 8);
     ok = M->d_colidx && M->d_vals && b200_memset0(M->d_colidx, pad * 4) == 0 && b200_memset0(M->d_vals, pad * 8) == 0;
-    if (ok) {
-      int g = (nrows + 255) / 256;
-      if (g > 16 * b200_num_sms()) g = 16 * b200_num_sms();
+    int g = (nrows + 255) / 256;
+    if (g > 16 * b200_num_sms()) g = 16 * b200_num_sms();
+    if (ok && g > 0) {
       k_fill_flagged<<<g, 256, 0, st>>>(nrows, d_rp, M->d_rowptr, d_ci, d_va, M->d_colidx, M->d_vals);
       b200_count_launch(1);
     }
@@ -872,6 +781,22 @@ extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, c
     b200_spmv_destroy(M);
     return nullptr;
   }
+  return M;
+}
+
+// an operator from a host CSR (P, the tests): uploaded, then built on the device like every other
+extern "C" B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr, const int *h_colidx,
+                                      const double *h_vals) {
+  if (b200_runtime_init() != 0) return nullptr;
+  const long long nnz = h_rowptr[nrows];
+  int *d_rp = (int *)b200_malloc((size_t)(nrows + 1) * 4), *d_ci = (int *)b200_malloc((size_t)nnz * 4);
+  double *d_va = (double *)b200_malloc((size_t)nnz * 8);
+  B200Spmv *M = nullptr;
+  if (d_rp && d_ci && d_va && b200_h2d(d_rp, h_rowptr, (size_t)(nrows + 1) * 4) == 0 &&
+      b200_h2d(d_ci, h_colidx, (size_t)nnz * 4) == 0 && b200_h2d(d_va, h_vals, (size_t)nnz * 8) == 0)
+    M = b200_spmv_create_dev(nrows, ncols, nnz, d_rp, d_ci, d_va);
+  // stream-ordered: the builder's kernels read the uploads before the blocks are handed out again
+  b200_free(d_rp); b200_free(d_ci); b200_free(d_va);
   return M;
 }
 

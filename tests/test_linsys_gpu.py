@@ -8,6 +8,7 @@ import pytest
 
 from scs_b200 import capi, problems
 from reference_replay import rel
+from test_spmv_plan_cpu import device_fill_restated, random_csr
 
 pytestmark = pytest.mark.gpu
 
@@ -154,34 +155,118 @@ def test_operator_without_rows(lib):
         lib.b200_spmv_destroy(M)
 
 
-@pytest.mark.parametrize("m,n,col_nnz,seed", [(3000, 50, 700, 4), (64, 5000, 40, 5), (30000, 10000, 10, 3)])
-def test_device_built_operators_equal_host_built(lib, m, n, col_nnz, seed, monkeypatch):
-    """scs_init_lin_sys_work builds both flagged streams on the device (kernels/setup.cu; rows longer than a warp-tile
-    are cut into the same balanced pieces as the host plan builder cuts them) -- the result must be BIT-identical to
-    the host builders' (SCS_B200_HOST_SETUP=1): same stream, same warp-tiles, same summation order."""
-    rng = np.random.default_rng(seed)
-    A = problems.random_sparse_csc(m, n, col_nnz, rng)
+class SpmvArgs(C.Structure):
+    """B200SpmvArgs (dev_api.h)"""
+    _fields_ = [("d_x", C.c_void_p), ("d_y", C.c_void_p), ("d_init", C.c_void_p), ("init_sign", C.c_double),
+                ("post", C.c_int), ("d_d", C.c_void_p), ("dform", C.c_int), ("d_dmask", C.c_void_p),
+                ("d_v", C.c_void_p), ("d_dot", C.c_void_p), ("hook", C.c_int), ("d_hook_arg", C.c_void_p),
+                ("hook_val", C.c_ulonglong), ("d_skip", C.c_void_p), ("pdl", C.c_int)]
+
+
+def host_csr(case):
+    """(nrows, ncols, rowptr, colidx, vals) of a host CSR: either orientation of the shapes above with long rows and of
+    C2 / 100, rows of 0 to 1500 entries, an operator without entries and one without columns"""
+    shapes = {"long_rows_of_At": (3000, 50, 700, 4), "long_rows_of_A": (64, 5000, 40, 5), "c2": (30000, 10000, 10, 3)}
+    if ":" in case:
+        which, shape = case.split(":")
+        m, n, col_nnz, seed = shapes[shape]
+        data, indices, indptr, _ = problems.random_sparse_csc(m, n, col_nnz, np.random.default_rng(seed))
+        if which == "At":  # the CSC arrays are the CSR of A'
+            return n, m, indptr, indices, data
+        import scipy.sparse as sp
+        R = sp.csc_matrix((data, indices, indptr), shape=(m, n)).tocsr()
+        R.sort_indices()
+        return m, n, R.indptr.astype(np.int32), R.indices.astype(np.int32), R.data
+    rng = np.random.default_rng(9)
+    nrows, ncols, lens = {
+        "row_lengths": (60, 2000, rng.permutation(np.repeat([0, 124, 125, 248, 249, 1500], 10))),
+        "no_entries": (500, 300, np.zeros(500, int)),
+        "no_columns": (40, 0, np.zeros(40, int)),
+    }[case]
+    return (nrows, ncols) + random_csr(nrows, ncols, rng, lens)
+
+
+@pytest.mark.parametrize("case", ["A:long_rows_of_At", "At:long_rows_of_At", "A:long_rows_of_A", "At:long_rows_of_A",
+                                  "A:c2", "At:c2", "row_lengths", "no_entries", "no_columns"])
+def test_operator_stream_from_host_csr(lib, case):
+    """b200_spmv_create uploads a host CSR and builds the operator on the device like every other: its stream (stored
+    row pointers, flagged column indices, values) is BIT-equal to the numpy statement of the fill, rows longer than a
+    warp-tile cut into the same balanced pieces, and its products match a plain CSR product."""
+    vp, ip, dp = C.c_void_p, C.POINTER(C.c_int), C.POINTER(C.c_double)
+    lib.b200_spmv_create.restype = vp
+    lib.b200_spmv_create.argtypes = [C.c_int, C.c_int, ip, ip, dp]
+    for name in ("b200_spmv_rowptr", "b200_spmv_colidx", "b200_spmv_vals"):
+        getattr(lib, name).restype = vp
+        getattr(lib, name).argtypes = [vp]
+    lib.b200_spmv_stored.restype = C.c_longlong
+    lib.b200_spmv_stored.argtypes = [vp]
+    lib.b200_spmv.restype = C.c_int
+    lib.b200_spmv.argtypes = [vp, vp]
+    lib.b200_spmv_destroy.argtypes = [vp]
+    lib.b200_malloc.restype = vp
+    lib.b200_malloc.argtypes = [C.c_size_t]
+    lib.b200_free.argtypes = [vp]
+    lib.b200_h2d.argtypes = [vp, vp, C.c_size_t]
+    lib.b200_d2h.argtypes = [vp, vp, C.c_size_t]
+    nrows, ncols, rp, ci, va = host_csr(case)
+    rp, ci, va = (np.ascontiguousarray(a, dtype=t) for a, t in ((rp, np.int32), (ci, np.int32), (va, np.float64)))
+    want_rp = np.concatenate([[0], np.cumsum(np.maximum(np.diff(rp), 1))]).astype(np.int32)  # one entry per empty row
+    want_idx, want_vals = device_fill_restated(rp, ci, va)
+    M = lib.b200_spmv_create(nrows, ncols, rp.ctypes.data_as(ip), ci.ctypes.data_as(ip), va.ctypes.data_as(dp))
+    assert M
+    d_x = lib.b200_malloc(8 * ncols)
+    d_y = lib.b200_malloc(8 * nrows)
+    try:
+        stored = lib.b200_spmv_stored(M)
+        assert stored == len(want_idx)
+        got_rp, got_idx, got_vals = np.empty(nrows + 1, np.int32), np.empty(stored, np.uint32), np.empty(stored)
+        for got, dev in ((got_rp, lib.b200_spmv_rowptr(M)), (got_idx, lib.b200_spmv_colidx(M)),
+                         (got_vals, lib.b200_spmv_vals(M))):
+            assert lib.b200_d2h(got.ctypes.data, dev, got.nbytes) == 0
+        assert lib.b200_sync() == 0
+        assert np.array_equal(got_rp, want_rp)
+        assert np.array_equal(got_idx, want_idx)
+        assert np.array_equal(got_vals.view(np.uint64), want_vals.view(np.uint64))
+        rng = np.random.default_rng(nrows + ncols)
+        for _ in range(2):
+            x, y = rng.standard_normal(ncols), np.full(nrows, np.nan)
+            assert lib.b200_h2d(d_x, x.ctypes.data, x.nbytes) == 0
+            args = SpmvArgs(d_x=d_x, d_y=d_y, init_sign=1.0)
+            assert lib.b200_spmv(M, C.byref(args)) == 0
+            assert lib.b200_d2h(y.ctypes.data, d_y, y.nbytes) == 0 and lib.b200_sync() == 0
+            ref = np.array([va[rp[r]:rp[r + 1]] @ x[ci[rp[r]:rp[r + 1]]] for r in range(nrows)])
+            assert rel(y, ref, 1e-300) <= 1e-13
+    finally:
+        lib.b200_free(d_x)
+        lib.b200_free(d_y)
+        lib.b200_spmv_destroy(M)
+
+
+def test_linsys_with_an_empty_a(lib):
+    """A without entries: both operators hold only explicit zeros, A x and A' y are zero, and the KKT solve is the
+    diagonal system [R_x 0; 0 -R_y] [x; y] = b."""
+    m, n = 30, 20
+    A = (np.zeros(0), np.zeros(0, np.int32), np.zeros(n + 1, np.int32), (m, n))
     hp = capi.HostProblem(A, np.zeros(m), np.zeros(n), {"l": m})
-    dr = diag_r_for(n, m, 0)
-    x, yv, rhs = rng.standard_normal(n), rng.standard_normal(m), rng.standard_normal(n + m)
-    outs = []
-    for host in (0, 1):
-        if host:
-            monkeypatch.setenv("SCS_B200_HOST_SETUP", "1")
-        else:
-            monkeypatch.delenv("SCS_B200_HOST_SETUP", raising=False)
-        w = lib.scs_init_lin_sys_work(C.byref(hp.A), None, capi.dptr(dr))
-        assert w
-        try:
-            ax, aty, sol = np.zeros(m), np.zeros(n), rhs.copy()
-            assert lib.scs_b200_accum_by_a(w, capi.dptr(x), capi.dptr(ax), 0) == 0
-            assert lib.scs_b200_accum_by_atrans(w, capi.dptr(yv), capi.dptr(aty), 0) == 0
-            assert lib.scs_solve_lin_sys(w, capi.dptr(sol), None, 1e-12) == 0
-            outs.append((ax, aty, sol))
-        finally:
-            lib.scs_free_lin_sys_work(w)
-    for a, b in zip(*outs):
-        assert np.array_equal(a, b)
+    dr = diag_r_for(n, m, 5)
+    rng = np.random.default_rng(8)
+    w = lib.scs_init_lin_sys_work(C.byref(hp.A), None, capi.dptr(dr))
+    assert w
+    try:
+        for acc in (0, 1):
+            y0, x0 = rng.standard_normal(m), rng.standard_normal(n)
+            ax, aty = y0.copy(), x0.copy()
+            assert lib.scs_b200_accum_by_a(w, capi.dptr(rng.standard_normal(n)), capi.dptr(ax), acc) == 0
+            assert lib.scs_b200_accum_by_atrans(w, capi.dptr(rng.standard_normal(m)), capi.dptr(aty), acc) == 0
+            assert np.array_equal(ax, y0 if acc else np.zeros(m))
+            assert np.array_equal(aty, x0 if acc else np.zeros(n))
+        rhs = rng.standard_normal(n + m)
+        sol = rhs.copy()
+        assert lib.scs_solve_lin_sys(w, capi.dptr(sol), None, 1e-12) == 0
+        want = np.linalg.solve(np.diag(np.concatenate([dr[:n], -dr[n:n + m]])), rhs)
+        assert rel(sol, want, 0.0) <= 1e-12
+    finally:
+        lib.scs_free_lin_sys_work(w)
 
 
 def test_spmv_full_size_c2_properties(lib):

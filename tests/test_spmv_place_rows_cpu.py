@@ -2,8 +2,7 @@
 called by `b200_spmv_permuted_rows`): rows taken from a window of the next 32 in smallest-column order, so that each
 starts at a phase (position modulo 4) where the kernel sums it as in A, with explicit zeros only where no row fits.
 The kernel's lane algorithm, re-executed in numpy, must give bit-for-bit the row sums of the original operator. No GPU
-needed: the placement is host code exported by the library. (tests/test_spmv_sorted_rows_cpu.py checks the earlier
-layout, in which every row kept its lane pieces from A at the cost of about one zero per row, on a numpy restatement.)"""
+needed: the placement is host code exported by the library."""
 import ctypes as C
 
 import numpy as np

@@ -1,9 +1,10 @@
-"""CPU checks of the v3 "flagged stream" SpMV plan (scs_b200/csrc/kernels/spmv.cu, host builder
-`spmv3_build_plan`): format invariants, and a numpy re-execution of the kernel's LANE algorithm
-(`spmv_flag_kernel`: 4 entries per lane, END ballots -> row numbers, in-lane sequential sums,
-segmented Hillis-Steele scan of the open tails, staging through a garbage-filled stage buffer
-exactly as the TMA producer cuts it) against a plain CSR product. No GPU needed: the builder is
-host code exported by the C-ABI library (operator: reference linsys/scs_matrix.c:161-186)."""
+"""CPU checks of the v3 "flagged stream" SpMV plan (scs_b200/csrc/kernels/spmv.cu, test export
+`b200_spmv3_plan_build`: the stream as the device builder fills it, by the same per-row fill `spmv3_fill_row` run on the
+host, and the virtual rows, warp-tiles and CTA partition of `spmv3_finish`): format invariants, and a numpy
+re-execution of the kernel's LANE algorithm (`spmv_flag_kernel`: 4 entries per lane, END ballots -> row numbers,
+in-lane sequential sums, segmented Hillis-Steele scan of the open tails, staging through a garbage-filled stage buffer
+exactly as the TMA producer cuts it) against a plain CSR product. No GPU needed (operator: reference
+linsys/scs_matrix.c:161-186)."""
 import ctypes as C
 
 import numpy as np
@@ -213,59 +214,6 @@ def test_plan_and_lane_algorithm(lib, case):
     assert np.abs(y - ref).max() / scale <= 1e-14
 
 
-@pytest.mark.parametrize("threads", ["1", "3", "8"])
-def test_plan_is_identical_for_any_host_thread_count(lib, threads, monkeypatch):
-    """the setup-time passes are split over host threads (disjoint output ranges): same plan for any count"""
-    rng = np.random.default_rng(77)
-    nrows, ncols = 20000, 9000
-    lens = np.minimum(rng.poisson(3.3, nrows), MAXROW)
-    rp, ci, va = random_csr(nrows, ncols, rng, lens)
-    monkeypatch.setenv("SCS_B200_HOST_THREADS", "1")
-    base = build_plan(lib, nrows, ncols, rp, ci, va, 148)
-    monkeypatch.setenv("SCS_B200_HOST_THREADS", threads)
-    other = build_plan(lib, nrows, ncols, rp, ci, va, 148)
-    for key in ("rowptr", "idx", "vals", "desc", "cta_begin"):
-        assert np.array_equal(base[key], other[key]), key
-    check_invariants(other, nrows, rp, ci, va)
-
-
-@pytest.mark.parametrize("threads", ["1", "2", "7", "16"])
-@pytest.mark.parametrize("shape", [(50, 20, 3), (3000, 1000, 10), (200, 5000, 2), (40000, 300, 50)])
-def test_parallel_transpose_matches_scipy(lib, threads, shape, monkeypatch):
-    """host CSC -> CSR (stable counting sort, reference cpu/indirect/private.c:7-46) on any thread count"""
-    import scipy.sparse as sp
-    from scs_b200 import problems
-    m, n, per = shape
-    rng = np.random.default_rng(m + n)
-    data, idx, ptr, _ = problems.random_sparse_csc(m, n, per, rng)
-    if m == 200:                                   # ragged: empty columns and empty rows
-        keep = rng.random(len(data)) < 0.5
-        cnt = np.add.reduceat(keep.astype(np.int64), ptr[:-1]) if len(data) else np.zeros(n, np.int64)
-        data, idx = data[keep], idx[keep]
-        ptr = np.concatenate([[0], np.cumsum(cnt)]).astype(np.int32)
-    monkeypatch.setenv("SCS_B200_HOST_THREADS", threads)
-    ip, dp = C.POINTER(C.c_int), C.POINTER(C.c_double)
-    lib.scs_b200_transpose_csc.restype = C.c_int
-    lib.scs_b200_transpose_csc.argtypes = [C.c_int, C.c_int, ip, ip, dp, C.POINTER(ip), C.POINTER(ip), C.POINTER(dp)]
-    cp, cidx, cx = ip(), ip(), dp()
-    idx = np.ascontiguousarray(idx, dtype=np.int32)
-    ptr = np.ascontiguousarray(ptr, dtype=np.int32)
-    data = np.ascontiguousarray(data)
-    assert lib.scs_b200_transpose_csc(m, n, ptr.ctypes.data_as(ip), idx.ctypes.data_as(ip), data.ctypes.data_as(dp),
-                                      C.byref(cp), C.byref(cidx), C.byref(cx)) == 0
-    nnz = int(ptr[-1])
-    got_p = np.ctypeslib.as_array(cp, (m + 1,)).copy()
-    got_i = np.ctypeslib.as_array(cidx, (max(nnz, 1),))[:nnz].copy()
-    got_x = np.ctypeslib.as_array(cx, (max(nnz, 1),))[:nnz].copy()
-    libc = C.CDLL(None)
-    libc.free.argtypes = [C.c_void_p]
-    for q in (cp, cidx, cx):
-        libc.free(C.cast(q, C.c_void_p))
-    R = sp.csc_matrix((data, idx, ptr), shape=(m, n)).tocsr()
-    R.sort_indices()
-    assert np.array_equal(got_p, R.indptr) and np.array_equal(got_i, R.indices) and np.array_equal(got_x, R.data)
-
-
 def test_plan_property_random_shapes(lib):
     """hypothesis: arbitrary row-length patterns (runs of empty rows, rows of exactly 124 entries, single
     rows, tiny column spaces) -> plan invariants hold and the lane algorithm reproduces the CSR product"""
@@ -369,9 +317,9 @@ def device_fill_restated(rp, ci, va):
 
 
 def test_device_fill_rule_equals_host_plan_stream(lib):
-    """The device builder (b200_spmv_create_dev) cuts long rows with its own kernel; the rule restated above must give
-    exactly the stream of the host plan builder (the hardware test of the real kernel:
-    tests/test_linsys_gpu.py::test_device_built_operators_equal_host_built)."""
+    """The rule restated above gives exactly the stream of the library's fill (spmv3_fill_row, run on the host by the
+    plan export); tests/test_linsys_gpu.py::test_operator_stream_from_host_csr checks the fill kernel on the device
+    against the same restatement."""
     rng = np.random.default_rng(77)
     for nrows, ncols, sampler in [
         (40, 3000, lambda: rng.choice([0, 1, 3, 124, 125, 200, 248, 249, 373, 700, 1500], 40)),
