@@ -11,6 +11,12 @@
  *      compiled against the reference headers can link this library instead.
  *      Compiled with USE_SPECTRAL_CONES, ScsCone gains the reference's spectral
  *      block; that layout is served by libscs_b200_spectral.so.
+ *      Compiled with DLONG, scs_int is 64 bits wide as in the reference's DLONG
+ *      build (scs_types.h:14-24 on LP64); those layouts are served by
+ *      libscs_b200_long.so, libscs_b200_spectral_long.so and the plugin-only
+ *      libscs_b200_linsys_long.so.  The kernels index with 32-bit integers: a
+ *      64-bit count, size or index is checked and narrowed at the entry points,
+ *      and a value that does not fit is refused, never truncated.
  *
  *  (2) the LINEAR-SYSTEM PLUGIN ABI -- the five link-time symbols every SCS
  *      backend defines (reference include/linsys.h:25-71).  Host pointers in and
@@ -39,8 +45,13 @@
 extern "C" {
 #endif
 
-/* primitive types of the reference build this ABI matches: DLONG=0, SFLOAT=0 (include/scs_types.h) */
+/* primitive types of the reference build this ABI matches: SFLOAT=0, and DLONG=0 unless compiled with DLONG
+ * (include/scs_types.h) */
+#ifdef DLONG
+typedef long long scs_int;
+#else
 typedef int scs_int;
+#endif
 typedef double scs_float;
 #define SCS_NULL 0
 

@@ -46,6 +46,12 @@ double b200_section_ms(int section);
  * transpose At gives the CSR of A (reference cpu/indirect/private.c:7-46). */
 typedef struct B200Spmv B200Spmv;
 
+/* Limits of every operator: row and column counts below 2^30 (bits 30 and 31 of a stored column index are flags), and
+ * at most B200_MAX_STORED entries in the stream, nnz plus one per empty row (the kernel forms stream positions up to
+ * stored + 128 in 32-bit int). The host layer checks user input against them before narrowing it to int. */
+#define B200_MAX_DIM ((1LL << 30) - 1)
+#define B200_MAX_STORED (2147483647LL - 128)
+
 /* an operator from a host CSR: the arrays are uploaded and the operator is built on the device like every other
  * (b200_spmv_create_dev, kernels/spmv.cu); nrows and nnz may be 0. NULL on failure */
 B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr, const int *h_colidx,
@@ -55,6 +61,11 @@ void b200_spmv_destroy(B200Spmv *M);
  * 0 ok, < 0 error */
 int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax, B200Spmv **A_out,
                             B200Spmv **At_out);
+/* the same from a CSC with 64-bit column pointers and row indices (the DLONG ABI): they are uploaded and narrowed to
+ * int on the device, and the build is refused (< 0) if a pointer decreases, leaves [0, nnz] or p[0] != 0, or a row
+ * index leaves [0, m) -- checked before any kernel reads an index. nnz = h_Ap[n] must not exceed B200_MAX_STORED. */
+int b200_setup_ops_from_csc64(int m, int n, const long long *h_Ap, const long long *h_Ai, const double *h_Ax,
+                              B200Spmv **A_out, B200Spmv **At_out);
 int b200_spmv_nrows(const B200Spmv *M);
 int b200_spmv_ncols(const B200Spmv *M);
 long long b200_spmv_nnz(const B200Spmv *M);

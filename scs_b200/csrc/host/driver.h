@@ -32,7 +32,7 @@
 /* rows of the spectral cones (reference cones.c:435-443); a log-det cone of order d has d(d+1)/2 + 2 */
 static inline long long b200_spectral_rows(const ScsCone *k) {
   long long rows = 0;
-  int i;
+  scs_int i;
   for (i = 0; i < k->dsize; ++i) rows += (long long)k->d[i] * (k->d[i] + 1) / 2 + 2;
   for (i = 0; i < k->nucsize; ++i) rows += (long long)k->nuc_m[i] * k->nuc_n[i] + 1;
   for (i = 0; i < k->ell1_size; ++i) rows += (long long)k->ell1[i] + 1;
@@ -95,6 +95,15 @@ struct SCS_WORK {
   FILE *log_csv_fout; /* opened ("w") at the start of every scs_solve, closed at its end (rw.c:686-705) */
   double *log_host; /* scratch: u, u_t, v, v_prev, rsk (l each), ax (m), aty (n), px (n) */
 };
+
+/* the integer-width boundary (host/abi.c): checks in scs_int width that print a message naming the limit and return
+ * nonzero, and int copies of the cone arrays for the kernel layer */
+int b200_cone_over_limits(const ScsCone *k);
+typedef struct {
+  int *q, *s, *cs, *nuc_m, *nuc_n, *ell1, *sl_n, *sl_k; /* NULL where the cone has none */
+} B200ConeInts;
+int b200_cone_ints(const ScsCone *k, B200ConeInts *c); /* 0, or -1 (out of memory, nothing held) */
+void b200_cone_ints_free(B200ConeInts *c);
 
 int b200_equilibrate(ScsMatrix *P, ScsMatrix *A, const int *bnd, int nbnd, double *D, double *E);
 double b200_normalize_b_c(int m, int n, const double *D, const double *E, double *b, double *c);

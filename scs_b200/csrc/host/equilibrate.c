@@ -46,7 +46,7 @@ static void enforce_boundaries(const int *bnd, int nbnd, double *vec, int mode) 
 
 static void ruiz_mats(const ScsMatrix *P, const ScsMatrix *A, double *Dt, double *Et, const int *bnd,
                       int nbnd) {
-  int i, j, kk;
+  scs_int i, j, kk;
   for (i = 0; i < A->m; ++i) Dt[i] = 0.;
   for (i = 0; i < A->n; ++i)
     for (j = A->p[i]; j < A->p[i + 1]; ++j) {
@@ -82,7 +82,7 @@ static void ruiz_mats(const ScsMatrix *P, const ScsMatrix *A, double *Dt, double
 
 static void l2_mats(const ScsMatrix *P, const ScsMatrix *A, double *Dt, double *Et, const int *bnd,
                     int nbnd) {
-  int i, j, kk;
+  scs_int i, j, kk;
   for (i = 0; i < A->m; ++i) Dt[i] = 0.;
   for (i = 0; i < A->n; ++i)
     for (j = A->p[i]; j < A->p[i + 1]; ++j) Dt[A->i[j]] += A->x[j] * A->x[j];
@@ -113,7 +113,7 @@ static void l2_mats(const ScsMatrix *P, const ScsMatrix *A, double *Dt, double *
 
 static void rescale(ScsMatrix *P, ScsMatrix *A, const double *Dt, const double *Et, double *D,
                     double *E) {
-  int i, j;
+  scs_int i, j;
   for (i = 0; i < A->n; ++i) {
     const double ei = Et[i];
     for (j = A->p[i]; j < A->p[i + 1]; ++j) A->x[j] *= Dt[A->i[j]] * ei;

@@ -35,20 +35,37 @@ static int b200_host_threads(long long work_items) {
 
 /* expand upper-triangular CSC P into the full symmetric matrix in CSR
  * (reference gpu/indirect/private.c:174-202 does the same for cuSPARSE);
- * also extracts diag(P) for the preconditioner. */
-static int expand_sym_upper(int n, const int *Pp, const int *Pi, const double *Px, int **Fp_out,
+ * also extracts diag(P) for the preconditioner. The input is of scs_int width, the output int: a P whose full
+ * symmetric form has more than B200_MAX_STORED entries, or a row index outside [0, n), is refused. */
+static int expand_sym_upper(int n, const scs_int *Pp, const scs_int *Pi, const double *Px, int **Fp_out,
                             int **Fi_out, double **Fx_out, double *diag) {
-  const int nnz = Pp[n];
   int *cnt = (int *)calloc((size_t)n + 1, sizeof(int));
   int *Fp = (int *)calloc((size_t)n + 1, sizeof(int));
   int *Fi;
   double *Fx;
-  int i, j, k, tot = 0;
+  int i, j, tot = 0;
+  scs_int k;
+  long long full = 0;
   if (!cnt || !Fp) { free(cnt); free(Fp); return -1; }
+  for (j = 0; j < n; ++j)
+    for (k = Pp[j]; k < Pp[j + 1]; ++k) {
+      if (Pi[k] < 0 || Pi[k] >= n) {
+        fprintf(stderr, "scs_b200: P row index %lld outside [0, %d)\n", (long long)Pi[k], n);
+        free(cnt); free(Fp);
+        return -1;
+      }
+      full += Pi[k] == j ? 1 : 2;
+    }
+  if (full > B200_MAX_STORED) {
+    fprintf(stderr, "scs_b200: the full symmetric P has %lld stored entries, above the limit 2^31 - 129 of one "
+            "operator\n", full);
+    free(cnt); free(Fp);
+    return -1;
+  }
   for (j = 0; j < n; ++j) diag[j] = 0.0;
   for (j = 0; j < n; ++j)
     for (k = Pp[j]; k < Pp[j + 1]; ++k) {
-      i = Pi[k];
+      i = (int)Pi[k];
       cnt[i]++;              /* entry (i,j) goes to row i */
       if (i != j) cnt[j]++;  /* mirrored entry (j,i) goes to row j */
       else diag[j] += Px[k];
@@ -63,7 +80,7 @@ static int expand_sym_upper(int n, const int *Pp, const int *Pi, const double *P
    * (mirrors, columns < row) then the upper part. Two passes keep it sorted. */
   for (j = 0; j < n; ++j)
     for (k = Pp[j]; k < Pp[j + 1]; ++k) {
-      i = Pi[k];
+      i = (int)Pi[k];
       if (i != j) { /* (i,j) with i<j stored; mirror (j,i): row j, col i < j */
         const int q = cnt[j]++;
         Fi[q] = i; Fx[q] = Px[k];
@@ -71,10 +88,9 @@ static int expand_sym_upper(int n, const int *Pp, const int *Pi, const double *P
     }
   for (j = 0; j < n; ++j)
     for (k = Pp[j]; k < Pp[j + 1]; ++k) {
-      i = Pi[k];
+      i = (int)Pi[k];
       { const int q = cnt[i]++; Fi[q] = j; Fx[q] = Px[k]; } /* row i, col j >= i */
     }
-  (void)nnz;
   free(cnt);
   *Fp_out = Fp; *Fi_out = Fi; *Fx_out = Fx;
   return 0;
@@ -97,7 +113,7 @@ static void run_jobs(void *(*fn)(void *), void *jobs, size_t stride, int T) {
 
 typedef struct {
   long long k0, k1;
-  const int *Ai;
+  const scs_int *Ai;
   int *cnt;
 } PcJob;
 static void *pc_worker(void *arg) { /* entries per row: integer counts, order-independent */
@@ -107,7 +123,7 @@ static void *pc_worker(void *arg) { /* entries per row: integer counts, order-in
   return NULL;
 }
 
-void b200_row_partition(int m, int n, const int *Ap, const int *Ai, int nranks, int *offsets) {
+void b200_row_partition(int m, int n, const scs_int *Ap, const scs_int *Ai, int nranks, int *offsets) {
   const long long nnz = Ap[n];
   int *cnt = (int *)calloc((size_t)m + 1, sizeof(int));
   long long acc = 0;
@@ -136,8 +152,21 @@ void b200_row_partition(int m, int n, const int *Ap, const int *Ai, int nranks, 
 }
 scs_int scs_b200_row_partition(scs_int m, scs_int n, const scs_int *Ap, const scs_int *Ai,
                                scs_int nranks, scs_int *offsets) {
+  int *offs;
+  scs_int r;
   if (m <= 0 || n <= 0 || nranks <= 0 || !Ap || !Ai || !offsets) return -1;
-  b200_row_partition(m, n, Ap, Ai, nranks, offsets);
+  if (b200_over_dim("m", -1, m) || b200_over_dim("n", -1, n) || b200_over_dim("nranks", -1, nranks) ||
+      b200_over_stored("nnz", Ap[n]))
+    return -1;
+  if (sizeof(scs_int) == sizeof(int)) {
+    b200_row_partition((int)m, (int)n, Ap, Ai, (int)nranks, (int *)offsets);
+    return 0;
+  }
+  offs = (int *)malloc(((size_t)nranks + 1) * sizeof(int));
+  if (!offs) return -1;
+  b200_row_partition((int)m, (int)n, Ap, Ai, (int)nranks, offs);
+  for (r = 0; r <= nranks; ++r) offsets[r] = offs[r];
+  free(offs);
   return 0;
 }
 
@@ -146,7 +175,7 @@ scs_int scs_b200_row_partition(scs_int m, scs_int n, const scs_int *Ap, const sc
  * number of threads. */
 typedef struct {
   int j0, j1, r0, r1, phase;
-  const int *Ap, *Ai;
+  const scs_int *Ap, *Ai;
   const double *Ax;
   int *Lp, *Li;
   double *Lx;
@@ -154,7 +183,8 @@ typedef struct {
 static void *rr_worker(void *arg) {
   RrJob *jb = (RrJob *)arg;
   const int r0 = jb->r0, r1 = jb->r1;
-  int j, k;
+  int j;
+  scs_int k;
   if (jb->phase == 0) {
     for (j = jb->j0; j < jb->j1; ++j) {
       int c = 0;
@@ -165,12 +195,12 @@ static void *rr_worker(void *arg) {
     for (j = jb->j0; j < jb->j1; ++j) {
       int q = jb->Lp[j];
       for (k = jb->Ap[j]; k < jb->Ap[j + 1]; ++k)
-        if (jb->Ai[k] >= r0 && jb->Ai[k] < r1) { jb->Li[q] = jb->Ai[k] - r0; jb->Lx[q] = jb->Ax[k]; ++q; }
+        if (jb->Ai[k] >= r0 && jb->Ai[k] < r1) { jb->Li[q] = (int)(jb->Ai[k] - r0); jb->Lx[q] = jb->Ax[k]; ++q; }
     }
   }
   return NULL;
 }
-static int restrict_rows(int n, const int *Ap, const int *Ai, const double *Ax, int r0, int r1,
+static int restrict_rows(int n, const scs_int *Ap, const scs_int *Ai, const double *Ax, int r0, int r1,
                          int **Lp_out, int **Li_out, double **Lx_out) {
   RrJob jobs[64];
   const long long nnz = Ap[n];
@@ -210,8 +240,8 @@ static int restrict_rows(int n, const int *Ap, const int *Ai, const double *Ax, 
   return 0;
 }
 /* test entry point (tests/test_sharding_cpu.py); the arrays are malloc'ed, the caller frees them */
-int scs_b200_restrict_rows_csc(int n, const int *Ap, const int *Ai, const double *Ax, int r0, int r1, int **Lp_out,
-                               int **Li_out, double **Lx_out) {
+int scs_b200_restrict_rows_csc(int n, const scs_int *Ap, const scs_int *Ai, const double *Ax, int r0, int r1,
+                               int **Lp_out, int **Li_out, double **Lx_out) {
   return restrict_rows(n, Ap, Ai, Ax, r0, r1, Lp_out, Li_out, Lx_out);
 }
 
@@ -239,6 +269,17 @@ static int build_both_ops(int m, int n, const int *Ap, const int *Ai, const doub
   if (b200_setup_ops_from_csc(m, n, Ap, Ai, Ax, A_out, At_out) != 0) return -1;
   setup_mark("linsys: both operators built on the device", t_mark);
   return 0;
+}
+/* the same from the caller's CSC, of scs_int width: with DLONG its 64-bit indices are narrowed on the device */
+static int build_both_ops_user(int m, int n, const scs_int *Ap, const scs_int *Ai, const double *Ax, B200Spmv **A_out,
+                               B200Spmv **At_out, double *t_mark) {
+#ifdef DLONG
+  if (b200_setup_ops_from_csc64(m, n, Ap, Ai, Ax, A_out, At_out) != 0) return -1;
+  setup_mark("linsys: both operators built on the device (64-bit indices narrowed there)", t_mark);
+  return 0;
+#else
+  return build_both_ops(m, n, Ap, Ai, Ax, A_out, At_out, t_mark);
+#endif
 }
 
 /* The reordered pair used inside the CG operator (kernels/spmv.cu "Reordered copies", DESIGN.md section 3.1): the rows
@@ -291,7 +332,13 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
   double t_mark = wall_ms();
   int *Lp = NULL, *Li = NULL;
   double *Lx = NULL;
-  const int n = A->n, m = A->m;
+  int n, m;
+  if (!A || b200_matrix_over_limits(A, P)) { /* in scs_int width, before anything is narrowed */
+    fprintf(stderr, "scs_b200: init_lin_sys_work refused its input\n");
+    return SCS_NULL;
+  }
+  n = (int)A->n;
+  m = (int)A->m;
   if (b200_runtime_init() != 0) {
     fprintf(stderr, "scs_b200: no usable sm_90 device: %s\n", b200_last_error());
     return SCS_NULL;
@@ -318,7 +365,7 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
       free(Lp); free(Li); free(Lx);
       if (rc != 0) goto fail;
     }
-  } else if (build_both_ops(m, n, A->p, A->i, A->x, &w->A, &w->At, &t_mark) != 0) {
+  } else if (build_both_ops_user(m, n, A->p, A->i, A->x, &w->A, &w->At, &t_mark) != 0) {
     goto fail;
   }
   if (!w->A || !w->At) goto fail;
@@ -452,7 +499,7 @@ int b200_linsys_full_equilibrate(const ScsMatrix *A, const int *bnd, int nbnd, d
   int rc = -1;
   double t_mark = wall_ms();
   B200Spmv *At = NULL, *Ar = NULL;
-  if (build_both_ops(A->m, A->n, A->p, A->i, A->x, &Ar, &At, &t_mark) == 0)
+  if (build_both_ops_user((int)A->m, (int)A->n, A->p, A->i, A->x, &Ar, &At, &t_mark) == 0)
     rc = b200_equilibrate_dev(Ar, At, bnd, nbnd, d_D, d_E);
   setup_mark("linsys: D, E from a temporary full copy", &t_mark);
   b200_spmv_destroy(Ar);

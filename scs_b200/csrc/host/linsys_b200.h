@@ -40,6 +40,11 @@ int b200_linsys_update_diag_r_dev(ScsLinSysWork *w, const double *d_diag_r);
 int b200_linsys_full_equilibrate(const ScsMatrix *A, const int *bnd, int nbnd, double *d_D, double *d_E);
 int b200_linsys_scale_local(ScsLinSysWork *w, const double *d_D, const double *d_E);
 /* contiguous row blocks balanced by nonzeros; offsets[nranks+1] (also exported for the tests) */
-void b200_row_partition(int m, int n, const int *Ap, const int *Ai, int nranks, int *offsets);
+void b200_row_partition(int m, int n, const scs_int *Ap, const scs_int *Ai, int nranks, int *offsets);
+/* the limits of the operators checked in scs_int width (host/abi.c): dimensions below 2^30, nnz(A) and nnz(P) at most
+ * B200_MAX_STORED; prints a message naming the limit and returns nonzero when one is exceeded */
+int b200_over_dim(const char *what, long long index, scs_int v);
+int b200_over_stored(const char *what, scs_int v);
+int b200_matrix_over_limits(const ScsMatrix *A, const ScsMatrix *P);
 
 #endif

@@ -18,9 +18,11 @@ struct SCS_B200_CONE_WORK {
 ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float *D) {
   ScsB200ConeWork *c;
   double *bl = SCS_NULL, *bu = SCS_NULL;
-  int j;
+  scs_int j;
   long long dims;
+  B200ConeInts ci;
   if (!k || m <= 0) return SCS_NULL;
+  if (b200_over_dim("m", -1, m) || b200_cone_over_limits(k)) return SCS_NULL; /* in scs_int width, before narrowing */
   if (k->cssize < 0 || (k->cssize > 0 && !k->cs)) return SCS_NULL;
   if (k->ep < 0 || k->ed < 0 || k->psize < 0 || (k->psize > 0 && !k->p)) return SCS_NULL;
   dims = (long long)k->z + k->l + k->bsize;
@@ -42,12 +44,12 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float
   dims += b200_spectral_rows(k);
 #endif
   if (dims != m) {
-    fprintf(stderr, "scs_b200: cone dims %lld != m %d\n", dims, m);
+    fprintf(stderr, "scs_b200: cone dims %lld != m %lld\n", dims, (long long)m);
     return SCS_NULL;
   }
   c = (ScsB200ConeWork *)calloc(1, sizeof(*c));
   if (!c) return SCS_NULL;
-  c->m = m;
+  c->m = (int)m;
   if (k->bsize > 1) {
     /* box bounds follow the row scaling (reference normalize_box_cone, cones.c:1160-1177);
      * as in the reference, the +-1e15 -> inf mapping only happens when a scaling is given */
@@ -65,22 +67,28 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float
       }
     }
   }
-  c->cones = b200_cones_create(m, k->z, k->l, k->bsize, bl, bu, k->qsize, k->q, k->ssize, k->s);
+  if (b200_cone_ints(k, &ci) != 0) goto fail; /* int copies for the kernel layer */
+  c->cones = b200_cones_create(c->m, (int)k->z, (int)k->l, (int)k->bsize, bl, bu, (int)k->qsize, ci.q, (int)k->ssize,
+                               ci.s);
   free(bl);
   free(bu);
   bl = bu = SCS_NULL;
-  if (!c->cones) goto fail;
+  if (!c->cones) goto fail_ints;
 #ifdef USE_SPECTRAL_CONES
-  if (b200_cones_set_spectral(c->cones, k->nucsize, k->nuc_m, k->nuc_n, k->ell1_size, k->ell1, k->sl_size, k->sl_n,
-                              k->sl_k) != 0)
-    goto fail;
+  if (b200_cones_set_spectral(c->cones, (int)k->nucsize, ci.nuc_m, ci.nuc_n, (int)k->ell1_size, ci.ell1,
+                              (int)k->sl_size, ci.sl_n, ci.sl_k) != 0)
+    goto fail_ints;
 #endif
-  if (b200_cones_set_triples(c->cones, k->ep, k->ed, k->psize, k->p) != 0) goto fail;
-  if (b200_cones_set_complex_psd(c->cones, k->cssize, k->cs, k->ep + k->ed + k->psize) != 0) goto fail;
+  if (b200_cones_set_triples(c->cones, (int)k->ep, (int)k->ed, (int)k->psize, k->p) != 0) goto fail_ints;
+  if (b200_cones_set_complex_psd(c->cones, (int)k->cssize, ci.cs, (int)(k->ep + k->ed + k->psize)) != 0)
+    goto fail_ints;
+  b200_cone_ints_free(&ci);
   c->d_x = (double *)b200_malloc((size_t)m * 8);
   c->d_ry = (double *)b200_malloc((size_t)m * 8);
   if (!c->d_x || !c->d_ry) goto fail;
   return c;
+fail_ints:
+  b200_cone_ints_free(&ci);
 fail:
   free(bl);
   free(bu);
@@ -113,15 +121,23 @@ struct SCS_B200_AA_WORK {
   double *d_f, *d_x;
 };
 
+static int over_int(long long v) { return v > 2147483647LL; }
+
 ScsB200AaWork *scs_b200_aa_init(scs_int dim, scs_int mem, scs_int min_len, scs_int type1,
                                 scs_float regularization, scs_float relaxation,
                                 scs_float safeguard_factor, scs_float max_weight_norm,
                                 scs_int ir_max_steps, scs_int verbosity) {
-  ScsB200AaWork *w = (ScsB200AaWork *)calloc(1, sizeof(*w));
+  ScsB200AaWork *w;
+  /* the vector length and the memory are int inside; larger 64-bit values are refused, not truncated */
+  if (over_int(dim) || b200_over_dim("mem", -1, mem) || b200_over_dim("min_len", -1, min_len) ||
+      b200_over_dim("ir_max_steps", -1, ir_max_steps))
+    return SCS_NULL;
+  w = (ScsB200AaWork *)calloc(1, sizeof(*w));
   if (!w) return SCS_NULL;
-  w->dim = dim;
-  w->a = b200_aa_create(dim, mem, min_len, type1, regularization, relaxation, safeguard_factor,
-                        max_weight_norm, ir_max_steps, verbosity);
+  w->dim = (int)dim;
+  w->a = b200_aa_create((int)dim, (int)mem, (int)min_len, type1 != 0, regularization, relaxation, safeguard_factor,
+                        max_weight_norm, (int)ir_max_steps,
+                        verbosity > 2 ? 2 : verbosity < 0 ? 0 : (int)verbosity); /* levels 0, 1, 2 */
   if (!w->a) { free(w); return SCS_NULL; }
   w->d_f = (double *)b200_malloc((size_t)dim * 8);
   w->d_x = (double *)b200_malloc((size_t)dim * 8);

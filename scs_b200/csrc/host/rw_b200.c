@@ -18,8 +18,9 @@
  *            nuc_n[]; I ell1_size, ell1[]; I sl_size, sl_n[], sl_k[]; F time_limit_secs
  * The default build skips the spectral arrays on reading and writes them empty; the spectral build
  * (USE_SPECTRAL_CONES) reads them into ScsCone and writes them as the reference's spectral build does.
- * The writer always emits I = 4 bytes and the version string of the API it implements ("3.2.11");
- * the reader accepts I = 4 or 8 (values must fit an int) and both settings layouts. */
+ * The writer emits I = sizeof(scs_int) -- 4 bytes, or 8 in the DLONG build, as the reference's writer of the same
+ * width does -- and the version string of the API it implements ("3.2.11"). The reader accepts I = 4 or 8 and both
+ * settings layouts: the DLONG build widens 4-byte files, the int build narrows 8-byte ones (values must fit an int). */
 #include "driver.h"
 #include <stdint.h>
 #include <stdio.h>
@@ -40,31 +41,39 @@ static void put_raw(Stream *s, const void *p, size_t bytes) {
   if (s->bad || bytes == 0) return;
   if (!p || fwrite(p, 1, bytes, s->f) != bytes) s->bad = 1;
 }
-static void put_i(Stream *s, int v) { put_raw(s, &v, sizeof(int)); }
+static void put_i(Stream *s, scs_int v) { put_raw(s, &v, sizeof(scs_int)); }
 static void put_f(Stream *s, double v) { put_raw(s, &v, sizeof(double)); }
-static void put_is(Stream *s, const int *v, int n) { if (n > 0) put_raw(s, v, (size_t)n * sizeof(int)); }
-static void put_fs(Stream *s, const double *v, int n) { if (n > 0) put_raw(s, v, (size_t)n * sizeof(double)); }
+static void put_is(Stream *s, const scs_int *v, scs_int n) { if (n > 0) put_raw(s, v, (size_t)n * sizeof(scs_int)); }
+static void put_fs(Stream *s, const double *v, scs_int n) { if (n > 0) put_raw(s, v, (size_t)n * sizeof(double)); }
 
 static void get_raw(Stream *s, void *p, size_t bytes) {
   if (s->bad || bytes == 0) return;
   if (fread(p, 1, bytes, s->f) != bytes) s->bad = 1;
 }
-static void get_is(Stream *s, int *dst, size_t n) {
+static void get_is(Stream *s, scs_int *dst, size_t n) {
   size_t i;
   if (s->bad || n == 0) return;
-  if (s->int_bytes == (int)sizeof(int)) {
-    get_raw(s, dst, n * sizeof(int));
+  if (s->int_bytes == (int)sizeof(scs_int)) {
+    get_raw(s, dst, n * sizeof(scs_int));
     return;
   }
-  for (i = 0; i < n && !s->bad; ++i) { /* 8-byte integers on file: narrow, refusing overflow */
+  if (s->int_bytes == 4) { /* 4-byte integers on file, 8-byte scs_int (DLONG): widen */
+    for (i = 0; i < n && !s->bad; ++i) {
+      int32_t narrow = 0;
+      get_raw(s, &narrow, sizeof(narrow));
+      dst[i] = narrow;
+    }
+    return;
+  }
+  for (i = 0; i < n && !s->bad; ++i) { /* 8-byte integers on file, int scs_int: narrow, refusing overflow */
     int64_t wide = 0;
     get_raw(s, &wide, sizeof(wide));
     if (wide > 2147483647LL || wide < -2147483647LL - 1) s->bad = 1;
-    dst[i] = (int)wide;
+    dst[i] = (scs_int)wide;
   }
 }
-static int get_i(Stream *s) {
-  int v = 0;
+static scs_int get_i(Stream *s) {
+  scs_int v = 0;
   get_is(s, &v, 1);
   return v;
 }
@@ -74,16 +83,16 @@ static double get_f(Stream *s) {
   return v;
 }
 /* allocate-and-read; a negative count is a format error, count 0 gives NULL */
-static int *get_i_array(Stream *s, int n) {
-  int *v;
+static scs_int *get_i_array(Stream *s, scs_int n) {
+  scs_int *v;
   if (n < 0) s->bad = 1;
   if (s->bad || n == 0) return SCS_NULL;
-  v = (int *)calloc((size_t)n, sizeof(int));
+  v = (scs_int *)calloc((size_t)n, sizeof(scs_int));
   if (!v) { s->bad = 1; return SCS_NULL; }
   get_is(s, v, (size_t)n);
   return v;
 }
-static double *get_f_array(Stream *s, int n) {
+static double *get_f_array(Stream *s, scs_int n) {
   double *v;
   if (n < 0) s->bad = 1;
   if (s->bad || n == 0) return SCS_NULL;
@@ -93,7 +102,7 @@ static double *get_f_array(Stream *s, int n) {
   return v;
 }
 #ifndef USE_SPECTRAL_CONES
-static void skip_i_array(Stream *s, int n) {
+static void skip_i_array(Stream *s, scs_int n) {
   char buf[4096];
   uint64_t left;
   if (n < 0) s->bad = 1;
@@ -109,7 +118,7 @@ static void skip_i_array(Stream *s, int n) {
 
 /* ------------------------------------------------------------------ writer */
 static void put_matrix(Stream *s, const ScsMatrix *M) {
-  const int nnz = M->p[M->n];
+  const scs_int nnz = M->p[M->n];
   if (nnz < 0) { s->bad = 1; return; }
   put_i(s, M->m);
   put_i(s, M->n);
@@ -121,14 +130,14 @@ static void put_matrix(Stream *s, const ScsMatrix *M) {
 scs_int scs_b200_write_data(const char *filename, const ScsData *d, const ScsCone *k,
                             const ScsSettings *stgs) {
   Stream s;
-  const uint32_t head[3] = {(uint32_t)sizeof(int), (uint32_t)sizeof(double), (uint32_t)strlen(FILE_API_VERSION)};
+  const uint32_t head[3] = {(uint32_t)sizeof(scs_int), (uint32_t)sizeof(double), (uint32_t)strlen(FILE_API_VERSION)};
   const uint32_t ext[2] = {EXT_MAGIC, 1u};
-  int nbox;
+  scs_int nbox;
   if (!filename || !d || !k || !stgs || !d->A) return -1;
   nbox = k->bsize > 1 ? k->bsize - 1 : 0;
   s.f = fopen(filename, "wb");
   s.bad = 0;
-  s.int_bytes = (int)sizeof(int);
+  s.int_bytes = (int)sizeof(scs_int);
   if (!s.f) {
     printf("Error: could not open %s for writing\n", filename);
     return -1;
@@ -177,7 +186,7 @@ scs_int scs_b200_write_data(const char *filename, const ScsData *d, const ScsCon
 /* ------------------------------------------------------------------ reader */
 static ScsMatrix *get_matrix(Stream *s) {
   ScsMatrix *M = (ScsMatrix *)calloc(1, sizeof(ScsMatrix));
-  int nnz;
+  scs_int nnz;
   if (!M) { s->bad = 1; return SCS_NULL; }
   M->m = get_i(s);
   M->n = get_i(s);
@@ -213,7 +222,8 @@ scs_int scs_b200_read_data(const char *filename, ScsData **d_out, ScsCone **k_ou
   Stream s;
   uint32_t head[3] = {0, 0, 0};
   char ver[16];
-  int current_layout, nbox;
+  int current_layout;
+  scs_int nbox;
   ScsData *d = SCS_NULL;
   ScsCone *k = SCS_NULL;
   ScsSettings *st = SCS_NULL;
@@ -221,7 +231,7 @@ scs_int scs_b200_read_data(const char *filename, ScsData **d_out, ScsCone **k_ou
   *d_out = SCS_NULL; *k_out = SCS_NULL; *stgs_out = SCS_NULL;
   s.f = fopen(filename, "rb");
   s.bad = 0;
-  s.int_bytes = (int)sizeof(int);
+  s.int_bytes = (int)sizeof(scs_int);
   if (!s.f) {
     printf("Error reading file %s\n", filename);
     return -1;
@@ -278,7 +288,7 @@ scs_int scs_b200_read_data(const char *filename, ScsData **d_out, ScsCone **k_ou
     const size_t got = fread(&magic, 1, sizeof(magic), s.f);
     if (got == sizeof(magic) && magic == EXT_MAGIC) {
       uint32_t ev = 0;
-      int cnt;
+      scs_int cnt;
       get_raw(&s, &ev, sizeof(ev));
       if (ev != 1u) { printf("Error: unsupported SCS file extension version %u\n", ev); s.bad = 1; }
       k->cssize = get_i(&s); k->cs = get_i_array(&s, k->cssize);

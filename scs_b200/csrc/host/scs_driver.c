@@ -55,15 +55,18 @@ void scs_set_default_settings(ScsSettings *stgs) {
   stgs->time_limit_secs = 0.;
 }
 
-static int sd_size(int s) { return (s * (s + 1)) / 2; }
+static scs_int sd_size(scs_int s) { return (s * (s + 1)) / 2; }
 
 /* ----------------------------------------------------------------- validation */
+/* Every count is read in scs_int width: nnz(A) is checked against the operator limit before i[] or x[] is read, and a
+ * 64-bit index that would truncate to a valid int (2^32 + 3 -> 3) fails the range checks. */
 static int validate_matrix(const ScsMatrix *A, const ScsMatrix *P) {
-  int i, j, Anz;
+  scs_int i, j, Anz;
   if (!A) { printf("A matrix missing\n"); return -1; }
   if (A->m <= 0 || A->n <= 0) { printf("A matrix dimensions must be positive\n"); return -1; }
   if (!A->x || !A->i || !A->p) { printf("data incompletely specified\n"); return -1; }
   if (A->p[0] != 0) { printf("A->p[0] must equal 0\n"); return -1; }
+  if (b200_over_stored("nnz(A) = A->p[n]", A->p[A->n])) return -1;
   for (j = 0; j < A->n; ++j)
     if (A->p[j] < 0 || A->p[j] > A->p[j + 1]) {
       printf("A->p (column pointers) must be nonnegative and nondecreasing\n");
@@ -82,11 +85,13 @@ static int validate_matrix(const ScsMatrix *A, const ScsMatrix *P) {
     if (!isfinite(A->x[i])) { printf("A contains a non-finite entry\n"); return -1; }
   }
   if (P) {
-    int Pnz;
+    scs_int Pnz;
+    long long full = 0; /* stored entries of the full symmetric P */
     if (!P->x || !P->i || !P->p) { printf("P matrix incompletely specified\n"); return -1; }
     if (P->n != A->n) { printf("P dimension inconsistent with n\n"); return -1; }
     if (P->m != P->n) { printf("P is not square\n"); return -1; }
     if (P->p[0] != 0) { printf("P->p[0] must equal 0\n"); return -1; }
+    if (b200_over_stored("nnz(P) = P->p[n]", P->p[P->n])) return -1;
     for (j = 0; j < P->n; ++j)
       if (P->p[j] < 0 || P->p[j] > P->p[j + 1]) {
         printf("P->p (column pointers) must be nonnegative and nondecreasing\n");
@@ -99,14 +104,17 @@ static int validate_matrix(const ScsMatrix *A, const ScsMatrix *P) {
         if (P->i[i] < 0 || P->i[i] >= P->n) { printf("P row index outside valid range\n"); return -1; }
         if (P->i[i] > j) { printf("P is not upper triangular\n"); return -1; }
         if (!isfinite(P->x[i])) { printf("P contains a non-finite entry\n"); return -1; }
+        full += P->i[i] == j ? 1 : 2;
       }
+    if (b200_over_stored("stored entries of the full symmetric P", full)) return -1;
   }
   return 0;
 }
 
 static int validate_cones(const ScsData *d, const ScsCone *k) {
-  int i;
+  scs_int i;
   long long dims;
+  if (b200_cone_over_limits(k)) return -1; /* every count and size below 2^30, before any sum of them */
   if (k->z < 0) { printf("free cone dimension error\n"); return -1; }
   if (k->l < 0) { printf("lp cone dimension error\n"); return -1; }
   if (k->bsize < 0) { printf("box cone dimension error\n"); return -1; }
@@ -167,8 +175,8 @@ static int validate_cones(const ScsData *d, const ScsCone *k) {
       return -1;
     }
   if (k->dsize > 0) { /* never dropped silently: its rows would go unprojected */
-    printf("log-det cones (dsize = %i) are not supported: this library projects the nuclear-norm, l1-norm and "
-           "sum-of-largest-eigenvalues spectral cones only\n", k->dsize);
+    printf("log-det cones (dsize = %lli) are not supported: this library projects the nuclear-norm, l1-norm and "
+           "sum-of-largest-eigenvalues spectral cones only\n", (long long)k->dsize);
     return -1;
   }
 #endif
@@ -192,6 +200,7 @@ static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs)
     printf("m and n must both be greater than 0; m = %li, n = %li\n", (long)d->m, (long)d->n);
     return -1;
   }
+  if (b200_over_dim("m", -1, d->m) || b200_over_dim("n", -1, d->n)) return -1;
   if (d->A && (d->A->m != d->m || d->A->n != d->n)) {
     printf("A dimensions inconsistent with m, n\n");
     return -1;
@@ -209,6 +218,7 @@ static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs)
   if (!isfinite(stgs->time_limit_secs) || stgs->time_limit_secs < 0) { printf("time_limit_secs must be a nonnegative finite number.\n"); return -1; }
   if (stgs->acceleration_interval <= 0) { printf("acceleration_interval must be positive (10 works well).\n"); return -1; }
   if (stgs->acceleration_lookback < 0) { printf("acceleration_lookback must be nonnegative\n"); return -1; }
+  if (b200_over_dim("acceleration_lookback", -1, stgs->acceleration_lookback)) return -1;
   if (!isfinite(stgs->acceleration_regularization) || stgs->acceleration_regularization < 0) {
     printf("acceleration_regularization must be a nonnegative finite number.\n");
     return -1;
@@ -224,19 +234,19 @@ static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs)
 /* ----------------------------------------------------------------- deep copies */
 static ScsMatrix *copy_matrix(const ScsMatrix *src) {
   ScsMatrix *A;
-  int nz;
+  scs_int nz;
   if (!src) return SCS_NULL;
   nz = src->p[src->n];
   A = (ScsMatrix *)calloc(1, sizeof(ScsMatrix));
   if (!A) return SCS_NULL;
   A->n = src->n; A->m = src->m;
   A->x = (double *)malloc(((size_t)nz + 1) * sizeof(double));
-  A->i = (int *)malloc(((size_t)nz + 1) * sizeof(int));
-  A->p = (int *)malloc(((size_t)src->n + 1) * sizeof(int));
+  A->i = (scs_int *)malloc(((size_t)nz + 1) * sizeof(scs_int));
+  A->p = (scs_int *)malloc(((size_t)src->n + 1) * sizeof(scs_int));
   if (!A->x || !A->i || !A->p) { free(A->x); free(A->i); free(A->p); free(A); return SCS_NULL; }
   memcpy(A->x, src->x, (size_t)nz * sizeof(double));
-  memcpy(A->i, src->i, (size_t)nz * sizeof(int));
-  memcpy(A->p, src->p, ((size_t)src->n + 1) * sizeof(int));
+  memcpy(A->i, src->i, (size_t)nz * sizeof(scs_int));
+  memcpy(A->p, src->p, ((size_t)src->n + 1) * sizeof(scs_int));
   return A;
 }
 static void free_matrix(ScsMatrix *A) {
@@ -381,15 +391,16 @@ static void print_header(const ScsWork *w) {
   printf("\n\t       SCS hot path on H100 (scs_b200 %s, API of SCS 3.2.11)\n", SCS_VERSION_STR);
   for (i = 0; i < 78; ++i) printf("-");
   printf("\nproblem:  variables n: %i, constraints m: %i\n", w->n, w->m);
-  printf("cones: \t  z: %i, l: %i, b: %i, q: %i cones, s: %i cones, exp: %i + %i dual, pow: %i\n", k->z, k->l,
-         k->bsize, k->qsize, k->ssize, k->ep, k->ed, k->psize);
+  printf("cones: \t  z: %i, l: %i, b: %i, q: %i cones, s: %i cones, exp: %i + %i dual, pow: %i\n", (int)k->z,
+         (int)k->l, (int)k->bsize, (int)k->qsize, (int)k->ssize, (int)k->ep, (int)k->ed, (int)k->psize);
   printf("settings: eps_abs: %.1e, eps_rel: %.1e, eps_infeas: %.1e\n\t  alpha: %.2f, scale: %.2e, "
-         "adaptive_scale: %i\n\t  max_iters: %i, normalize: %i, rho_x: %.2e\n",
+         "adaptive_scale: %lli\n\t  max_iters: %lli, normalize: %lli, rho_x: %.2e\n",
          w->stgs->eps_abs, w->stgs->eps_rel, w->stgs->eps_infeas, w->stgs->alpha, w->stgs->scale,
-         w->stgs->adaptive_scale, w->stgs->max_iters, w->stgs->normalize, w->stgs->rho_x);
+         (long long)w->stgs->adaptive_scale, (long long)w->stgs->max_iters, (long long)w->stgs->normalize,
+         w->stgs->rho_x);
   if (w->stgs->acceleration_lookback)
-    printf("\t  acceleration_lookback: %i, acceleration_interval: %i\n",
-           w->stgs->acceleration_lookback, w->stgs->acceleration_interval);
+    printf("\t  acceleration_lookback: %lli, acceleration_interval: %lli\n",
+           (long long)w->stgs->acceleration_lookback, (long long)w->stgs->acceleration_interval);
   printf("lin-sys:  %s\n\t  nnz(A): %li, nnz(P): %li\n", scs_get_lin_sys_method(),
          (long)w->nnzA, (long)w->nnzP);
 }
@@ -399,6 +410,7 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   const double t0 = now_ms();
   double t_mark = t0;
   int n, m, i, dev_equil = 0;
+  B200ConeInts ci;
   size_t l;
   if (!d || !k || !stgs) {
     printf("ERROR: Missing ScsData, ScsCone, or ScsSettings input\n");
@@ -449,20 +461,20 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
     w->k->bl = (double *)dup_mem(k->bl, (size_t)(k->bsize - 1) * 8);
     if (!w->k->bu || !w->k->bl) goto fail;
   }
-  if (k->qsize > 0) { w->k->q = (int *)dup_mem(k->q, (size_t)k->qsize * 4); if (!w->k->q) goto fail; }
+  if (k->qsize > 0) { w->k->q = (scs_int *)dup_mem(k->q, (size_t)k->qsize * sizeof(scs_int)); if (!w->k->q) goto fail; }
   if (k->psize > 0) { w->k->p = (double *)dup_mem(k->p, (size_t)k->psize * 8); if (!w->k->p) goto fail; }
-  if (k->cssize > 0) { w->k->cs = (int *)dup_mem(k->cs, (size_t)k->cssize * 4); if (!w->k->cs) goto fail; }
-  if (k->ssize > 0) { w->k->s = (int *)dup_mem(k->s, (size_t)k->ssize * 4); if (!w->k->s) goto fail; }
+  if (k->cssize > 0) { w->k->cs = (scs_int *)dup_mem(k->cs, (size_t)k->cssize * sizeof(scs_int)); if (!w->k->cs) goto fail; }
+  if (k->ssize > 0) { w->k->s = (scs_int *)dup_mem(k->s, (size_t)k->ssize * sizeof(scs_int)); if (!w->k->s) goto fail; }
 #ifdef USE_SPECTRAL_CONES
   if (k->nucsize > 0) {
-    w->k->nuc_m = (int *)dup_mem(k->nuc_m, (size_t)k->nucsize * 4);
-    w->k->nuc_n = (int *)dup_mem(k->nuc_n, (size_t)k->nucsize * 4);
+    w->k->nuc_m = (scs_int *)dup_mem(k->nuc_m, (size_t)k->nucsize * sizeof(scs_int));
+    w->k->nuc_n = (scs_int *)dup_mem(k->nuc_n, (size_t)k->nucsize * sizeof(scs_int));
     if (!w->k->nuc_m || !w->k->nuc_n) goto fail;
   }
-  if (k->ell1_size > 0) { w->k->ell1 = (int *)dup_mem(k->ell1, (size_t)k->ell1_size * 4); if (!w->k->ell1) goto fail; }
+  if (k->ell1_size > 0) { w->k->ell1 = (scs_int *)dup_mem(k->ell1, (size_t)k->ell1_size * sizeof(scs_int)); if (!w->k->ell1) goto fail; }
   if (k->sl_size > 0) {
-    w->k->sl_n = (int *)dup_mem(k->sl_n, (size_t)k->sl_size * 4);
-    w->k->sl_k = (int *)dup_mem(k->sl_k, (size_t)k->sl_size * 4);
+    w->k->sl_n = (scs_int *)dup_mem(k->sl_n, (size_t)k->sl_size * sizeof(scs_int));
+    w->k->sl_k = (scs_int *)dup_mem(k->sl_k, (size_t)k->sl_size * sizeof(scs_int));
     if (!w->k->sl_n || !w->k->sl_k) goto fail;
   }
 #endif
@@ -574,25 +586,30 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   memcpy(w->c_orig, d->c, (size_t)n * 8);
   if (scs_update(w, w->b_orig, w->c_orig) != 0) goto fail;
 
-  w->cones = b200_cones_create(m, w->k->z, w->k->l, w->k->bsize, w->k->bl, w->k->bu, w->k->qsize,
-                               w->k->q, w->k->ssize, w->k->s);
+  /* the kernel layer takes int copies of the cone arrays (validated below 2^30) */
+  if (b200_cone_ints(w->k, &ci) != 0) goto fail;
+  w->cones = b200_cones_create(m, (int)w->k->z, (int)w->k->l, (int)w->k->bsize, w->k->bl, w->k->bu,
+                               (int)w->k->qsize, ci.q, (int)w->k->ssize, ci.s);
 #ifdef USE_SPECTRAL_CONES
-  if (w->cones && b200_cones_set_spectral(w->cones, w->k->nucsize, w->k->nuc_m, w->k->nuc_n, w->k->ell1_size,
-                                          w->k->ell1, w->k->sl_size, w->k->sl_n, w->k->sl_k) != 0) {
+  if (w->cones && b200_cones_set_spectral(w->cones, (int)w->k->nucsize, ci.nuc_m, ci.nuc_n, (int)w->k->ell1_size,
+                                          ci.ell1, (int)w->k->sl_size, ci.sl_n, ci.sl_k) != 0) {
     printf("ERROR: init_cone failure (spectral cones)\n");
+    b200_cone_ints_free(&ci);
     goto fail;
   }
 #endif
-  if (!w->cones || b200_cones_set_triples(w->cones, w->k->ep, w->k->ed, w->k->psize, w->k->p) != 0 ||
-      b200_cones_set_complex_psd(w->cones, w->k->cssize, w->k->cs, w->k->ep + w->k->ed + w->k->psize) != 0) {
+  if (!w->cones || b200_cones_set_triples(w->cones, (int)w->k->ep, (int)w->k->ed, (int)w->k->psize, w->k->p) != 0 ||
+      b200_cones_set_complex_psd(w->cones, (int)w->k->cssize, ci.cs, (int)(w->k->ep + w->k->ed + w->k->psize)) != 0) {
     printf("ERROR: init_cone failure\n");
+    b200_cone_ints_free(&ci);
     goto fail;
   }
+  b200_cone_ints_free(&ci);
   if (!w->p) w->p = scs_init_lin_sys_work(w->d->A, w->d->P, w->h_diag_r);
   if (!w->p) { printf("ERROR: init_lin_sys_work failure\n"); goto fail; }
   if (w->stgs->acceleration_lookback) {
-    w->accel = b200_aa_create((int)l, w->stgs->acceleration_lookback, w->stgs->acceleration_lookback,
-                              w->stgs->acceleration_type_1, w->stgs->acceleration_regularization,
+    w->accel = b200_aa_create((int)l, (int)w->stgs->acceleration_lookback, (int)w->stgs->acceleration_lookback,
+                              w->stgs->acceleration_type_1 != 0, w->stgs->acceleration_regularization,
                               w->stgs->acceleration_relaxation, AA_SAFEGUARD_FACTOR,
                               AA_MAX_WEIGHT_NORM, AA_IR_MAX_STEPS, 0);
     if (!w->accel && w->stgs->verbose) printf("WARN: aa_init returned NULL, no acceleration applied.\n");

@@ -71,13 +71,60 @@ __global__ void k_gather_transposed(long long nnz, const int *__restrict__ perm,
   }
 }
 
-// Both operators from the host CSC of A (m x n; m, n or nnz may be 0). Returns 0 and sets *A_out (CSR of A) / *At_out
-// (CSR of A' = the CSC arrays); < 0 on failure.
-extern "C" int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax,
-                                       B200Spmv **A_out, B200Spmv **At_out) {
+// The 64-bit CSC of the DLONG ABI narrowed to the int32 arrays of the builder, one grid-stride pass over the pointers
+// and the entries. *d_bad receives 1 if p[0] != 0, a pointer decreases or leaves [0, nnz], or a row index leaves [0, m):
+// nothing else checks the plugin path's input, and a truncated index (2^32 + 3 -> 3) would look valid.
+__global__ void k_narrow_csc(int m, int n, long long nnz, const long long *__restrict__ Ap64,
+                             const long long *__restrict__ Ai64, int *__restrict__ Ap, int *__restrict__ Ai,
+                             int *__restrict__ d_bad) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
+  bool bad = false;
+  for (long long j = t; j <= n; j += stride) {
+    const long long v = Ap64[j];
+    bad |= v < 0 || v > nnz || (j == 0 && v != 0) || (j < n && Ap64[j + 1] < v);
+    Ap[j] = (int)v;
+  }
+  for (long long k = t; k < nnz; k += stride) {
+    const long long v = Ai64[k];
+    bad |= v < 0 || v >= m;
+    Ai[k] = (int)v;
+  }
+  if (bad) atomicOr(d_bad, 1);
+}
+
+// uploads the 64-bit arrays, narrows them into d_Ap / d_Ai and reads the flag back before anything reads an index
+static int narrow_csc(int m, int n, long long nnz, const long long *h_Ap64, const long long *h_Ai64, int *d_Ap,
+                      int *d_Ai) {
+  long long *d_Ap64 = (long long *)b200_malloc((size_t)(n + 1) * 8);
+  long long *d_Ai64 = (long long *)b200_malloc((size_t)nnz * 8);
+  int *d_bad = (int *)b200_malloc(4);
+  int h_bad = 1, rc = -1;
+  if (d_Ap64 && d_Ai64 && d_bad && b200_h2d(d_Ap64, h_Ap64, (size_t)(n + 1) * 8) == 0 &&
+      b200_h2d(d_Ai64, h_Ai64, (size_t)nnz * 8) == 0 && b200_memset0(d_bad, 4) == 0) {
+    const long long work = nnz > n ? nnz : (long long)n + 1;
+    const long long g = (work + 255) / 256 < 8LL * b200_num_sms() ? (work + 255) / 256 : 8LL * b200_num_sms();
+    k_narrow_csc<<<(int)g, 256, 0, (cudaStream_t)b200_stream()>>>(m, n, nnz, d_Ap64, d_Ai64, d_Ap, d_Ai, d_bad);
+    b200_count_launch(1);
+    if (cudaGetLastError() == cudaSuccess && b200_d2h(&h_bad, d_bad, 4) == 0 && b200_sync() == 0) {
+      rc = h_bad ? -1 : 0;
+      if (h_bad)
+        b200_set_error("b200_setup_ops_from_csc64: column pointers must start at 0 and not decrease, and row indices "
+                       "must lie in [0, m)", cudaErrorInvalidValue, __FILE__, __LINE__);
+    }
+  }
+  b200_sync();
+  b200_free(d_Ap64); b200_free(d_Ai64); b200_free(d_bad);
+  return rc;
+}
+
+// Both operators from the host CSC of A (m x n; m, n or nnz may be 0): int32 arrays (h_Ap, h_Ai) or 64-bit ones
+// (h_Ap64, h_Ai64, narrowed on the device by k_narrow_csc). Returns 0 and sets *A_out (CSR of A) / *At_out (CSR of A' =
+// the CSC arrays); < 0 on failure.
+static int setup_ops(int m, int n, long long nnz, const int *h_Ap, const int *h_Ai, const long long *h_Ap64,
+                     const long long *h_Ai64, const double *h_Ax, B200Spmv **A_out, B200Spmv **At_out) {
   *A_out = *At_out = nullptr;
   if (b200_runtime_init() != 0) return -1;
-  const long long nnz = h_Ap[n];
   cudaStream_t st = (cudaStream_t)b200_stream();
   int *d_Ap = (int *)b200_malloc((size_t)(n + 1) * 4), *d_Ai = (int *)b200_malloc((size_t)nnz * 4);
   double *d_Ax = (double *)b200_malloc((size_t)nnz * 8);
@@ -94,9 +141,12 @@ extern "C" int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int 
   dev_mark("allocations", &t_mark);
   do {
     if (!d_Ap || !d_Ai || !d_Ax || !d_Tp || !d_cnt || !d_Ti || !d_Tx || !d_cols || !d_iota || !d_keys || !d_perm) break;
-    if (b200_h2d(d_Ap, h_Ap, (size_t)(n + 1) * 4) != 0 || b200_h2d(d_Ai, h_Ai, (size_t)nnz * 4) != 0 ||
-        b200_h2d(d_Ax, h_Ax, (size_t)nnz * 8) != 0)
+    if (h_Ap64) {
+      if (narrow_csc(m, n, nnz, h_Ap64, h_Ai64, d_Ap, d_Ai) != 0) break;
+    } else if (b200_h2d(d_Ap, h_Ap, (size_t)(n + 1) * 4) != 0 || b200_h2d(d_Ai, h_Ai, (size_t)nnz * 4) != 0) {
       break;
+    }
+    if (b200_h2d(d_Ax, h_Ax, (size_t)nnz * 8) != 0) break;
     dev_mark("H2D of the CSC arrays", &t_mark);
     // A' first: its CSR is the CSC as given
     At = b200_spmv_create_dev(n, m, nnz, d_Ap, d_Ai, d_Ax);
@@ -143,6 +193,21 @@ extern "C" int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int 
   *A_out = A;
   *At_out = At;
   return 0;
+}
+extern "C" int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax,
+                                       B200Spmv **A_out, B200Spmv **At_out) {
+  return setup_ops(m, n, h_Ap[n], h_Ap, h_Ai, nullptr, nullptr, h_Ax, A_out, At_out);
+}
+extern "C" int b200_setup_ops_from_csc64(int m, int n, const long long *h_Ap, const long long *h_Ai,
+                                         const double *h_Ax, B200Spmv **A_out, B200Spmv **At_out) {
+  const long long nnz = h_Ap[n];
+  if (nnz < 0 || nnz > B200_MAX_STORED) {
+    *A_out = *At_out = nullptr;
+    b200_set_error("b200_setup_ops_from_csc64: nnz must lie in [0, 2^31 - 129]", cudaErrorInvalidValue, __FILE__,
+                   __LINE__);
+    return -1;
+  }
+  return setup_ops(m, n, nnz, nullptr, nullptr, h_Ap, h_Ai, h_Ax, A_out, At_out);
 }
 
 // ---------------------------------------------------------------------------------------------

@@ -150,7 +150,7 @@ __device__ __forceinline__ void spmv_tail(double dot_acc, double *dot_out, int h
 #define SPMV3_CAP (SPMV3_NCW * SPMV3_WT + 8)
 #define SPMV3_MAXROW 124
 // the kernel forms stream positions up to stored + 128 in 32-bit int (kb = (k0 & ~3) + 4 * lane, ka + cnt)
-#define SPMV3_MAX_STORED (2147483647LL - 128)
+#define SPMV3_MAX_STORED B200_MAX_STORED
 
 static size_t spmv3_smem_bytes() {
   return (size_t)SPMV3_STAGES * (SPMV3_CAP * 12 + SPMV3_NCW * 16) + 2 * SPMV3_STAGES * 8 + 64 * 8 +
