@@ -22,6 +22,11 @@
  *      backend defines (reference include/linsys.h:25-71).  Host pointers in and
  *      out, exactly as the stock src/scs.c calls them (scs.c:1092,1127,763,1220).
  *
+ *      The device-data entry points (scs_b200_init_device / _update_device /
+ *      _solve_device, declared in scs_b200_device.h) take the problem and
+ *      return the solution in GPU memory; like the outer ABI, the plugin-only
+ *      libraries leave them out.
+ *
  *  (3) OPERATOR-LEVEL entry points (scs_b200_*): the cone projection, Anderson
  *      acceleration and SpMV operators of the hot path callable one at a time
  *      with host buffers.  The reference keeps these internal
@@ -169,6 +174,11 @@ scs_int scs(const ScsData *d, const ScsCone *k, const ScsSettings *stgs,
             ScsSolution *sol, ScsInfo *info);
 void scs_set_default_settings(ScsSettings *stgs);
 const char *scs_version(void);
+
+/* Host<->device copies made by this library since the last reset: out[0] = bytes host to device, out[1] = the largest
+ * single such copy, out[2], out[3] = the same device to host. */
+void scs_b200_transfer_stats(long long out[4]);
+void scs_b200_transfer_stats_reset(void);
 
 /* ------------------------------------------------------------------ (2) --
  * Linear-system plugin ABI.  Replaces reference linsys/cpu/indirect/private.c

@@ -383,6 +383,15 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_comm_finalize.restype = I
     lib.scs_b200_row_partition.restype = I
     lib.scs_b200_row_partition.argtypes = [I, I, IP, IP, I, IP]
+    lib.scs_b200_init_device.restype = C.c_void_p
+    lib.scs_b200_init_device.argtypes = [C.POINTER(ScsData), C.POINTER(cone), C.POINTER(ScsSettings), C.c_void_p]
+    lib.scs_b200_update_device.restype = I
+    lib.scs_b200_update_device.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_void_p]
+    lib.scs_b200_solve_device.restype = I
+    lib.scs_b200_solve_device.argtypes = [C.c_void_p, C.POINTER(ScsSolution), C.POINTER(ScsInfo), I, C.c_void_p]
+    lib.scs_b200_transfer_stats.restype = None
+    lib.scs_b200_transfer_stats.argtypes = [C.POINTER(C.c_longlong)]
+    lib.scs_b200_transfer_stats_reset.restype = None
     lib.scs_b200_launch_count.restype = C.c_longlong
     lib.scs_b200_device_ok.restype = I
     lib.scs_b200_release_memory.restype = None

@@ -75,6 +75,17 @@ int b200_vec_scale_by(long long len, double *d_a, const double *d_d, double f);
  * bnd[1..nbnd) = sizes of the cones sharing one D value. d_D (m), d_E (n) are outputs. */
 int b200_equilibrate_dev(B200Spmv *A_rows, B200Spmv *A_cols, const int *bnd, int nbnd, double *d_D,
                          double *d_E);
+/* the same with P != 0, bit for bit host/equilibrate.c: P scaled in place on its upper CSC (d_Pp, d_Pi, d_Px); d_Fp,
+ * d_Fi, d_Fsrc: the structure of the full P (b200_sym_expand_structure) */
+int b200_equilibrate_qp_dev(B200Spmv *A_rows, B200Spmv *A_cols, const int *d_Pp, const int *d_Pi, double *d_Px,
+                            const int *d_Fp, const int *d_Fi, const int *d_Fsrc, const int *bnd, int nbnd,
+                            double *d_D, double *d_E);
+/* b = b_orig * D, c = c_orig * E (D, E NULL: plain copies); h_max (host, 4) receives max |b_orig|, max |b|,
+ * max |c_orig|, max |c| (synchronises). b200_scale_b_c then multiplies both by sigma: together the device form of
+ * host/equilibrate.c b200_normalize_b_c, bit for bit */
+int b200_normalize_b_c_dev(int m, int n, const double *d_b_orig, const double *d_c_orig, const double *d_D,
+                           const double *d_E, double *d_b, double *d_c, double *h_max);
+int b200_scale_b_c(int m, int n, double *d_b, double *d_c, double sigma);
 int b200_rescale_dev(B200Spmv *M, const double *d_rowscale, const double *d_colscale, int row_is_d);
 
 /* ---------------------------------------------------------------- cones (kernels/cones.cu) */

@@ -38,6 +38,12 @@ int b200_section_mark(int section);
 int b200_section_flush(void);          /* syncs with the last mark */
 double b200_section_ms(int section);
 
+int b200_is_device_ptr(const void *p); /* 1: device or managed memory of the library's device */
+/* ordering with a caller's cudaStream_t (NULL = legacy default stream), host-asynchronous: the library stream waits
+ * for the work enqueued so far on the caller's stream / the caller's stream waits for the library stream */
+int b200_wait_for_caller(void *caller_stream);
+int b200_caller_waits(void *caller_stream);
+
 /* ------------------------------------------------------------ SpMV ------- */
 /* A sparse operator stored row-major (CSR): row r has entries
  * [rowptr[r], rowptr[r+1]) with column indices colidx[] and values vals[].
@@ -66,6 +72,26 @@ int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, cons
  * index leaves [0, m) -- checked before any kernel reads an index. nnz = h_Ap[n] must not exceed B200_MAX_STORED. */
 int b200_setup_ops_from_csc64(int m, int n, const long long *h_Ap, const long long *h_Ai, const double *h_Ax,
                               B200Spmv **A_out, B200Spmv **At_out);
+/* the same from the builder's own device CSC (int32 indices, validated); the arrays are only read */
+int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d_Ap, const int *d_Ai, const double *d_Ax,
+                            B200Spmv **A_out, B200Spmv **At_out);
+/* The validating copy of a caller's device CSC (idx64: 64-bit indices, narrowed) into the builder's int32 / fp64
+ * arrays (kernels/setup.cu). First the pointers: *flags = B200_CSC_BAD_* bits. Only with *flags == 0, the entries:
+ * *first = ~0, or (k << 2 | code) of the first entry k that fails (code B200_CSC_BAD_ROW / _UPPER / _VAL, upper != 0
+ * for the upper triangle of P); *ndiag = its diagonal entries. d_x and d_Ax may both be NULL. */
+enum { B200_CSC_BAD_P0 = 1, B200_CSC_BAD_PTR = 2 };
+enum { B200_CSC_BAD_ROW = 0, B200_CSC_BAD_UPPER = 1, B200_CSC_BAD_VAL = 2 };
+int b200_csc_check_ptrs(int n, long long nnz, const void *d_p, int idx64, int *d_Ap, unsigned *flags);
+int b200_csc_copy_entries(int rows, int n, long long nnz, const void *d_i, const double *d_x, int idx64,
+                          const int *d_Ap, int upper, int *d_Ai, double *d_Ax, unsigned long long *first,
+                          long long *ndiag);
+/* the full symmetric P from its n x n upper CSC on the device, in the CSR of the host's expand_sym_upper: the
+ * structure (d_Fp n+1, d_Fi and d_Fsrc `full`: the CSC entry each full entry copies), then, from the CSC's values, the
+ * operator and diag(P) (d_diag, n) */
+int b200_sym_expand_structure(int n, long long nnz, long long full, const int *d_Pp, const int *d_Pi, int *d_Fp,
+                              int *d_Fi, int *d_Fsrc);
+int b200_sym_build(int n, long long full, const int *d_Fp, const int *d_Fi, const int *d_Fsrc, const double *d_Px,
+                   double *d_diag, B200Spmv **P_out);
 int b200_spmv_nrows(const B200Spmv *M);
 int b200_spmv_ncols(const B200Spmv *M);
 long long b200_spmv_nnz(const B200Spmv *M);

@@ -5,6 +5,7 @@
 #ifndef B200_DRIVER_H
 #define B200_DRIVER_H
 #include "../../../include/scs_b200.h"
+#include "../../../include/scs_b200_device.h"
 #include "../admm_api.h"
 #include "../dev_api.h"
 #include "linsys_b200.h"
@@ -94,6 +95,11 @@ struct SCS_WORK {
   char *log_csv_name; /* deep copy of ScsSettings.log_csv_filename */
   FILE *log_csv_fout; /* opened ("w") at the start of every scs_solve, closed at its end (rw.c:686-705) */
   double *log_host; /* scratch: u, u_t, v, v_prev, rsk (l each), ax (m), aty (n), px (n) */
+  /* device-data entry points (scs_b200_*_device): b_orig, c_orig on the device (NULL until a device call needs them);
+   * *_on_dev = the device copy is the current one and the host copy stale; bc_host_stale = d->b, d->c (host) are
+   * stale; sol_on_dev = the ScsSolution of the running solve holds device pointers */
+  double *d_b_orig, *d_c_orig;
+  int b_on_dev, c_on_dev, bc_host_stale, sol_on_dev;
 };
 
 /* the integer-width boundary (host/abi.c): checks in scs_int width that print a message naming the limit and return

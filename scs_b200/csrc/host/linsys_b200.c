@@ -326,6 +326,8 @@ static int cg_ops_refresh(ScsLinSysWork *w) {
   return b200_cg_classify_diag(&w->cg, w->d_perm);
 }
 
+static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_mark_p);
+
 ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
                                      const scs_float *diag_r) {
   ScsLinSysWork *w;
@@ -384,6 +386,41 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
     if (!w->P || !w->d_Pdiag) goto fail;
     setup_mark("linsys: operator P (host expansion, device build)", &t_mark);
   }
+  if (linsys_vectors(w, diag_r, &t_mark) != 0) goto fail;
+  return w;
+fail:
+  fprintf(stderr, "scs_b200: init_lin_sys_work failed: %s\n", b200_last_error());
+  scs_free_lin_sys_work(w);
+  return SCS_NULL;
+}
+
+/* single GPU, from operators built on the device (the device-data entry points, host/scs_driver.c): the workspace takes
+ * A, At, P and d_Pdiag over, also when it fails */
+ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B200Spmv *P, double *d_Pdiag,
+                                    const scs_float *diag_r) {
+  double t_mark = wall_ms();
+  ScsLinSysWork *w = (ScsLinSysWork *)calloc(1, sizeof(ScsLinSysWork));
+  if (!w) {
+    b200_spmv_destroy(A); b200_spmv_destroy(At); b200_spmv_destroy(P); b200_free(d_Pdiag);
+    return SCS_NULL;
+  }
+  w->n = n; w->m = m;
+  w->nnz = b200_spmv_nnz(At);
+  w->nranks = 1;
+  w->mloc = m;
+  w->A = A; w->At = At; w->P = P; w->d_Pdiag = d_Pdiag;
+  if (linsys_vectors(w, diag_r, &t_mark) != 0) {
+    fprintf(stderr, "scs_b200: init_lin_sys_work failed: %s\n", b200_last_error());
+    scs_free_lin_sys_work(w);
+    return SCS_NULL;
+  }
+  return w;
+}
+
+/* the work vectors, the preconditioner and the CG loop's reordered pair of a workspace whose operators are built */
+static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_mark_p) {
+  const int n = w->n, m = w->m;
+  double t_mark = *t_mark_p;
   w->d_diag_r = (double *)b200_malloc(((size_t)n + m + 1) * 8);
   w->d_b = (double *)b200_malloc(((size_t)n + m) * 8);
   w->d_s = (double *)b200_malloc((size_t)n * 8);
@@ -402,7 +439,7 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
   if (!w->d_diag_r || !w->d_b || !w->d_s || !w->cg.d_M || !w->cg.d_r ||
       !w->cg.d_Gp || !w->cg.d_z || !w->cg.d_tmp || !w->cg.d_ctl || !w->cg.d_partials ||
       !w->cg.d_counter || !w->cg.h_ctl || !w->cg.d_red || !w->cg.d_ry_inv)
-    goto fail;
+    return -1;
   b200_memset0(w->cg.d_counter, 64);
   b200_memset0(w->cg.d_ctl, sizeof(B200CgCtl));
   memset(w->cg.h_ctl, 0, sizeof(B200CgCtl));
@@ -420,7 +457,7 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
     sig.nranks = w->nranks; sig.rank = w->rank;
     for (r = 0; r < w->nranks && r < 8; ++r) sig.flags[r] = b200_p2p_flags(r);
     w->cg.d_p2p_sig = (B200P2pSignal *)b200_malloc(sizeof(sig));
-    if (!w->cg.d_p2p_sig || b200_h2d(w->cg.d_p2p_sig, &sig, sizeof(sig)) != 0) goto fail;
+    if (!w->cg.d_p2p_sig || b200_h2d(w->cg.d_p2p_sig, &sig, sizeof(sig)) != 0) return -1;
     /* sharded-x push mode (kernels/cg.cu k_cgx_iteration): p lives in the exchange allocation so that the peers can
      * store their slices into it, and the K2 SpMV pushes its rows to the owners' inboxes. Needs the flagged-stream
      * kernel without virtual rows for A' and the (single) exchange p vector. */
@@ -437,24 +474,21 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
       w->p_in_exchange = 1;
       w->cg.d_p = b200_p2p_pvec(w->rank);
       w->cg.d_p2p_route = (B200P2pRoute *)b200_malloc(sizeof(rt));
-      if (!w->cg.d_p2p_route || b200_h2d(w->cg.d_p2p_route, &rt, sizeof(rt)) != 0) goto fail;
+      if (!w->cg.d_p2p_route || b200_h2d(w->cg.d_p2p_route, &rt, sizeof(rt)) != 0) return -1;
     }
   }
   if (!w->cg.d_p) {
     w->cg.d_p = (double *)b200_malloc((size_t)n * 8);
-    if (!w->cg.d_p) goto fail;
+    if (!w->cg.d_p) return -1;
   }
-  if (b200_h2d(w->d_diag_r, diag_r, ((size_t)n + m) * 8) != 0) goto fail;
-  if (b200_cg_set_preconditioner(&w->cg, w->d_Pdiag) != 0) goto fail;
-  if (b200_sync() != 0) goto fail;
+  if (b200_h2d(w->d_diag_r, diag_r, ((size_t)n + m) * 8) != 0) return -1;
+  if (b200_cg_set_preconditioner(&w->cg, w->d_Pdiag) != 0) return -1;
+  if (b200_sync() != 0) return -1;
   setup_mark("linsys: vectors, preconditioner", &t_mark);
-  if (cg_ops_build(w) != 0 || cg_ops_refresh(w) != 0 || b200_sync() != 0) goto fail;
+  if (cg_ops_build(w) != 0 || cg_ops_refresh(w) != 0 || b200_sync() != 0) return -1;
   setup_mark("linsys: reordered pair for the CG operator", &t_mark);
-  return w;
-fail:
-  fprintf(stderr, "scs_b200: init_lin_sys_work failed: %s\n", b200_last_error());
-  scs_free_lin_sys_work(w);
-  return SCS_NULL;
+  *t_mark_p = t_mark;
+  return 0;
 }
 
 void scs_free_lin_sys_work(ScsLinSysWork *w) {

@@ -37,6 +37,8 @@ struct SCS_LIN_SYS_WORK {
 int b200_linsys_solve_dev(ScsLinSysWork *w, double *d_b, const double *d_s, double tol,
                           const double *d_tol);
 int b200_linsys_update_diag_r_dev(ScsLinSysWork *w, const double *d_diag_r);
+ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B200Spmv *P, double *d_Pdiag,
+                                    const scs_float *diag_r);
 int b200_linsys_full_equilibrate(const ScsMatrix *A, const int *bnd, int nbnd, double *d_D, double *d_E);
 int b200_linsys_scale_local(ScsLinSysWork *w, const double *d_D, const double *d_E);
 /* contiguous row blocks balanced by nonzeros; offsets[nranks+1] (also exported for the tests) */

@@ -111,6 +111,89 @@ static int validate_matrix(const ScsMatrix *A, const ScsMatrix *P) {
   return 0;
 }
 
+/* The caller's device CSC arrays, validated and copied into the library's own int32 / fp64 blocks */
+typedef struct {
+  int *Ap, *Ai, *Pp, *Pi;
+  double *Ax, *Px;
+  long long nnzA, nnzP, fullP;
+} DevMats;
+static void dev_mats_free(DevMats *dm) {
+  b200_free(dm->Ap); b200_free(dm->Ai); b200_free(dm->Ax);
+  b200_free(dm->Pp); b200_free(dm->Pi); b200_free(dm->Px);
+  memset(dm, 0, sizeof(*dm));
+}
+static scs_int read_dev_int(const scs_int *d_v) {
+  scs_int v = -1;
+  if (b200_d2h(&v, d_v, sizeof(scs_int)) != 0 || b200_sync() != 0) return -1;
+  return v;
+}
+/* validate_matrix on device arrays: the same checks, in the same order, with the same messages. The host reads p[n],
+ * then the pointer flags, then the first failing entry: no kernel reads an index before the check that guards it. */
+static int validate_matrix_dev(const ScsMatrix *A, const ScsMatrix *P, DevMats *dm) {
+  const int idx64 = sizeof(scs_int) == 8;
+  unsigned flags = 0;
+  unsigned long long first = 0;
+  long long ndiag = 0;
+  scs_int Anz;
+  if (!A) { printf("A matrix missing\n"); return -1; }
+  if (A->m <= 0 || A->n <= 0) { printf("A matrix dimensions must be positive\n"); return -1; }
+  if (!A->x || !A->i || !A->p) { printf("data incompletely specified\n"); return -1; }
+  Anz = read_dev_int(A->p + A->n);
+  dm->Ap = (int *)b200_malloc(((size_t)A->n + 1) * 4);
+  if (!dm->Ap || b200_csc_check_ptrs((int)A->n, (long long)Anz, A->p, idx64, dm->Ap, &flags) != 0) return -1;
+  if (flags & B200_CSC_BAD_P0) { printf("A->p[0] must equal 0\n"); return -1; }
+  if (b200_over_stored("nnz(A) = A->p[n]", Anz)) return -1;
+  if (flags & B200_CSC_BAD_PTR) { printf("A->p (column pointers) must be nonnegative and nondecreasing\n"); return -1; }
+  if (((double)Anz / A->m > A->n) || Anz < 0) {
+    printf("Anz (nonzeros in A) = %li, outside of valid range\n", (long)Anz);
+    return -1;
+  }
+  dm->nnzA = Anz;
+  dm->Ai = (int *)b200_malloc((size_t)Anz * 4);
+  dm->Ax = (double *)b200_malloc((size_t)Anz * 8);
+  if (!dm->Ai || !dm->Ax ||
+      b200_csc_copy_entries((int)A->m, (int)A->n, Anz, A->i, A->x, idx64, dm->Ap, 0, dm->Ai, dm->Ax, &first, &ndiag) != 0)
+    return -1;
+  if (first != ~0ULL) {
+    const long long kk = (long long)(first >> 2);
+    if ((first & 3) == B200_CSC_BAD_ROW) {
+      printf("A row index %li outside valid range [0, %li]\n", (long)read_dev_int(A->i + kk), (long)A->m - 1);
+    } else {
+      printf("A contains a non-finite entry\n");
+    }
+    return -1;
+  }
+  if (P) {
+    scs_int Pnz;
+    if (!P->x || !P->i || !P->p) { printf("P matrix incompletely specified\n"); return -1; }
+    if (P->n != A->n) { printf("P dimension inconsistent with n\n"); return -1; }
+    if (P->m != P->n) { printf("P is not square\n"); return -1; }
+    Pnz = read_dev_int(P->p + P->n);
+    dm->Pp = (int *)b200_malloc(((size_t)P->n + 1) * 4);
+    if (!dm->Pp || b200_csc_check_ptrs((int)P->n, (long long)Pnz, P->p, idx64, dm->Pp, &flags) != 0) return -1;
+    if (flags & B200_CSC_BAD_P0) { printf("P->p[0] must equal 0\n"); return -1; }
+    if (b200_over_stored("nnz(P) = P->p[n]", Pnz)) return -1;
+    if (flags & B200_CSC_BAD_PTR) { printf("P->p (column pointers) must be nonnegative and nondecreasing\n"); return -1; }
+    if (((double)Pnz / P->m > P->n) || Pnz < 0) { printf("Pnz outside of valid range\n"); return -1; }
+    dm->nnzP = Pnz;
+    dm->Pi = (int *)b200_malloc((size_t)Pnz * 4);
+    dm->Px = (double *)b200_malloc((size_t)Pnz * 8);
+    if (!dm->Pi || !dm->Px ||
+        b200_csc_copy_entries((int)P->n, (int)P->n, Pnz, P->i, P->x, idx64, dm->Pp, 1, dm->Pi, dm->Px, &first,
+                              &ndiag) != 0)
+      return -1;
+    if (first != ~0ULL) {
+      const int code = (int)(first & 3);
+      printf(code == B200_CSC_BAD_ROW ? "P row index outside valid range\n"
+             : code == B200_CSC_BAD_UPPER ? "P is not upper triangular\n" : "P contains a non-finite entry\n");
+      return -1;
+    }
+    dm->fullP = 2 * (long long)Pnz - ndiag;
+    if (b200_over_stored("stored entries of the full symmetric P", dm->fullP)) return -1;
+  }
+  return 0;
+}
+
 static int validate_cones(const ScsData *d, const ScsCone *k) {
   scs_int i;
   long long dims;
@@ -195,7 +278,7 @@ static int validate_cones(const ScsData *d, const ScsCone *k) {
   return 0;
 }
 
-static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
+static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm) {
   if (d->m <= 0 || d->n <= 0) {
     printf("m and n must both be greater than 0; m = %li, n = %li\n", (long)d->m, (long)d->n);
     return -1;
@@ -206,7 +289,10 @@ static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs)
     return -1;
   }
   if (!d->b || !d->c) { printf("b or c missing\n"); return -1; }
-  if (validate_matrix(d->A, d->P) < 0) { printf("invalid linear system input data\n"); return -1; }
+  if ((dm ? validate_matrix_dev(d->A, d->P, dm) : validate_matrix(d->A, d->P)) < 0) {
+    printf("invalid linear system input data\n");
+    return -1;
+  }
   if (validate_cones(d, k) < 0) { printf("cone validation error\n"); return -1; }
   if (stgs->max_iters <= 0) { printf("max_iters must be positive\n"); return -1; }
   if (!isfinite(stgs->eps_abs) || stgs->eps_abs < 0) { printf("eps_abs tolerance must be a nonnegative finite number\n"); return -1; }
@@ -292,6 +378,7 @@ void scs_finish(ScsWork *w) {
   b200_free(w->d_b); b200_free(w->d_c); b200_free(w->d_D); b200_free(w->d_E);
   b200_free(w->d_ax); b200_free(w->d_aty); b200_free(w->d_px);
   b200_free(w->d_sol_x); b200_free(w->d_sol_y); b200_free(w->d_sol_s);
+  b200_free(w->d_b_orig); b200_free(w->d_c_orig);
   init_mark("finish: device vectors", &t_mark);
   b200_host_free(w->h_sc);
   init_mark("finish: pinned scalars", &t_mark);
@@ -360,6 +447,11 @@ scs_int scs_update(ScsWork *w, scs_float *b, scs_float *c) {
   const double t0 = now_ms();
   const int n = w->n, m = w->m;
   int i;
+  /* originals last set through scs_b200_update_device and kept here: their host copies are brought up to date */
+  if ((!b && w->b_on_dev && b200_d2h(w->b_orig, w->d_b_orig, (size_t)m * 8) != 0) ||
+      (!c && w->c_on_dev && b200_d2h(w->c_orig, w->d_c_orig, (size_t)n * 8) != 0) || b200_sync() != 0)
+    return -1;
+  w->b_on_dev = w->c_on_dev = w->bc_host_stale = 0;
   if (b) {
     if (w->b_orig != b) memcpy(w->b_orig, b, (size_t)m * sizeof(double));
     w->nm_b_orig = 0.0;
@@ -405,7 +497,13 @@ static void print_header(const ScsWork *w) {
          (long)w->nnzA, (long)w->nnzP);
 }
 
-ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
+static int update_bc_dev(ScsWork *w);
+static int build_ops_dev(ScsWork *w, DevMats *dm);
+static void write_data_dev(const char *filename, const ScsData *d, const ScsCone *k, const ScsSettings *stgs);
+
+/* dm == NULL: scs_init, the data in host memory. Else the device-data entry point: d's arrays are device pointers,
+ * validated into dm's blocks, from which the operators are built on the device (build_ops_dev) */
+static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm) {
   ScsWork *w;
   const double t0 = now_ms();
   double t_mark = t0;
@@ -416,7 +514,7 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
     printf("ERROR: Missing ScsData, ScsCone, or ScsSettings input\n");
     return SCS_NULL;
   }
-  if (validate(d, k, stgs) < 0) {
+  if (validate(d, k, stgs, dm) < 0) {
     printf("ERROR: Validation returned failure\n");
     return SCS_NULL;
   }
@@ -426,7 +524,8 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   }
   if (stgs->write_data_filename) { /* reference scs.c:1270-1273 */
     printf("Writing raw problem data to %s\n", stgs->write_data_filename);
-    scs_b200_write_data(stgs->write_data_filename, d, k, stgs);
+    if (dm) write_data_dev(stgs->write_data_filename, d, k, stgs);
+    else scs_b200_write_data(stgs->write_data_filename, d, k, stgs);
   }
   w = (ScsWork *)calloc(1, sizeof(ScsWork));
   if (!w) return SCS_NULL;
@@ -439,17 +538,23 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   w->stgs = (ScsSettings *)calloc(1, sizeof(ScsSettings));
   if (!w->d || !w->k || !w->stgs) goto fail;
   w->d->n = n; w->d->m = m;
-  w->nnzA = d->A->p[n];
-  w->nnzP = d->P ? d->P->p[n] : 0;
+  w->nnzA = dm ? dm->nnzA : d->A->p[n];
+  w->nnzP = dm ? dm->nnzP : d->P ? d->P->p[n] : 0;
   /* Equilibrate on the device when possible (P = 0, single GPU): the user's A is uploaded as
    * is and both resident orientations are rescaled in place (kernels/equil.cu), so no host
    * copy of A is needed at all. Otherwise (P != 0 or row-sharded) equilibrate a host copy. */
   dev_equil = stgs->normalize && !d->P && !getenv("SCS_B200_HOST_EQUIL");
-  w->d->A = dev_equil ? SCS_NULL : copy_matrix(d->A);
-  w->d->P = d->P ? copy_matrix(d->P) : SCS_NULL;
-  w->d->b = (double *)dup_mem(d->b, (size_t)m * 8);
-  w->d->c = (double *)dup_mem(d->c, (size_t)n * 8);
-  if ((!dev_equil && !w->d->A) || (d->P && !w->d->P) || !w->d->b || !w->d->c) goto fail;
+  if (dm) { /* no host copy of A or P; the host copies of b and c are filled when a host call needs them */
+    w->d->b = (double *)malloc((size_t)m * 8);
+    w->d->c = (double *)malloc((size_t)n * 8);
+    if (!w->d->b || !w->d->c) goto fail;
+  } else {
+    w->d->A = dev_equil ? SCS_NULL : copy_matrix(d->A);
+    w->d->P = d->P ? copy_matrix(d->P) : SCS_NULL;
+    w->d->b = (double *)dup_mem(d->b, (size_t)m * 8);
+    w->d->c = (double *)dup_mem(d->c, (size_t)n * 8);
+    if ((!dev_equil && !w->d->A) || (d->P && !w->d->P) || !w->d->b || !w->d->c) goto fail;
+  }
   *w->k = *k;
   w->k->bu = w->k->bl = SCS_NULL; w->k->q = SCS_NULL; w->k->s = SCS_NULL;
   w->k->cs = SCS_NULL; w->k->p = SCS_NULL;
@@ -501,7 +606,7 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
     w->D = (double *)malloc((size_t)m * 8);
     w->E = (double *)malloc((size_t)n * 8);
     if (!w->D || !w->E) goto fail;
-    if (!dev_equil) {
+    if (!dev_equil && !dm) {
       if (b200_equilibrate(w->d->P, w->d->A, w->cone_boundaries, w->cone_boundaries_len, w->D, w->E) != 0)
         goto fail;
       if (w->k->bsize > 1) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
@@ -525,14 +630,14 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   w->d_c = (double *)b200_malloc((size_t)n * 8);
   w->d_ax = (double *)b200_malloc((size_t)m * 8);
   w->d_aty = (double *)b200_malloc((size_t)n * 8);
-  w->d_px = w->d->P ? (double *)b200_malloc((size_t)n * 8) : SCS_NULL;
+  w->d_px = d->P ? (double *)b200_malloc((size_t)n * 8) : SCS_NULL;
   w->d_sol_x = (double *)b200_malloc((size_t)n * 8);
   w->d_sol_y = (double *)b200_malloc((size_t)m * 8);
   w->d_sol_s = (double *)b200_malloc((size_t)m * 8);
   w->h_sc = (double *)b200_host_alloc(SC_COUNT * 8);
   if (!w->adm.d_u || !w->adm.d_u_t || !w->adm.d_v || !w->adm.d_v_prev || !w->adm.d_rsk ||
       !w->adm.d_g || !w->adm.d_R || !w->adm.d_ws || !w->adm.d_sc || !w->adm.d_part ||
-      !w->adm.d_cnt || !w->d_b || !w->d_c || !w->d_ax || !w->d_aty || (w->d->P && !w->d_px) ||
+      !w->adm.d_cnt || !w->d_b || !w->d_c || !w->d_ax || !w->d_aty || (d->P && !w->d_px) ||
       !w->d_sol_x || !w->d_sol_y || !w->d_sol_s || !w->h_sc) {
     printf("ERROR: device memory allocation failure: %s\n", b200_last_error());
     goto fail;
@@ -551,14 +656,17 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
     w->d_D = (double *)b200_malloc((size_t)m * 8);
     w->d_E = (double *)b200_malloc((size_t)n * 8);
     if (!w->d_D || !w->d_E) goto fail;
-    if (!dev_equil) {
+    if (!dev_equil && !dm) {
       i |= b200_h2d(w->d_D, w->D, (size_t)m * 8);
       i |= b200_h2d(w->d_E, w->E, (size_t)n * 8);
     }
   }
   if (i != 0) goto fail;
   init_mark("init: validate, copies, device vectors", &t_mark);
-  if (dev_equil) {
+  if (dm) {
+    if (build_ops_dev(w, dm) != 0) goto fail;
+    init_mark("init: operators, equilibration and preconditioner from device data", &t_mark);
+  } else if (dev_equil) {
     /* upload the raw A (both orientations), equilibrate in place on the device */
     if (b200_comm_nranks() > 1) {
       /* row-sharded: D, E from temporary full copies, then scale the resident row block once */
@@ -582,9 +690,19 @@ ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
     init_mark("init: device equilibration + preconditioner", &t_mark);
   }
   /* b, c: stores *_orig, normalises, uploads */
-  memcpy(w->b_orig, d->b, (size_t)m * 8);
-  memcpy(w->c_orig, d->c, (size_t)n * 8);
-  if (scs_update(w, w->b_orig, w->c_orig) != 0) goto fail;
+  if (dm) {
+    w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
+    w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
+    if (!w->d_b_orig || !w->d_c_orig || b200_d2d(w->d_b_orig, d->b, (size_t)m * 8) != 0 ||
+        b200_d2d(w->d_c_orig, d->c, (size_t)n * 8) != 0)
+      goto fail;
+    w->b_on_dev = w->c_on_dev = 1;
+    if (update_bc_dev(w) != 0) goto fail;
+  } else {
+    memcpy(w->b_orig, d->b, (size_t)m * 8);
+    memcpy(w->c_orig, d->c, (size_t)n * 8);
+    if (scs_update(w, w->b_orig, w->c_orig) != 0) goto fail;
+  }
 
   /* the kernel layer takes int copies of the cone arrays (validated below 2^30) */
   if (b200_cone_ints(w->k, &ci) != 0) goto fail;
@@ -624,6 +742,8 @@ fail:
   scs_finish(w);
   return SCS_NULL;
 }
+
+ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) { return init_work(d, k, stgs, SCS_NULL); }
 
 /* ----------------------------------------------------------------- residuals */
 static void compute_residuals(B200Residuals *r, double pd) {
@@ -742,9 +862,10 @@ static int update_work(ScsWork *w, ScsSolution *sol) {
   w->r_norm.last_iter = -1;
   w->r_orig.last_iter = -1;
   if (w->stgs->warm_start && sol && sol->x && sol->y && sol->s) {
-    if (b200_h2d(w->d_sol_x, sol->x, (size_t)n * 8) != 0) return -1;
-    if (b200_h2d(w->d_sol_y, sol->y, (size_t)m * 8) != 0) return -1;
-    if (b200_h2d(w->d_sol_s, sol->s, (size_t)m * 8) != 0) return -1;
+    int (*in)(void *, const void *, size_t) = w->sol_on_dev ? b200_d2d : b200_h2d;
+    if (in(w->d_sol_x, sol->x, (size_t)n * 8) != 0) return -1;
+    if (in(w->d_sol_y, sol->y, (size_t)m * 8) != 0) return -1;
+    if (in(w->d_sol_s, sol->s, (size_t)m * 8) != 0) return -1;
     if (w->D && b200_admm_normalize_sol(n, m, w->d_D, w->d_E, w->primal_scale, w->dual_scale,
                                         w->d_sol_x, w->d_sol_y, w->d_sol_s) != 0)
       return -1;
@@ -839,7 +960,11 @@ static int failure(ScsWork *w, int m, int n, ScsSolution *sol, ScsInfo *info, in
     memset(&info->aa_stats, 0, sizeof(info->aa_stats));
     info->aa_stats.last_aa_norm = NAN;
   }
-  if (sol) {
+  if (sol && w && w->sol_on_dev) { /* device buffers, checked at entry */
+    b200_vec_fill(n, sol->x, NAN);
+    b200_vec_fill(m, sol->y, NAN);
+    b200_vec_fill(m, sol->s, NAN);
+  } else if (sol) {
     if (n > 0) {
       if (!sol->x) sol->x = (double *)calloc((size_t)n, sizeof(double));
       if (sol->x) fill_nan(sol->x, n);
@@ -851,7 +976,6 @@ static int failure(ScsWork *w, int m, int n, ScsSolution *sol, ScsInfo *info, in
       if (sol->s) fill_nan(sol->s, m);
     }
   }
-  (void)w;
   printf("Failure:%s\n", msg);
   end_interrupt_listener(); /* every failure() inside scs_solve leaves the solve; outside it the count is 0: no-op */
   return status;
@@ -878,9 +1002,12 @@ static int finalize(ScsWork *w, ScsSolution *sol, ScsInfo *info, int iter) {
   const B200Residuals *r = &w->r_orig;
   double fx = 1.0, fy = 1.0, fs = 1.0; /* NaN means "fill with NaN" */
   double nm_s, nm_y, sty;
-  if (!sol->x) sol->x = (double *)calloc((size_t)n, sizeof(double));
-  if (!sol->y) sol->y = (double *)calloc((size_t)m, sizeof(double));
-  if (!sol->s) sol->s = (double *)calloc((size_t)m, sizeof(double));
+  int (*out)(void *, const void *, size_t) = w->sol_on_dev ? b200_d2d : b200_d2h;
+  if (!w->sol_on_dev) {
+    if (!sol->x) sol->x = (double *)calloc((size_t)n, sizeof(double));
+    if (!sol->y) sol->y = (double *)calloc((size_t)m, sizeof(double));
+    if (!sol->s) sol->s = (double *)calloc((size_t)m, sizeof(double));
+  }
   if (!sol->x || !sol->y || !sol->s) return -1;
   if (b200_admm_unnormalize_sol(&w->adm, w->d_D, w->d_E, w->primal_scale, w->dual_scale, w->d_sol_x,
                                 w->d_sol_y, w->d_sol_s) != 0)
@@ -960,9 +1087,9 @@ static int finalize(ScsWork *w, ScsSolution *sol, ScsInfo *info, int iter) {
   else if (b200_vec_scale(m, w->d_sol_y, fy) != 0) return -1;
   if (isnan(fs)) { if (b200_vec_fill(m, w->d_sol_s, NAN) != 0) return -1; }
   else if (b200_vec_scale(m, w->d_sol_s, fs) != 0) return -1;
-  if (b200_d2h(sol->x, w->d_sol_x, (size_t)n * 8) != 0) return -1;
-  if (b200_d2h(sol->y, w->d_sol_y, (size_t)m * 8) != 0) return -1;
-  if (b200_d2h(sol->s, w->d_sol_s, (size_t)m * 8) != 0) return -1;
+  if (out(sol->x, w->d_sol_x, (size_t)n * 8) != 0) return -1;
+  if (out(sol->y, w->d_sol_y, (size_t)m * 8) != 0) return -1;
+  if (out(sol->s, w->d_sol_s, (size_t)m * 8) != 0) return -1;
   return b200_sync();
 }
 
@@ -1009,6 +1136,12 @@ static int log_data_to_csv(ScsWork *w, int iter, double t_solve) {
   long long i;
   if (!f) return 0;
   if (populate_residual_struct(w, iter) != 0) return -1;
+  if (w->bc_host_stale) { /* set on the device (scs_b200_update_device): a debugging mode may copy them here */
+    if (b200_d2h(w->d->b, w->d_b, (size_t)m * 8) != 0 || b200_d2h(w->d->c, w->d_c, (size_t)n * 8) != 0 ||
+        b200_sync() != 0)
+      return -1;
+    w->bc_host_stale = 0;
+  }
   if (!w->log_host) {
     w->log_host = (double *)malloc((size_t)(5 * l + m + 2 * (long long)n) * sizeof(double));
     if (!w->log_host) return -1;
@@ -1299,3 +1432,197 @@ scs_int scs_b200_set_max_iters(ScsWork *w, scs_int max_iters) {
 }
 long long scs_b200_launch_count(void) { return b200_launches(); }
 scs_int scs_b200_device_ok(void) { return b200_device_ok(); }
+
+/* ----------------------------------------------------------------- device-data entry points */
+/* scs_update's normalisation on the device originals: b200_normalize_b_c's products and maxima, bit for bit; the
+ * four maxima are the only values that reach the host */
+static int update_bc_dev(ScsWork *w) {
+  const double t0 = now_ms();
+  double mx[4], sigma;
+  if (b200_normalize_b_c_dev(w->m, w->n, w->d_b_orig, w->d_c_orig, w->D ? w->d_D : SCS_NULL, w->D ? w->d_E : SCS_NULL,
+                             w->d_b, w->d_c, mx) != 0)
+    return -1;
+  w->nm_b_orig = mx[0];
+  w->nm_c_orig = mx[2];
+  if (w->D) {
+    sigma = mx[3] > mx[1] ? mx[3] : mx[1];
+    sigma = sigma < 1e-4 ? 1.0 : sigma;
+    sigma = sigma > 1e4 ? 1e4 : sigma;
+    sigma = SAFEDIV_POS(1.0, sigma);
+    if (b200_scale_b_c(w->m, w->n, w->d_b, w->d_c, sigma) != 0) return -1;
+    w->primal_scale = sigma;
+    w->dual_scale = sigma;
+  }
+  if (b200_sync() != 0) return -1;
+  w->bc_host_stale = 1;
+  w->setup_time = now_ms() - t0;
+  return 0;
+}
+
+/* the linear-system workspace from dm's blocks: both operators of A; with P, the structure of the full P, the
+ * P-aware equilibration on the device and then P's operator and diagonal; with P = 0, the equilibration scs_init
+ * uses: b200_equilibrate_dev on the built pair, or, where scs_init equilibrates on the host (SCS_B200_HOST_EQUIL),
+ * b200_equilibrate_qp_dev with an empty P, which is host/equilibrate.c bit for bit */
+static int build_ops_dev(ScsWork *w, DevMats *dm) {
+  const int n = w->n, m = w->m;
+  B200Spmv *A = SCS_NULL, *At = SCS_NULL, *P = SCS_NULL;
+  int *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL, *Pp0 = SCS_NULL;
+  double *d_Pdiag = SCS_NULL;
+  const int host_order = !dm->Pp && w->D && getenv("SCS_B200_HOST_EQUIL");
+  int rc = -1;
+  do {
+    if (b200_setup_ops_from_dev(m, n, dm->nnzA, dm->Ap, dm->Ai, dm->Ax, &A, &At) != 0) break;
+    if (host_order) { /* P = 0 as an n x n matrix without entries: its column and row ranges are all empty */
+      Pp0 = (int *)b200_malloc(((size_t)n + 1) * 4);
+      if (!Pp0 || b200_memset0(Pp0, ((size_t)n + 1) * 4) != 0 ||
+          b200_equilibrate_qp_dev(A, At, Pp0, SCS_NULL, SCS_NULL, Pp0, SCS_NULL, SCS_NULL, w->cone_boundaries,
+                                  w->cone_boundaries_len, w->d_D, w->d_E) != 0)
+        break;
+    }
+    if (dm->Pp) {
+      Fp = (int *)b200_malloc(((size_t)n + 1) * 4);
+      Fi = (int *)b200_malloc((size_t)dm->fullP * 4);
+      Fsrc = (int *)b200_malloc((size_t)dm->fullP * 4);
+      d_Pdiag = (double *)b200_malloc((size_t)n * 8);
+      if (!Fp || !Fi || !Fsrc || !d_Pdiag ||
+          b200_sym_expand_structure(n, dm->nnzP, dm->fullP, dm->Pp, dm->Pi, Fp, Fi, Fsrc) != 0)
+        break;
+      if (w->D && b200_equilibrate_qp_dev(A, At, dm->Pp, dm->Pi, dm->Px, Fp, Fi, Fsrc, w->cone_boundaries,
+                                          w->cone_boundaries_len, w->d_D, w->d_E) != 0)
+        break;
+      if (b200_sym_build(n, dm->fullP, Fp, Fi, Fsrc, dm->Px, d_Pdiag, &P) != 0) break;
+    }
+    w->p = b200_linsys_from_ops(m, n, A, At, P, d_Pdiag, w->h_diag_r); /* takes them over */
+    A = At = P = SCS_NULL;
+    d_Pdiag = SCS_NULL;
+    if (!w->p) break;
+    if (w->D && !dm->Pp && !host_order) {
+      if (b200_equilibrate_dev(w->p->A, w->p->At, w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0 ||
+          b200_linsys_update_diag_r_dev(w->p, w->p->d_diag_r) != 0)
+        break;
+    }
+    if (w->D) {
+      if (b200_d2h(w->D, w->d_D, (size_t)m * 8) != 0 || b200_d2h(w->E, w->d_E, (size_t)n * 8) != 0 ||
+          b200_sync() != 0)
+        break;
+      if (w->k->bsize > 1) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
+    }
+    rc = 0;
+  } while (0);
+  b200_sync();
+  b200_spmv_destroy(A); b200_spmv_destroy(At); b200_spmv_destroy(P);
+  b200_free(Fp); b200_free(Fi); b200_free(Fsrc); b200_free(d_Pdiag); b200_free(Pp0);
+  return rc;
+}
+
+/* ScsSettings.write_data_filename with device data: a debugging mode, the arrays are copied to the host to be written */
+static int dev_to_host(void **dst, const void *d_src, size_t bytes) {
+  *dst = malloc(bytes ? bytes : 1);
+  return *dst && b200_d2h(*dst, d_src, bytes) == 0 ? 0 : -1;
+}
+static void write_data_dev(const char *filename, const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
+  ScsData hd = *d;
+  ScsMatrix hA = *d->A, hP;
+  const long long nnzA = read_dev_int(d->A->p + d->A->n), nnzP = d->P ? read_dev_int(d->P->p + d->P->n) : 0;
+  int ok = dev_to_host((void **)&hA.p, d->A->p, ((size_t)d->n + 1) * sizeof(scs_int)) == 0 &&
+           dev_to_host((void **)&hA.i, d->A->i, (size_t)nnzA * sizeof(scs_int)) == 0 &&
+           dev_to_host((void **)&hA.x, d->A->x, (size_t)nnzA * 8) == 0 &&
+           dev_to_host((void **)&hd.b, d->b, (size_t)d->m * 8) == 0 &&
+           dev_to_host((void **)&hd.c, d->c, (size_t)d->n * 8) == 0;
+  hd.A = &hA;
+  hd.P = SCS_NULL;
+  memset(&hP, 0, sizeof(hP));
+  if (d->P) {
+    hP = *d->P;
+    hP.p = SCS_NULL; hP.i = SCS_NULL; hP.x = SCS_NULL;
+    ok = ok && dev_to_host((void **)&hP.p, d->P->p, ((size_t)d->n + 1) * sizeof(scs_int)) == 0 &&
+         dev_to_host((void **)&hP.i, d->P->i, (size_t)nnzP * sizeof(scs_int)) == 0 &&
+         dev_to_host((void **)&hP.x, d->P->x, (size_t)nnzP * 8) == 0;
+    hd.P = &hP;
+  }
+  if (ok && b200_sync() == 0) scs_b200_write_data(filename, &hd, k, stgs);
+  else printf("Error: could not copy the problem data to the host for %s\n", filename);
+  free(hA.p); free(hA.i); free(hA.x); free(hP.p); free(hP.i); free(hP.x); free(hd.b); free(hd.c);
+}
+
+/* a device pointer of the library's device, else a message and 0 */
+static int dev_ptr_ok(const void *p, const char *what) {
+  if (b200_is_device_ptr(p)) return 1;
+  printf("ERROR: %s must point to device memory of the library's CUDA device\n", what);
+  return 0;
+}
+static int single_gpu(void) {
+  if (b200_comm_nranks() <= 1) return 1;
+  printf("ERROR: the device-data entry points drive a single GPU; this process is one of %d ranks\n",
+         b200_comm_nranks());
+  return 0;
+}
+
+ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, void *stream) {
+  DevMats dm;
+  ScsWork *w;
+  memset(&dm, 0, sizeof(dm));
+  if (!d || !k || !stgs) {
+    printf("ERROR: Missing ScsData, ScsCone, or ScsSettings input\n");
+    return SCS_NULL;
+  }
+  if (b200_runtime_init() != 0) {
+    printf("ERROR: scs_b200 needs an sm_90 (H100) CUDA device: %s\n", b200_last_error());
+    return SCS_NULL;
+  }
+  if (!single_gpu()) return SCS_NULL;
+  if ((d->A && ((d->A->p && !dev_ptr_ok(d->A->p, "A->p")) || (d->A->i && !dev_ptr_ok(d->A->i, "A->i")) ||
+                (d->A->x && !dev_ptr_ok(d->A->x, "A->x")))) ||
+      (d->P && ((d->P->p && !dev_ptr_ok(d->P->p, "P->p")) || (d->P->i && !dev_ptr_ok(d->P->i, "P->i")) ||
+                (d->P->x && !dev_ptr_ok(d->P->x, "P->x")))) ||
+      (d->b && !dev_ptr_ok(d->b, "b")) || (d->c && !dev_ptr_ok(d->c, "c"))) {
+    printf("ERROR: Validation returned failure\n");
+    return SCS_NULL;
+  }
+  if (b200_wait_for_caller(stream) != 0) return SCS_NULL;
+  w = init_work(d, k, stgs, &dm);
+  b200_sync(); /* the builder's blocks are free only once its kernels have run */
+  dev_mats_free(&dm);
+  b200_caller_waits(stream);
+  return w;
+}
+
+scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream) {
+  const int n = w ? w->n : 0, m = w ? w->m : 0;
+  int rc = -1;
+  if (!w || !single_gpu() || (d_b && !dev_ptr_ok(d_b, "b")) || (d_c && !dev_ptr_ok(d_c, "c"))) return -1;
+  if (b200_wait_for_caller(stream) != 0) return -1;
+  do {
+    if (!w->d_b_orig) w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
+    if (!w->d_c_orig) w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
+    if (!w->d_b_orig || !w->d_c_orig) break;
+    /* an original kept from a host call is uploaded once (a workspace of scs_init, or after scs_update) */
+    if (d_b ? b200_d2d(w->d_b_orig, d_b, (size_t)m * 8) != 0
+            : !w->b_on_dev && b200_h2d(w->d_b_orig, w->b_orig, (size_t)m * 8) != 0)
+      break;
+    if (d_c ? b200_d2d(w->d_c_orig, d_c, (size_t)n * 8) != 0
+            : !w->c_on_dev && b200_h2d(w->d_c_orig, w->c_orig, (size_t)n * 8) != 0)
+      break;
+    w->b_on_dev = w->c_on_dev = 1;
+    rc = update_bc_dev(w);
+  } while (0);
+  b200_caller_waits(stream);
+  return rc;
+}
+
+scs_int scs_b200_solve_device(ScsWork *w, ScsSolution *d_sol, ScsInfo *info, scs_int warm_start, void *stream) {
+  scs_int status;
+  if (!w || !d_sol || !info) {
+    printf("ERROR: missing ScsWork, ScsSolution or ScsInfo input\n");
+    return -1;
+  }
+  if (!single_gpu() || !dev_ptr_ok(d_sol->x, "sol->x") || !dev_ptr_ok(d_sol->y, "sol->y") ||
+      !dev_ptr_ok(d_sol->s, "sol->s"))
+    return -1;
+  if (b200_wait_for_caller(stream) != 0) return -1;
+  w->sol_on_dev = 1;
+  status = scs_solve(w, d_sol, info, warm_start);
+  w->sol_on_dev = 0;
+  b200_caller_waits(stream);
+  return status;
+}

@@ -206,11 +206,58 @@ extern "C" void b200_host_free(void *p) {
   cudaFreeHost(p);
 }
 
+// Bytes and the largest single copy of b200_h2d and b200_d2h, per direction since the last reset (a copy staged in
+// chunks counts as one): what lets a caller check that a device-resident problem never crosses PCIe.
+static long long g_xfer[4];  // h2d bytes, h2d largest, d2h bytes, d2h largest
+static void count_xfer(int dir, size_t bytes) {
+  std::lock_guard<std::mutex> lk(g_stage_mu);
+  g_xfer[2 * dir] += (long long)bytes;
+  if ((long long)bytes > g_xfer[2 * dir + 1]) g_xfer[2 * dir + 1] = (long long)bytes;
+}
+extern "C" void scs_b200_transfer_stats(long long out[4]) {
+  std::lock_guard<std::mutex> lk(g_stage_mu);
+  for (int i = 0; i < 4; ++i) out[i] = g_xfer[i];
+}
+extern "C" void scs_b200_transfer_stats_reset(void) {
+  std::lock_guard<std::mutex> lk(g_stage_mu);
+  for (int i = 0; i < 4; ++i) g_xfer[i] = 0;
+}
+
+// 1 if p is device (or managed) memory of the library's device, else 0
+extern "C" int b200_is_device_ptr(const void *p) {
+  if (!p || b200_runtime_init() != 0) return 0;
+  cudaPointerAttributes at;
+  if (cudaPointerGetAttributes(&at, p) != cudaSuccess) {
+    cudaGetLastError();
+    return 0;
+  }
+  return (at.type == cudaMemoryTypeDevice || at.type == cudaMemoryTypeManaged) && at.device == g_dev;
+}
+// Ordering with a caller's stream (NULL: the legacy default stream). The library stream is non-blocking, so nothing
+// orders it with the caller's work implicitly: an event recorded on one stream is waited for by the other. Neither
+// call blocks the host.
+static cudaEvent_t g_ev_join = nullptr;
+static int join(cudaStream_t from, cudaStream_t to) {
+  if (!g_ev_join) CUDA_OK(cudaEventCreateWithFlags(&g_ev_join, cudaEventDisableTiming));
+  CUDA_OK(cudaEventRecord(g_ev_join, from));
+  CUDA_OK(cudaStreamWaitEvent(to, g_ev_join, 0));
+  return 0;
+}
+extern "C" int b200_wait_for_caller(void *caller_stream) {
+  if (b200_runtime_init() != 0) return -1;
+  return join((cudaStream_t)caller_stream, g_stream);
+}
+extern "C" int b200_caller_waits(void *caller_stream) {
+  if (b200_runtime_init() != 0) return -1;
+  return join(g_stream, (cudaStream_t)caller_stream);
+}
+
 // Host<->device copies. The caller's buffer may be pageable: stage through the
 // pinned bounce buffer in chunks so that the copy is a true async DMA and the
 // caller's memory can be reused as soon as the call returns.
 extern "C" int b200_h2d(void *d_dst, const void *src, size_t bytes) {
   if (b200_runtime_init() != 0) return -1;
+  count_xfer(0, bytes);
   cudaPointerAttributes at;
   bool pinned = (cudaPointerGetAttributes(&at, src) == cudaSuccess && at.type == cudaMemoryTypeHost);
   cudaGetLastError();
@@ -232,6 +279,7 @@ extern "C" int b200_h2d(void *d_dst, const void *src, size_t bytes) {
 }
 extern "C" int b200_d2h(void *dst, const void *d_src, size_t bytes) {
   if (b200_runtime_init() != 0) return -1;
+  count_xfer(1, bytes);
   cudaPointerAttributes at;
   bool pinned = (cudaPointerGetAttributes(&at, dst) == cudaSuccess && at.type == cudaMemoryTypeHost);
   cudaGetLastError();

@@ -118,16 +118,112 @@ static int narrow_csc(int m, int n, long long nnz, const long long *h_Ap64, cons
   return rc;
 }
 
-// Both operators from the host CSC of A (m x n; m, n or nnz may be 0): int32 arrays (h_Ap, h_Ai) or 64-bit ones
-// (h_Ap64, h_Ai64, narrowed on the device by k_narrow_csc). Returns 0 and sets *A_out (CSR of A) / *At_out (CSR of A' =
-// the CSC arrays); < 0 on failure.
-static int setup_ops(int m, int n, long long nnz, const int *h_Ap, const int *h_Ai, const long long *h_Ap64,
-                     const long long *h_Ai64, const double *h_Ax, B200Spmv **A_out, B200Spmv **At_out) {
+// The validating copy of a caller's device CSC (the device-data entry points) into the builder's int32 / fp64 arrays,
+// in two grid-stride passes templated on the index width (int, or the 64-bit indices of the DLONG ABI, narrowed as they are copied). The first pass copies the
+// column pointers and sets B200_CSC_BAD_P0 (p[0] != 0) or B200_CSC_BAD_PTR (a pointer decreases or leaves [0, nnz]).
+// The second runs only once the host has read a clean flag, so it may find an entry's column by bisection of the
+// copied pointers: it copies the row indices (and the values, when given) and records in *d_first the smallest
+// (k << 2 | code) of an entry that fails, code = B200_CSC_BAD_ROW (row outside [0, rows)), B200_CSC_BAD_UPPER (for P,
+// a row below the diagonal) or B200_CSC_BAD_VAL (a non-finite value), in the order the host checks each entry.
+// A truncated index (2^32 + 3 -> 3) is checked in its own width and would look valid if narrowed first.
+template <typename IdxT>
+__global__ void k_csc_copy_ptrs(int n, long long nnz, const IdxT *__restrict__ p, int *__restrict__ Ap,
+                                unsigned *__restrict__ d_bad) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  unsigned bad = 0;
+  for (long long j = blockIdx.x * (long long)blockDim.x + threadIdx.x; j <= n; j += stride) {
+    const long long v = (long long)p[j];
+    if (j == 0 && v != 0) bad |= B200_CSC_BAD_P0;
+    if (v < 0 || v > nnz || (j < n && (long long)p[j + 1] < v)) bad |= B200_CSC_BAD_PTR;
+    Ap[j] = (int)v;
+  }
+  if (bad) atomicOr(d_bad, bad);
+}
+template <typename IdxT>
+__global__ void k_csc_copy_entries(int rows, int n, long long nnz, const IdxT *__restrict__ pi,
+                                   const double *__restrict__ px, const int *__restrict__ Ap, int upper,
+                                   int *__restrict__ Ai, double *__restrict__ Ax,
+                                   unsigned long long *__restrict__ d_first, unsigned long long *__restrict__ d_ndiag) {
+  const long long stride = (long long)gridDim.x * blockDim.x;
+  unsigned long long first = ~0ULL, ndiag = 0;
+  for (long long k = blockIdx.x * (long long)blockDim.x + threadIdx.x; k < nnz; k += stride) {
+    const long long r = (long long)pi[k];
+    int code = -1;
+    if (r < 0 || r >= rows) code = B200_CSC_BAD_ROW;
+    if (upper && code < 0) {
+      int lo = 0, hi = n;  // the column j with Ap[j] <= k < Ap[j + 1]: the last pointer <= k
+      while (hi - lo > 1) {
+        const int mid = lo + (hi - lo) / 2;
+        if (Ap[mid] <= k) lo = mid; else hi = mid;
+      }
+      if (r > lo) code = B200_CSC_BAD_UPPER;
+      ndiag += r == lo;
+    }
+    if (px) {
+      const double v = px[k];
+      if (code < 0 && !isfinite(v)) code = B200_CSC_BAD_VAL;
+      Ax[k] = v;
+    }
+    if (code >= 0 && ((unsigned long long)k << 2 | (unsigned)code) < first) first = (unsigned long long)k << 2 | code;
+    Ai[k] = (int)r;
+  }
+  if (first != ~0ULL) atomicMin(d_first, first);
+  if (ndiag) atomicAdd(d_ndiag, ndiag);
+}
+
+static int csc_grid(long long work) {
+  const long long g = (work + 255) / 256, cap = 8LL * b200_num_sms();
+  return (int)(g < 1 ? 1 : g > cap ? cap : g);
+}
+// the pointer pass: *flags receives the B200_CSC_BAD_* bits of the pointers (one 4-byte read-back)
+extern "C" int b200_csc_check_ptrs(int n, long long nnz, const void *d_p, int idx64, int *d_Ap, unsigned *flags) {
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  unsigned *d_bad = (unsigned *)b200_malloc(4);
+  int rc = -1;
+  *flags = 0;
+  if (d_bad && b200_memset0(d_bad, 4) == 0) {
+    if (idx64) k_csc_copy_ptrs<<<csc_grid((long long)n + 1), 256, 0, st>>>(n, nnz, (const long long *)d_p, d_Ap, d_bad);
+    else k_csc_copy_ptrs<<<csc_grid((long long)n + 1), 256, 0, st>>>(n, nnz, (const int *)d_p, d_Ap, d_bad);
+    b200_count_launch(1);
+    if (cudaGetLastError() == cudaSuccess && b200_d2h(flags, d_bad, 4) == 0 && b200_sync() == 0) rc = 0;
+  }
+  b200_free(d_bad);
+  return rc;
+}
+// the entry pass, after a clean pointer pass: *first = ~0 when every entry is valid, else the smallest k << 2 | code;
+// *ndiag = the diagonal entries (upper != 0). d_x / d_Ax may be NULL (indices only). One 16-byte read-back.
+extern "C" int b200_csc_copy_entries(int rows, int n, long long nnz, const void *d_i, const double *d_x, int idx64,
+                                     const int *d_Ap, int upper, int *d_Ai, double *d_Ax, unsigned long long *first,
+                                     long long *ndiag) {
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  unsigned long long *d_out = (unsigned long long *)b200_malloc(16), h[2] = {~0ULL, 0};
+  int rc = -1;
+  if (d_out && cudaMemsetAsync(d_out, 0xff, 8, st) == cudaSuccess && b200_memset0(d_out + 1, 8) == 0) {
+    if (nnz > 0) {
+      if (idx64)
+        k_csc_copy_entries<<<csc_grid(nnz), 256, 0, st>>>(rows, n, nnz, (const long long *)d_i, d_x, d_Ap, upper,
+                                                          d_Ai, d_Ax, d_out, d_out + 1);
+      else
+        k_csc_copy_entries<<<csc_grid(nnz), 256, 0, st>>>(rows, n, nnz, (const int *)d_i, d_x, d_Ap, upper, d_Ai,
+                                                          d_Ax, d_out, d_out + 1);
+      b200_count_launch(1);
+    }
+    if (cudaGetLastError() == cudaSuccess && b200_d2h(h, d_out, 16) == 0 && b200_sync() == 0) rc = 0;
+  }
+  b200_free(d_out);
+  *first = h[0];
+  *ndiag = (long long)h[1];
+  return rc;
+}
+
+// Both operators from the builder's device CSC of A (m x n; m, n or nnz may be 0; int32 indices, already validated).
+// Returns 0 and sets *A_out (CSR of A) / *At_out (CSR of A' = the CSC arrays); < 0 on failure. The arrays are read
+// only, and may be freed in stream order once this returns.
+extern "C" int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d_Ap, const int *d_Ai,
+                                       const double *d_Ax, B200Spmv **A_out, B200Spmv **At_out) {
   *A_out = *At_out = nullptr;
   if (b200_runtime_init() != 0) return -1;
   cudaStream_t st = (cudaStream_t)b200_stream();
-  int *d_Ap = (int *)b200_malloc((size_t)(n + 1) * 4), *d_Ai = (int *)b200_malloc((size_t)nnz * 4);
-  double *d_Ax = (double *)b200_malloc((size_t)nnz * 8);
   int *d_Tp = (int *)b200_malloc((size_t)(m + 2) * 4), *d_cnt = (int *)b200_malloc((size_t)(m + 2) * 4);
   int *d_Ti = (int *)b200_malloc((size_t)nnz * 4);
   double *d_Tx = (double *)b200_malloc((size_t)nnz * 8);
@@ -140,14 +236,7 @@ static int setup_ops(int m, int n, long long nnz, const int *h_Ap, const int *h_
   double t_mark = setup_now_ms();
   dev_mark("allocations", &t_mark);
   do {
-    if (!d_Ap || !d_Ai || !d_Ax || !d_Tp || !d_cnt || !d_Ti || !d_Tx || !d_cols || !d_iota || !d_keys || !d_perm) break;
-    if (h_Ap64) {
-      if (narrow_csc(m, n, nnz, h_Ap64, h_Ai64, d_Ap, d_Ai) != 0) break;
-    } else if (b200_h2d(d_Ap, h_Ap, (size_t)(n + 1) * 4) != 0 || b200_h2d(d_Ai, h_Ai, (size_t)nnz * 4) != 0) {
-      break;
-    }
-    if (b200_h2d(d_Ax, h_Ax, (size_t)nnz * 8) != 0) break;
-    dev_mark("H2D of the CSC arrays", &t_mark);
+    if (!d_Tp || !d_cnt || !d_Ti || !d_Tx || !d_cols || !d_iota || !d_keys || !d_perm) break;
     // A' first: its CSR is the CSC as given
     At = b200_spmv_create_dev(n, m, nnz, d_Ap, d_Ai, d_Ax);
     if (!At) break;
@@ -179,7 +268,7 @@ static int setup_ops(int m, int n, long long nnz, const int *h_Ap, const int *h_
     rc = 0;
   } while (0);
   b200_sync();
-  b200_free(d_Ap); b200_free(d_Ai); b200_free(d_Ax); b200_free(d_Tp); b200_free(d_cnt); b200_free(d_Ti);
+  b200_free(d_Tp); b200_free(d_cnt); b200_free(d_Ti);
   b200_free(d_Tx); b200_free(d_cols); b200_free(d_iota); b200_free(d_keys); b200_free(d_perm); b200_free(d_tmp);
   dev_mark("frees", &t_mark);
   if (rc != 0) {
@@ -193,6 +282,27 @@ static int setup_ops(int m, int n, long long nnz, const int *h_Ap, const int *h_
   *A_out = A;
   *At_out = At;
   return 0;
+}
+// the same from the host CSC: int32 arrays (h_Ap, h_Ai) or 64-bit ones (h_Ap64, h_Ai64, narrowed on the device by
+// k_narrow_csc), uploaded into the builder's arrays
+static int setup_ops(int m, int n, long long nnz, const int *h_Ap, const int *h_Ai, const long long *h_Ap64,
+                     const long long *h_Ai64, const double *h_Ax, B200Spmv **A_out, B200Spmv **At_out) {
+  *A_out = *At_out = nullptr;
+  if (b200_runtime_init() != 0) return -1;
+  int *d_Ap = (int *)b200_malloc((size_t)(n + 1) * 4), *d_Ai = (int *)b200_malloc((size_t)nnz * 4);
+  double *d_Ax = (double *)b200_malloc((size_t)nnz * 8);
+  double t_mark = setup_now_ms();
+  int rc = -1;
+  if (d_Ap && d_Ai && d_Ax &&
+      (h_Ap64 ? narrow_csc(m, n, nnz, h_Ap64, h_Ai64, d_Ap, d_Ai)
+              : (b200_h2d(d_Ap, h_Ap, (size_t)(n + 1) * 4) | b200_h2d(d_Ai, h_Ai, (size_t)nnz * 4))) == 0 &&
+      b200_h2d(d_Ax, h_Ax, (size_t)nnz * 8) == 0) {
+    dev_mark("H2D of the CSC arrays", &t_mark);
+    rc = b200_setup_ops_from_dev(m, n, nnz, d_Ap, d_Ai, d_Ax, A_out, At_out);
+  }
+  b200_sync();
+  b200_free(d_Ap); b200_free(d_Ai); b200_free(d_Ax);
+  return rc;
 }
 extern "C" int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax,
                                        B200Spmv **A_out, B200Spmv **At_out) {
@@ -257,4 +367,99 @@ extern "C" int b200_gather_vec(int n, const int *d_perm, const double *d_src, do
   b200_count_launch(1);
   CUDA_OK(cudaGetLastError());
   return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
+// The full symmetric P from its upper-triangular CSC on the device, in exactly the CSR the host's expand_sym_upper
+// (host/linsys_b200.c) produces: row r holds first the mirrors of column r's strict-upper entries in k order, then its
+// direct entries (r, j), j >= r, by ascending j. A stable radix sort by row of the list [every entry's mirror in (j, k)
+// order, then every direct entry in (j, k) order] gives that order; the mirror of a diagonal entry is keyed to row n,
+// which sorts last and is dropped. The structure is built first, with d_Fsrc[q] = the CSC entry that full entry q
+// copies, so that the values can be taken after the upper CSC has been equilibrated in place.
+__global__ void k_sym_items(int n, long long nnz, const int *__restrict__ Pi, const int *__restrict__ cols,
+                            int *__restrict__ keys) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < nnz; t += (long long)gridDim.x * blockDim.x) {
+    const int i = Pi[t], j = cols[t];
+    keys[t] = i != j ? j : n;  // mirror (j, i): row j
+    keys[nnz + t] = i;         // direct (i, j): row i
+  }
+}
+__global__ void k_sym_gather(long long full, long long nnz, const int *__restrict__ item, const int *__restrict__ Pi,
+                             const int *__restrict__ cols, int *__restrict__ Fi, int *__restrict__ Fsrc) {
+  for (long long q = blockIdx.x * (long long)blockDim.x + threadIdx.x; q < full; q += (long long)gridDim.x * blockDim.x) {
+    const long long t = item[q];
+    const long long k = t < nnz ? t : t - nnz;
+    Fi[q] = t < nnz ? Pi[k] : cols[k];
+    Fsrc[q] = (int)k;
+  }
+}
+// n x n upper CSC (d_Pp, d_Pi, nnz entries, `full` entries in the symmetric form) -> d_Fp (n + 1), d_Fi, d_Fsrc (full)
+extern "C" int b200_sym_expand_structure(int n, long long nnz, long long full, const int *d_Pp, const int *d_Pi,
+                                         int *d_Fp, int *d_Fi, int *d_Fsrc) {
+  if (2 * nnz > 2147483647LL) {
+    b200_set_error("b200_sym_expand_structure: 2 nnz(P) must fit in an int", cudaErrorInvalidValue, __FILE__, __LINE__);
+    return -1;
+  }
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  const int items = (int)(2 * nnz), g = csc_grid(items);
+  int *d_cols = (int *)b200_malloc((size_t)nnz * 4), *d_keys = (int *)b200_malloc((size_t)items * 4);
+  int *d_keys2 = (int *)b200_malloc((size_t)items * 4), *d_iota = (int *)b200_malloc((size_t)items * 4);
+  int *d_item = (int *)b200_malloc((size_t)items * 4), *d_cnt = (int *)b200_malloc((size_t)(n + 1) * 4);
+  void *d_tmp = nullptr;
+  int rc = -1;
+  do {
+    if (!d_cols || !d_keys || !d_keys2 || !d_iota || !d_item || !d_cnt) break;
+    if (b200_memset0(d_cnt, (size_t)(n + 1) * 4) != 0) break;
+    k_expand_cols<<<g, 256, 0, st>>>(n, d_Pp, d_cols);
+    k_sym_items<<<g, 256, 0, st>>>(n, nnz, d_Pi, d_cols, d_keys);
+    k_iota<<<g, 256, 0, st>>>(items, d_iota);
+    int bits = 1;
+    while ((1LL << bits) < (long long)n + 1) ++bits;
+    size_t tmp_bytes = 0;
+    if (cub::DeviceRadixSort::SortPairs(nullptr, tmp_bytes, d_keys, d_keys2, d_iota, d_item, items, 0, bits, st) !=
+        cudaSuccess)
+      break;
+    d_tmp = b200_malloc(tmp_bytes ? tmp_bytes : 16);
+    if (!d_tmp) break;
+    if (cub::DeviceRadixSort::SortPairs(d_tmp, tmp_bytes, d_keys, d_keys2, d_iota, d_item, items, 0, bits, st) !=
+        cudaSuccess)
+      break;
+    k_count_rows<<<g, 256, 0, st>>>(full, d_keys2, d_cnt);
+    k_sym_gather<<<g, 256, 0, st>>>(full, nnz, d_item, d_Pi, d_cols, d_Fi, d_Fsrc);
+    b200_count_launch(6);
+    if (cudaGetLastError() != cudaSuccess || b200_dev_exclusive_scan_int(d_cnt, d_Fp, n + 1) != 0) break;
+    rc = 0;
+  } while (0);
+  b200_sync();
+  b200_free(d_cols); b200_free(d_keys); b200_free(d_keys2); b200_free(d_iota); b200_free(d_item); b200_free(d_cnt);
+  b200_free(d_tmp);
+  return rc;
+}
+// d_Fx[q] = d_Px[d_Fsrc[q]]; d_diag[r] = the sum of row r's diagonal entries in row order (expand_sym_upper's diag)
+__global__ void k_sym_values(int n, const int *__restrict__ Fp, const int *__restrict__ Fi,
+                             const int *__restrict__ Fsrc, const double *__restrict__ Px, double *__restrict__ Fx,
+                             double *__restrict__ diag) {
+  for (int r = blockIdx.x * blockDim.x + threadIdx.x; r < n; r += gridDim.x * blockDim.x) {
+    double d = 0.0;
+    for (int q = Fp[r]; q < Fp[r + 1]; ++q) {
+      const double v = Px[Fsrc[q]];
+      Fx[q] = v;
+      if (Fi[q] == r) d += v;
+    }
+    diag[r] = d;
+  }
+}
+// the operator of the full symmetric P (*P_out) and its diagonal (d_diag, n) from the structure above and the values
+// of the upper CSC
+extern "C" int b200_sym_build(int n, long long full, const int *d_Fp, const int *d_Fi, const int *d_Fsrc,
+                              const double *d_Px, double *d_diag, B200Spmv **P_out) {
+  double *d_Fx = (double *)b200_malloc((size_t)full * 8);
+  *P_out = nullptr;
+  if (!d_Fx) return -1;
+  k_sym_values<<<csc_grid(n), 256, 0, (cudaStream_t)b200_stream()>>>(n, d_Fp, d_Fi, d_Fsrc, d_Px, d_Fx, d_diag);
+  b200_count_launch(1);
+  if (cudaGetLastError() == cudaSuccess) *P_out = b200_spmv_create_dev(n, n, full, d_Fp, d_Fi, d_Fx);
+  b200_sync();
+  b200_free(d_Fx);
+  return *P_out ? 0 : -1;
 }
