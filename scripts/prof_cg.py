@@ -1,7 +1,8 @@
 """Lean driver for ncu / timing of the CG loop's kernels AS THEY RUN IN A SOLVE: builds the C2 operator, creates the
 linsys workspace and runs genuine CG iterations on a real right-hand side (K1 = spmv_flag_kernel<1>, K2 =
-spmv_flag_kernel<2>, K3 = k_cg_update, K4 = k_cg_pupdate).  REPS (default 20) iterations with per-kernel CUDA events,
-then REPS iterations timed as a whole (no events inside: programmatic dependent launch overlap intact)."""
+spmv_flag_kernel<2>, K3 = k_cg_update, K4 = k_cg_pupdate; up to n = 2 SMs x 4096, K3 / K4 = the two phases of the
+fused k_cg_update_p).  REPS (default 20) iterations with per-kernel CUDA events, then REPS iterations timed as a whole
+(no events inside: programmatic dependent launch overlap intact)."""
 import ctypes as C
 import os
 import sys

@@ -217,6 +217,7 @@ typedef struct {
   B200P2pSignal *d_p2p_sig; /* device copy of the peer flag table */
   B200P2pRoute *d_p2p_route; /* device copy of the push-routing table (sharded-x mode); d_p then lives in the
                                 peer-mapped exchange allocation */
+  int k34_fused;       /* 1: K3 and K4 run as one kernel (k_cg_update_p); set by b200_cg_plan_k34 */
 } B200Cg;
 
 /* M_j = 1 / (R_x,j + P_jj + sum_k A_kj^2 / R_y,k)   (private.c:50-82) */
@@ -224,12 +225,14 @@ int b200_cg_set_preconditioner(const B200Cg *cg, const double *d_Pdiag);
 /* after b200_cg_set_preconditioner, with the reordered pair and d_perm (its rows) in place: fills d_diag_tab and
  * d_ry_mask and sets ry_form / rx_form (one 4-byte read-back) */
 int b200_cg_classify_diag(B200Cg *cg, const int *d_perm);
+/* single GPU: sets k34_fused when n <= 2 SMs * 4096 and the fused kernel's grid is co-resident on the device */
+int b200_cg_plan_k34(B200Cg *cg);
 /* Full device solve of [[R_x+P, A'],[A, -R_y]] [x;y] = b in place on d_b (n+m),
  * warm start d_s (n) or NULL; returns CG iterations (>=0) or <0 on error.
  * Synchronises with the host only to poll the done flag. (private.c:284-324) */
 int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double tol, int max_its,
                   int its_hint, const double *d_tol /* optional device tol */);
-/* one CG iteration (4 kernels), for timing */
+/* one CG iteration (4 kernels, or 3 with k34_fused), for timing */
 int b200_cg_one_iteration(B200Cg *cg, double *d_x);
 /* algorithmic bytes of one CG iteration; per_kernel (optional): K1, K2, K3, K4 (DESIGN.md section 3) */
 double b200_cg_iter_alg_bytes(const B200Cg *cg, double *per_kernel);

@@ -483,6 +483,7 @@ static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_m
   }
   if (b200_h2d(w->d_diag_r, diag_r, ((size_t)n + m) * 8) != 0) return -1;
   if (b200_cg_set_preconditioner(&w->cg, w->d_Pdiag) != 0) return -1;
+  if (b200_cg_plan_k34(&w->cg) != 0) return -1;
   if (b200_sync() != 0) return -1;
   setup_mark("linsys: vectors, preconditioner", &t_mark);
   if (cg_ops_build(w) != 0 || cg_ops_refresh(w) != 0 || b200_sync() != 0) return -1;

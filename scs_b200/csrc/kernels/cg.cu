@@ -17,7 +17,9 @@
 //   K2  Gp  = R_x p + [P p] + A' tmp ;  p'Gp ; alpha spmv (CSR of A'), POST_FMA_DOT + hook
 //   K3  x += alpha p; r -= alpha Gp; z = M r; z'r, ||r||_inf; stop test; beta
 //   K4  p = z + beta p
-// Algorithmic bytes: 24 nnz + 4 (m+n+2) + 24 m + 120 n   (DESIGN.md).
+// Up to n = 2 SMs * 4096 (single GPU), K3 and K4 run as one kernel, k_cg_update_p, that keeps z and p in registers
+// across a grid barrier: 3 kernels per iteration, z never stored.
+// Algorithmic bytes: 24 nnz + 4 (m+n+2) + 24 m + 120 n; 96 n instead of 120 n fused   (DESIGN.md).
 #include "../common.cuh"
 #include "../dev_api.h"
 #include <math.h>
@@ -231,6 +233,133 @@ k_cg_pupdate(int n, double *__restrict__ p, const double *__restrict__ z, const 
     p2[i] = pa;
   }
   if ((n & 1) && blockIdx.x == 0 && threadIdx.x == 0) p[n - 1] = fma(beta, p[n - 1], z[n - 1]);
+}
+
+// K3 + K4 as one pass, for n <= 2 SMs * 4096 (cg_plan_k34): K3's grid is then not capped, so every thread of it
+// covers at most CG_FUSED_V2 double2 elements and can keep their z and p in registers across the beta dependency.
+//   phase 1  k_cg_update over the same grid: the same elements in the same order, the same cg_update_elem, the same
+//            block_sum / block_max / grid_finish slots and ticket, so z'r, ||r||_inf and beta are the same bits. z is
+//            never stored. The last block writes the control block as K3 does, then releases a grid barrier by storing
+//            ctl->iters last; every other block spins on iters (read before its ticket, so it cannot see the new value
+//            too early).
+//   phase 2  k_cg_pupdate from the registers: p = z + beta p unless the stop test fired.
+// The barrier needs every block resident at once (checked at setup). The next K1 may take SM resources only after
+// the barrier has released: pdl_launch_dependents() before it could hand a block's SM slot to K1 while that block is
+// still to be scheduled, and the resident blocks would spin for ever. The spin gives up after ~1.5 s and raises the
+// sticky ctl->pad[0] (the host fails the solve). stamps (timing runs only, else NULL): block 0's %globaltimer at entry
+// and at the release, and the latest block end (atomicMax), in ns.
+#define CG_FUSED_V2 4
+__device__ __forceinline__ unsigned long long cg_globaltimer() {
+  unsigned long long t;
+  asm volatile("mov.u64 %0, %globaltimer;" : "=l"(t));
+  return t;
+}
+__global__ void __launch_bounds__(VEC_THREADS, 2)
+k_cg_update_p(int n, double *__restrict__ x, double *__restrict__ r, double *__restrict__ p,
+              const double *__restrict__ Gp, const double *__restrict__ M, B200CgCtl *ctl, double *partials,
+              unsigned int *counter, unsigned long long *stamps) {
+  if (stamps != nullptr && blockIdx.x == 0 && threadIdx.x == 0) stamps[0] = cg_globaltimer();
+  pdl_wait();  // K2 (Gp, alpha) complete and visible
+  if (ctl->done) return;
+  __shared__ double s_red[128];
+  __shared__ double s_beta;
+  __shared__ int s_done;
+  const double alpha = ctl->alpha;
+  const double nalpha = -alpha;
+  const int iters0 = *((volatile int *)&ctl->iters);  // before this block's ticket: the last block bumps it after
+  double acc0 = 0.0, acc1 = 0.0;
+  const int n2 = n >> 1;
+  double2 *x2 = reinterpret_cast<double2 *>(x), *r2 = reinterpret_cast<double2 *>(r),
+          *p2 = reinterpret_cast<double2 *>(p);
+  const double2 *g2 = reinterpret_cast<const double2 *>(Gp), *m2 = reinterpret_cast<const double2 *>(M);
+  const int stride = gridDim.x * blockDim.x;
+  const int i0 = blockIdx.x * blockDim.x + threadIdx.x;
+  // K3 visits i0, i0 + stride, ... in increasing order (pairs, then the remainder): so does this loop
+  double2 zk[CG_FUSED_V2], pk[CG_FUSED_V2];
+#pragma unroll
+  for (int k = 0; k < CG_FUSED_V2; ++k) {
+    const int i = i0 + k * stride;
+    if (i < n2) {
+      double2 xa = x2[i], ra = r2[i], pa = p2[i], ga = g2[i], ma = m2[i], za;
+      cg_update_elem(alpha, nalpha, xa.x, ra.x, pa.x, ga.x, ma.x, za.x, acc0, acc1);
+      cg_update_elem(alpha, nalpha, xa.y, ra.y, pa.y, ga.y, ma.y, za.y, acc0, acc1);
+      x2[i] = xa; r2[i] = ra;
+      zk[k] = za; pk[k] = pa;
+    }
+  }
+  const bool tail = (n & 1) && blockIdx.x == 0 && threadIdx.x == 0;
+  double zt = 0.0, pt = 0.0;
+  if (tail) {
+    const int k = n - 1;
+    double xv = x[k], rv = r[k];
+    pt = p[k];
+    cg_update_elem(alpha, nalpha, xv, rv, pt, Gp[k], M[k], zt, acc0, acc1);
+    x[k] = xv; r[k] = rv;
+  }
+  double sm[1] = {acc0}, mx[1] = {acc1};
+  block_sum<1>(sm, s_red);
+  block_max<1>(mx, s_red + 64);
+  double both[2] = {sm[0], mx[0]};
+  if (grid_finish<2>(both, partials, counter, 2u, s_red)) {
+    if (threadIdx.x == 0) {
+      // k_cg_update's last block, with iters stored last: it releases the barrier
+      const double ztr_prev = ctl->ztr;
+      const int iters = iters0 + 1;
+      int done = 0;
+      double beta = 0.0;
+      ctl->ztr_prev = ztr_prev;
+      ctl->ztr = both[0];
+      ctl->rnorm = both[1];
+      if (both[1] < ctl->tol) {
+        done = 1;
+      } else if (ztr_prev == 0.0) {
+        done = 1;
+      } else {
+        beta = both[0] / ztr_prev;
+        ctl->beta = beta;
+        if (iters >= ctl->max_its) done = 1;
+      }
+      if (done) ctl->done = 1;
+      __threadfence();
+      *((volatile int *)&ctl->iters) = iters;
+      s_done = done;
+      s_beta = beta;
+    }
+  } else if (threadIdx.x == 0) {
+    const volatile int *vit = (const volatile int *)&ctl->iters;
+    const long long t0 = clock64();
+    bool released = true;
+    while (*vit == iters0) {
+      if (*((volatile int *)&ctl->pad[0]) || clock64() - t0 > 3000000000LL) {
+        ctl->pad[0] = 1;
+        released = false;
+        break;
+      }
+    }
+    __threadfence();  // acquire side: the last block's control-block stores precede its store of iters
+    s_done = released ? *((volatile int *)&ctl->done) : 1;  // after a timeout p is left alone
+    s_beta = *((volatile double *)&ctl->beta);
+  }
+  __syncthreads();
+  pdl_launch_dependents();  // every block has arrived: the next K1 may take SM resources now
+  if (stamps != nullptr && blockIdx.x == 0 && threadIdx.x == 0) stamps[1] = cg_globaltimer();
+  if (!s_done) {
+    const double beta = s_beta;
+#pragma unroll
+    for (int k = 0; k < CG_FUSED_V2; ++k) {
+      const int i = i0 + k * stride;
+      if (i < n2) {
+        double2 pa = pk[k];
+        pa.x = fma(beta, pa.x, zk[k].x); pa.y = fma(beta, pa.y, zk[k].y);
+        p2[i] = pa;
+      }
+    }
+    if (tail) p[n - 1] = fma(beta, pt, zt);
+  }
+  if (stamps != nullptr) {
+    __syncthreads();
+    if (threadIdx.x == 0) atomicMax(stamps + 2, cg_globaltimer());
+  }
 }
 
 
@@ -1021,15 +1150,39 @@ static int cg_iteration_shard_x(B200Cg *cg, double *d_x, cudaEvent_t *ev = nullp
   return 0;
 }
 
+// K3 / K4 grid (also the fused kernel's): 8 doubles per thread, at most 2 blocks of VEC_THREADS per SM
+static int k34_grid(int n) {
+  int g = (n + VEC_THREADS * 8 - 1) / (VEC_THREADS * 8);
+  if (g > 2 * b200_num_sms()) g = 2 * b200_num_sms();
+  if (g < 1) g = 1;
+  return g;
+}
+
+extern "C" int b200_cg_plan_k34(B200Cg *cg) {
+  cg->k34_fused = 0;
+  if (cg->nranks > 1) return 0;
+  // uncapped grid: each thread holds at most CG_FUSED_V2 double2 of z and p
+  if ((long long)cg->n > 2LL * b200_num_sms() * VEC_THREADS * 2 * CG_FUSED_V2) return 0;
+  int per_sm = 0;
+  CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cg_update_p, VEC_THREADS, 0));
+  cg->k34_fused = (long long)per_sm * b200_num_sms() >= k34_grid(cg->n) ? 1 : 0;
+  return 0;
+}
+
 static int cg_iteration(B200Cg *cg, double *d_x) {
   if (shard_x_active(cg)) return cg_iteration_shard_x(cg, d_x);
   cudaStream_t st = (cudaStream_t)b200_stream();
   const int n = cg->n;
-  int g = (n + VEC_THREADS * 8 - 1) / (VEC_THREADS * 8);
-  if (g > 2 * b200_num_sms()) g = 2 * b200_num_sms();
-  if (g < 1) g = 1;
+  const int g = k34_grid(n);
   if (mat_vec(cg, cg->d_p, cg->d_Gp, 1, &cg->d_ctl->done) != 0) return -1;
   const bool pdl = cg_pdl_enabled();
+  if (cg->k34_fused) {
+    CUDA_OK(b200_launch(k_cg_update_p, dim3(g), dim3(VEC_THREADS), 0, st, pdl, n, d_x, cg->d_r, cg->d_p,
+                        (const double *)cg->d_Gp, (const double *)cg->d_M, cg->d_ctl, cg->d_partials, cg->d_counter,
+                        (unsigned long long *)nullptr));
+    b200_count_launch(1);
+    return 0;
+  }
   CUDA_OK(b200_launch(k_cg_update, dim3(g), dim3(VEC_THREADS), 0, st, pdl, n, d_x, cg->d_r, (const double *)cg->d_p,
                       (const double *)cg->d_Gp, (const double *)cg->d_M, cg->d_z, cg->d_ctl, cg->d_partials,
                       cg->d_counter));
@@ -1045,6 +1198,8 @@ extern "C" int b200_cg_one_iteration(B200Cg *cg, double *d_x) { return cg_iterat
 // the solver's own p / tmp / r, every kernel bracketed by CUDA events on the library stream. out_ms[0..3] = average
 // per launch of K1 (tmp = R_y^-1 A p, spmv POST_MUL), K2 (Gp = R_x p + A' tmp, p'Gp, alpha: spmv POST_FMA_DOT + hook),
 // K3 (k_cg_update), K4 (k_cg_pupdate); out_ms[4] = whole iteration (first event to last, launch gaps included).
+// With k34_fused, out_ms[2] / [3] are the two phases of k_cg_update_p from its globaltimer stamps: entry to the grid
+// barrier's release (K3's work and reductions, the barrier) and release to the end of the last block (K4's stores).
 // Single-GPU, P = NULL path only (the configuration the roofline is quoted on).
 extern "C" int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *out_ms) {
   if (cg->nranks > 1 && shard_x_active(cg) && !cg->P && reps > 0) {
@@ -1079,15 +1234,20 @@ extern "C" int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *o
   if (cg->nranks > 1 || cg->P || reps <= 0) return -1;
   cudaStream_t st = (cudaStream_t)b200_stream();
   const int n = cg->n;
-  int g = (n + VEC_THREADS * 8 - 1) / (VEC_THREADS * 8);
-  if (g > 2 * b200_num_sms()) g = 2 * b200_num_sms();
-  if (g < 1) g = 1;
+  const int g = k34_grid(n);
   std::vector<cudaEvent_t> ev((size_t)reps * 5);
   for (auto &e : ev) e = nullptr;
   int rc = -1;
   bool ok = true;
   for (auto &e : ev)
     if (cudaEventCreate(&e) != cudaSuccess) ok = false;
+  // fused K3 + K4: 3 globaltimer stamps per iteration (entry, release, end), see k_cg_update_p
+  unsigned long long *d_stamps = nullptr;
+  if (ok && cg->k34_fused) {
+    d_stamps = (unsigned long long *)b200_malloc((size_t)reps * 3 * sizeof(unsigned long long));
+    if (!d_stamps || cudaMemsetAsync(d_stamps, 0, (size_t)reps * 3 * sizeof(unsigned long long), st) != cudaSuccess)
+      ok = false;
+  }
   if (ok) {
     const int *d_skip = &cg->d_ctl->done;
     for (int r = 0; r < reps && ok; ++r) {
@@ -1105,22 +1265,41 @@ extern "C" int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *o
       a.d_dot = &cg->d_ctl->pGp; a.hook = B200_HOOK_CG_ALPHA; a.d_hook_arg = cg->d_ctl;
       if (b200_spmv(re ? cg->At_cg : cg->At, &a) != 0) ok = false;
       cudaEventRecord(ev[(size_t)r * 5 + 2], st);
-      k_cg_update<<<g, VEC_THREADS, 0, st>>>(n, d_x, cg->d_r, cg->d_p, cg->d_Gp, cg->d_M, cg->d_z, cg->d_ctl,
-                                             cg->d_partials, cg->d_counter);
-      cudaEventRecord(ev[(size_t)r * 5 + 3], st);
-      k_cg_pupdate<<<g, VEC_THREADS, 0, st>>>(n, cg->d_p, cg->d_z, cg->d_ctl);
-      cudaEventRecord(ev[(size_t)r * 5 + 4], st);
-      b200_count_launch(2);
+      if (cg->k34_fused) {
+        k_cg_update_p<<<g, VEC_THREADS, 0, st>>>(n, d_x, cg->d_r, cg->d_p, cg->d_Gp, cg->d_M, cg->d_ctl,
+                                                 cg->d_partials, cg->d_counter, d_stamps + (size_t)r * 3);
+        cudaEventRecord(ev[(size_t)r * 5 + 3], st);
+        cudaEventRecord(ev[(size_t)r * 5 + 4], st);
+        b200_count_launch(1);
+      } else {
+        k_cg_update<<<g, VEC_THREADS, 0, st>>>(n, d_x, cg->d_r, cg->d_p, cg->d_Gp, cg->d_M, cg->d_z, cg->d_ctl,
+                                               cg->d_partials, cg->d_counter);
+        cudaEventRecord(ev[(size_t)r * 5 + 3], st);
+        k_cg_pupdate<<<g, VEC_THREADS, 0, st>>>(n, cg->d_p, cg->d_z, cg->d_ctl);
+        cudaEventRecord(ev[(size_t)r * 5 + 4], st);
+        b200_count_launch(2);
+      }
     }
     if (cudaStreamSynchronize(st) != cudaSuccess) ok = false;
   }
+  std::vector<unsigned long long> h_stamps(d_stamps ? (size_t)reps * 3 : 0);
+  if (ok && d_stamps &&
+      cudaMemcpy(h_stamps.data(), d_stamps, h_stamps.size() * sizeof(unsigned long long), cudaMemcpyDeviceToHost) !=
+          cudaSuccess)
+    ok = false;
   if (ok) {
     for (int k = 0; k < 5; ++k) out_ms[k] = 0.0;
     for (int r = 0; r < reps; ++r) {
-      for (int k = 0; k < 4; ++k) {
+      for (int k = 0; k < (d_stamps ? 2 : 4); ++k) {
         float ms = 0.f;
         cudaEventElapsedTime(&ms, ev[(size_t)r * 5 + k], ev[(size_t)r * 5 + k + 1]);
         out_ms[k] += ms;
+      }
+      if (d_stamps) {
+        // fused: slot 2 = entry to the barrier's release (block 0), slot 3 = release to the last block's end
+        const unsigned long long *s = &h_stamps[(size_t)r * 3];
+        out_ms[2] += (double)(long long)(s[1] - s[0]) * 1e-6;
+        out_ms[3] += (double)(long long)(s[2] - s[1]) * 1e-6;
       }
       float ms = 0.f;
       cudaEventElapsedTime(&ms, ev[(size_t)r * 5], ev[(size_t)r * 5 + 4]);
@@ -1129,6 +1308,7 @@ extern "C" int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *o
     for (int k = 0; k < 5; ++k) out_ms[k] /= reps;
     rc = 0;
   }
+  b200_free(d_stamps);
   for (auto &e : ev)
     if (e) cudaEventDestroy(e);
   return rc;
@@ -1145,8 +1325,10 @@ extern "C" double b200_cg_iter_alg_bytes(const B200Cg *cg, double *per_kernel) {
   double k[4];
   k[0] = e1 * nnz + 4.0 * (m + 1.0) + 8.0 * n + 8.0 * m + ry;
   k[1] = e2 * nnz + 4.0 * (n + 1.0) + 8.0 * m + 16.0 * n + rx;
-  k[2] = 64.0 * n;
-  k[3] = 24.0 * n;
+  // K3 reads x, r, p, Gp, M and writes x, r, z; K4 reads z, p and writes p. Fused: z is never stored and p is read
+  // once, so phase 1 moves 56 n and phase 2 writes p (8 n).
+  k[2] = cg->k34_fused ? 56.0 * n : 64.0 * n;
+  k[3] = cg->k34_fused ? 8.0 * n : 24.0 * n;
   if (per_kernel)
     for (int i = 0; i < 4; ++i) per_kernel[i] = k[i];
   return k[0] + k[1] + k[2] + k[3];
@@ -1191,7 +1373,7 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
   b200_count_launch(1);
   CUDA_OK(cudaGetLastError());
 
-  // main loop in batches. An iteration enqueued after `done` costs 4 empty launches (~12 us), a
+  // main loop in batches. An iteration enqueued after `done` costs 3 or 4 empty launches (~12 us), a
   // host poll costs a ~40 us bubble: the first batch is the previous solve's count plus a 6 % margin
   // (consecutive ADMM iterations need nearly the same number of CG steps), later batches are small.
   int batch = its_hint + (its_hint / 16 > 2 ? its_hint / 16 : 2);
@@ -1207,7 +1389,9 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
     CUDA_OK(cudaMemcpyAsync(cg->h_ctl, cg->d_ctl, sizeof(B200CgCtl), cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaStreamSynchronize(st));
     if (cg->h_ctl->pad[0]) {
-      b200_set_error("peer-memory wait timed out in k_cg_finish_p2p", cudaErrorUnknown, __FILE__, __LINE__);
+      b200_set_error(cg->nranks > 1 ? "peer-memory wait timed out in k_cg_finish_p2p"
+                                    : "grid barrier wait timed out in k_cg_update_p",
+                     cudaErrorUnknown, __FILE__, __LINE__);
       return -1;
     }
     if (cg->h_ctl->done) break;
