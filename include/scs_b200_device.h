@@ -30,6 +30,18 @@ extern "C" {
 ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, void *stream);
 scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream);
 scs_int scs_b200_solve_device(ScsWork *w, ScsSolution *d_sol, ScsInfo *info, scs_int warm_start, void *stream);
+
+/* New values of A (and P) with the sparsity pattern the workspace was built with. A (and P, exactly when the
+ * workspace has one) as for scs_b200_init_device: the structs in host memory, x, i, p device pointers; the same m, n,
+ * p and i as at init, only x may differ. Afterwards the workspace acts exactly like a fresh init through the same door
+ * with the same settings on (A, P, the current original b and c): the next solve, cold or warm from the same given
+ * x, y, s, returns the same bits. The equilibration is redone as init did it, b and c are renormalised from their
+ * originals, the scale goes back to stgs->scale, and AA, the box Newton warm start and the iterates are reset; the
+ * operator layouts, cone workspaces, AA and CG workspaces are kept. A caller with new b and c as well calls
+ * scs_b200_update_device afterwards. Refused (-1, with a message, the workspace untouched): A missing, P given or
+ * missing against the workspace, another m or n, another pattern, invalid entries (init's messages), a host pointer or
+ * memory of another device, a process that is one of several ranks. Accepts workspaces of scs_init too. */
+scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMatrix *P, void *stream);
 #ifdef __cplusplus
 }
 #endif

@@ -387,6 +387,8 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_init_device.argtypes = [C.POINTER(ScsData), C.POINTER(cone), C.POINTER(ScsSettings), C.c_void_p]
     lib.scs_b200_update_device.restype = I
     lib.scs_b200_update_device.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_void_p]
+    lib.scs_b200_update_matrix_device.restype = I
+    lib.scs_b200_update_matrix_device.argtypes = [C.c_void_p, C.POINTER(ScsMatrix), C.POINTER(ScsMatrix), C.c_void_p]
     lib.scs_b200_solve_device.restype = I
     lib.scs_b200_solve_device.argtypes = [C.c_void_p, C.POINTER(ScsSolution), C.POINTER(ScsInfo), I, C.c_void_p]
     lib.scs_b200_transfer_stats.restype = None

@@ -128,6 +128,8 @@ void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_
 void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off, const double *d_mats,
                              const double *d_w, double *d_x, const double *d_s, const double *d_ry);
 void b200_cones_destroy(B200Cones *c);
+/* new box bounds (HOST arrays of bsize - 1, already scaled) and the box Newton warm start back to 1, as at creation */
+int b200_cones_set_box(B200Cones *c, const double *h_bl, const double *h_bu);
 /* Projects the box/SOC/PSD rows. On entry d_x (length m, the y block of u) holds
  * x = -r .* u on those rows and d_s holds the saved u (k_cone_pre); on exit
  * d_x = Pi(x) ./ r + s on those rows. d_ry: R_y (m). */
@@ -148,6 +150,7 @@ void b200_aa_destroy(B200Aa *a);
 double b200_aa_apply_dev(B200Aa *a, double *d_f, const double *d_x);
 int b200_aa_safeguard_dev(B200Aa *a, double *d_f_new, double *d_x_new);
 void b200_aa_reset_dev(B200Aa *a);
+void b200_aa_restart_dev(B200Aa *a); /* the state of a new workspace: reset, and its statistics zeroed */
 void b200_aa_stats(const B200Aa *a, int *out_ints8, double *out_dbl2);
 
 #ifdef __cplusplus

@@ -92,6 +92,17 @@ int b200_sym_expand_structure(int n, long long nnz, long long full, const int *d
                               int *d_Fi, int *d_Fsrc);
 int b200_sym_build(int n, long long full, const int *d_Fp, const int *d_Fi, const int *d_Fsrc, const double *d_Px,
                    double *d_diag, B200Spmv **P_out);
+/* the values behind b200_sym_build: d_Fx (`full`, in the structure's order) and diag(P) (d_diag, n) */
+int b200_sym_values(int n, const int *d_Fp, const int *d_Fi, const int *d_Fsrc, const double *d_Px, double *d_Fx,
+                    double *d_diag);
+/* the builder's transpose of a device CSC (int32, validated) into the CSR d_Tp (m + 1), d_Ti, d_Tx (nnz) */
+int b200_csc_transpose(int m, int n, long long nnz, const int *d_Ap, const int *d_Ai, const double *d_Ax, int *d_Tp,
+                       int *d_Ti, double *d_Tx);
+/* new values on an operator's own pattern (kernels/spmv.cu): ORs `bit` into the device flag *d_bad unless the CSR
+ * (d_rp, d_ci, nnz) has M's pattern (enqueued, no read-back); then, after a clean flag, its values d_va into M's stream */
+int b200_spmv_check_pattern(const B200Spmv *M, const int *d_rp, const int *d_ci, long long nnz, unsigned bit,
+                            unsigned *d_bad);
+int b200_spmv_scatter_values(B200Spmv *M, const int *d_rp, const double *d_va);
 int b200_spmv_nrows(const B200Spmv *M);
 int b200_spmv_ncols(const B200Spmv *M);
 long long b200_spmv_nnz(const B200Spmv *M);

@@ -100,7 +100,13 @@ struct SCS_WORK {
    * stale; sol_on_dev = the ScsSolution of the running solve holds device pointers */
   double *d_b_orig, *d_c_orig;
   int b_on_dev, c_on_dev, bc_host_stale, sol_on_dev;
+  /* what init decided and the solves overwrite, kept for scs_b200_update_matrix_device: the equilibration it used
+   * (B200_EQUIL_*), the initial scale, and the box bounds as given (normalize_box_cone scales k->bl / k->bu) */
+  int equil;
+  double scale0;
+  double *bl_orig, *bu_orig;
 };
+enum { B200_EQUIL_NONE = 0, B200_EQUIL_PAIR = 1, B200_EQUIL_QP_NO_P = 2, B200_EQUIL_QP = 3 };
 
 /* the integer-width boundary (host/abi.c): checks in scs_int width that print a message naming the limit and return
  * nonzero, and int copies of the cone arrays for the kernel layer */

@@ -384,6 +384,7 @@ void scs_finish(ScsWork *w) {
   init_mark("finish: pinned scalars", &t_mark);
   free(w->D); free(w->E); free(w->b_orig); free(w->c_orig); free(w->h_diag_r);
   free(w->cone_boundaries);
+  free(w->bl_orig); free(w->bu_orig);
   if (w->d) {
     free_matrix(w->d->A); free_matrix(w->d->P); free(w->d->b); free(w->d->c); free(w->d);
   }
@@ -544,6 +545,10 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
    * is and both resident orientations are rescaled in place (kernels/equil.cu), so no host
    * copy of A is needed at all. Otherwise (P != 0 or row-sharded) equilibrate a host copy. */
   dev_equil = stgs->normalize && !d->P && !getenv("SCS_B200_HOST_EQUIL");
+  /* the device form of each choice, for scs_b200_update_matrix_device: host/equilibrate.c is b200_equilibrate_qp_dev */
+  w->equil = !stgs->normalize ? B200_EQUIL_NONE : d->P ? B200_EQUIL_QP : dev_equil ? B200_EQUIL_PAIR
+                                                                                  : B200_EQUIL_QP_NO_P;
+  w->scale0 = stgs->scale;
   if (dm) { /* no host copy of A or P; the host copies of b and c are filled when a host call needs them */
     w->d->b = (double *)malloc((size_t)m * 8);
     w->d->c = (double *)malloc((size_t)n * 8);
@@ -564,7 +569,9 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   if (k->bsize > 1) {
     w->k->bu = (double *)dup_mem(k->bu, (size_t)(k->bsize - 1) * 8);
     w->k->bl = (double *)dup_mem(k->bl, (size_t)(k->bsize - 1) * 8);
-    if (!w->k->bu || !w->k->bl) goto fail;
+    w->bu_orig = (double *)dup_mem(k->bu, (size_t)(k->bsize - 1) * 8);
+    w->bl_orig = (double *)dup_mem(k->bl, (size_t)(k->bsize - 1) * 8);
+    if (!w->k->bu || !w->k->bl || !w->bu_orig || !w->bl_orig) goto fail;
   }
   if (k->qsize > 0) { w->k->q = (scs_int *)dup_mem(k->q, (size_t)k->qsize * sizeof(scs_int)); if (!w->k->q) goto fail; }
   if (k->psize > 0) { w->k->p = (double *)dup_mem(k->p, (size_t)k->psize * 8); if (!w->k->p) goto fail; }
@@ -1606,6 +1613,150 @@ scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float
     w->b_on_dev = w->c_on_dev = 1;
     rc = update_bc_dev(w);
   } while (0);
+  b200_caller_waits(stream);
+  return rc;
+}
+
+/* New values of A (and P) on the pattern the workspace was built with (DESIGN.md section 1, "Matrix update"): the
+ * validating copy of init, the builder's transpose, a pattern check of every entry against the resident streams (one
+ * 4-byte read-back), and only then the values scattered into A, A' and P, the equilibration init chose, the
+ * preconditioner and the CG copy refreshed, and the state of a fresh init restored. */
+static void pattern_differs(const char *which) {
+  printf("ERROR: the pattern of %s differs from the one the workspace was built with\n", which);
+}
+scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMatrix *P, void *stream) {
+  const double t0 = now_ms();
+  double t_mark = t0;
+  const int n = w ? w->n : 0, m = w ? w->m : 0;
+  DevMats dm;
+  int *Tp = SCS_NULL, *Ti = SCS_NULL, *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL, *Pp0 = SCS_NULL;
+  double *Tx = SCS_NULL, *Fx = SCS_NULL;
+  unsigned *d_bad = SCS_NULL, bad = ~0u;
+  int rc = -1;
+  memset(&dm, 0, sizeof(dm));
+  if (!w) { printf("ERROR: missing ScsWork input\n"); return -1; }
+  if (!single_gpu()) return -1;
+  if (!A) { printf("ERROR: A matrix missing\n"); return -1; }
+  if (P && !w->p->P) { printf("ERROR: P is given, but the workspace was built without P\n"); return -1; }
+  if (!P && w->p->P) { printf("ERROR: the workspace was built with P, and no P is given\n"); return -1; }
+  if (A->m != m || A->n != n) {
+    printf("ERROR: A is %li x %li; the workspace was built for %i x %i\n", (long)A->m, (long)A->n, m, n);
+    return -1;
+  }
+  if (P && (P->m != n || P->n != n)) {
+    printf("ERROR: P is %li x %li; the workspace was built for %i x %i\n", (long)P->m, (long)P->n, n, n);
+    return -1;
+  }
+  if ((A->p && !dev_ptr_ok(A->p, "A->p")) || (A->i && !dev_ptr_ok(A->i, "A->i")) ||
+      (A->x && !dev_ptr_ok(A->x, "A->x")) ||
+      (P && ((P->p && !dev_ptr_ok(P->p, "P->p")) || (P->i && !dev_ptr_ok(P->i, "P->i")) ||
+             (P->x && !dev_ptr_ok(P->x, "P->x")))))
+    return -1;
+  if (b200_wait_for_caller(stream) != 0) return -1;
+  do {
+    /* 1. everything is checked before the first write to a resident array */
+    if (validate_matrix_dev(A, P, &dm) != 0) { printf("invalid linear system input data\n"); break; }
+    if (dm.nnzA != w->nnzA) { pattern_differs("A"); break; }
+    if (P && (dm.nnzP != w->nnzP || dm.fullP != b200_spmv_nnz(w->p->P))) { pattern_differs("P"); break; }
+    init_mark("update: validating copy", &t_mark);
+    Tp = (int *)b200_malloc(((size_t)m + 1) * 4);
+    Ti = (int *)b200_malloc((size_t)dm.nnzA * 4);
+    Tx = (double *)b200_malloc((size_t)dm.nnzA * 8);
+    d_bad = (unsigned *)b200_malloc(4);
+    if (!Tp || !Ti || !Tx || !d_bad || b200_memset0(d_bad, 4) != 0 ||
+        b200_csc_transpose(m, n, dm.nnzA, dm.Ap, dm.Ai, dm.Ax, Tp, Ti, Tx) != 0)
+      goto dev_fail;
+    init_mark("update: transpose", &t_mark);
+    if (P) {
+      Fp = (int *)b200_malloc(((size_t)n + 1) * 4);
+      Fi = (int *)b200_malloc((size_t)dm.fullP * 4);
+      Fsrc = (int *)b200_malloc((size_t)dm.fullP * 4);
+      if (!Fp || !Fi || !Fsrc || b200_sym_expand_structure(n, dm.nnzP, dm.fullP, dm.Pp, dm.Pi, Fp, Fi, Fsrc) != 0)
+        goto dev_fail;
+    }
+    if (b200_spmv_check_pattern(w->p->At, dm.Ap, dm.Ai, dm.nnzA, 1u, d_bad) != 0 ||
+        b200_spmv_check_pattern(w->p->A, Tp, Ti, dm.nnzA, 1u, d_bad) != 0 ||
+        (P && b200_spmv_check_pattern(w->p->P, Fp, Fi, dm.fullP, 2u, d_bad) != 0) ||
+        b200_d2h(&bad, d_bad, 4) != 0 || b200_sync() != 0)
+      goto dev_fail;
+    init_mark("update: pattern check", &t_mark);
+    if (bad) { pattern_differs(bad & 1u ? "A" : "P"); break; }
+    /* 2. the raw values into both orientations of A, equilibrated in place as init did */
+    if (b200_spmv_scatter_values(w->p->At, dm.Ap, dm.Ax) != 0 || b200_spmv_scatter_values(w->p->A, Tp, Tx) != 0)
+      goto dev_fail;
+    if (w->equil == B200_EQUIL_PAIR) {
+      if (b200_equilibrate_dev(w->p->A, w->p->At, w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0)
+        goto dev_fail;
+    } else if (w->equil == B200_EQUIL_QP_NO_P) { /* P = 0 as an n x n matrix without entries */
+      Pp0 = (int *)b200_malloc(((size_t)n + 1) * 4);
+      if (!Pp0 || b200_memset0(Pp0, ((size_t)n + 1) * 4) != 0 ||
+          b200_equilibrate_qp_dev(w->p->A, w->p->At, Pp0, SCS_NULL, SCS_NULL, Pp0, SCS_NULL, SCS_NULL,
+                                  w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0)
+        goto dev_fail;
+    } else if (w->equil == B200_EQUIL_QP) {
+      if (b200_equilibrate_qp_dev(w->p->A, w->p->At, dm.Pp, dm.Pi, dm.Px, Fp, Fi, Fsrc, w->cone_boundaries,
+                                  w->cone_boundaries_len, w->d_D, w->d_E) != 0)
+        goto dev_fail;
+    }
+    /* 3. P's values and diagonal from the (equilibrated) upper CSC */
+    if (P) {
+      Fx = (double *)b200_malloc((size_t)(dm.fullP > 0 ? dm.fullP : 1) * 8);
+      if (!Fx || b200_sym_values(n, Fp, Fi, Fsrc, dm.Px, Fx, w->p->d_Pdiag) != 0 ||
+          b200_spmv_scatter_values(w->p->P, Fp, Fx) != 0)
+        goto dev_fail;
+    }
+    init_mark("update: values, equilibration", &t_mark);
+    /* 4. the initial scale and diag_r; the preconditioner, A_cg's values and the R_y tables follow them */
+    w->stgs->scale = w->scale0;
+    set_diag_r_host(w);
+    if (b200_admm_set_diag_r(&w->adm, w->k->z, w->stgs->rho_x, w->stgs->scale) != 0 ||
+        b200_linsys_update_diag_r_dev(w->p, w->adm.d_R) != 0)
+      goto dev_fail;
+    w->p->last_cg_its = 0;
+    init_mark("update: preconditioner, CG copy", &t_mark);
+    /* 5. D and E on the host (box bounds, CSV log); the box bounds renormalised from the originals */
+    if (w->D && (b200_d2h(w->D, w->d_D, (size_t)m * 8) != 0 || b200_d2h(w->E, w->d_E, (size_t)n * 8) != 0 ||
+                 b200_sync() != 0))
+      goto dev_fail;
+    if (w->k->bsize > 1) {
+      memcpy(w->k->bl, w->bl_orig, (size_t)(w->k->bsize - 1) * 8);
+      memcpy(w->k->bu, w->bu_orig, (size_t)(w->k->bsize - 1) * 8);
+      if (w->D) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
+    }
+    if (b200_cones_set_box(w->cones, w->k->bl, w->k->bu) != 0) goto dev_fail;
+    /* 6. the iterates, the scalar board, AA and the residual caches as init leaves them */
+    if (b200_memset0(w->adm.d_cnt, 64) != 0 || b200_memset0(w->adm.d_sc, SC_COUNT * 8) != 0 ||
+        b200_memset0(w->adm.d_u, ((size_t)n + m + 1) * 8) != 0 ||
+        b200_memset0(w->adm.d_u_t, ((size_t)n + m + 1) * 8) != 0 ||
+        b200_memset0(w->adm.d_v, ((size_t)n + m + 1) * 8) != 0 ||
+        b200_memset0(w->adm.d_v_prev, ((size_t)n + m + 1) * 8) != 0 ||
+        b200_memset0(w->adm.d_rsk, ((size_t)n + m + 1) * 8) != 0 ||
+        b200_memset0(w->adm.d_g, ((size_t)n + m + 1) * 8) != 0)
+      goto dev_fail;
+    if (w->accel) b200_aa_restart_dev(w->accel);
+    w->r_orig.last_iter = w->r_norm.last_iter = -1;
+    /* 7. b and c renormalised from the originals with the new D, E (a host original is uploaded once) */
+    if (!w->d_b_orig) w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
+    if (!w->d_c_orig) w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
+    if (!w->d_b_orig || !w->d_c_orig || (!w->b_on_dev && b200_h2d(w->d_b_orig, w->b_orig, (size_t)m * 8) != 0) ||
+        (!w->c_on_dev && b200_h2d(w->d_c_orig, w->c_orig, (size_t)n * 8) != 0))
+      goto dev_fail;
+    w->b_on_dev = w->c_on_dev = 1;
+    if (update_bc_dev(w) != 0) goto dev_fail;
+    /* scs_init's host copies of A and P hold the old values: nothing reads them after init */
+    free_matrix(w->d->A); free_matrix(w->d->P);
+    w->d->A = w->d->P = SCS_NULL;
+    init_mark("update: box bounds, resets, b and c", &t_mark);
+    rc = 0;
+    break;
+  dev_fail:
+    printf("ERROR: scs_b200_update_matrix_device failed (%s)\n", b200_last_error());
+  } while (0);
+  b200_sync();
+  b200_free(Tp); b200_free(Ti); b200_free(Tx); b200_free(d_bad);
+  b200_free(Fp); b200_free(Fi); b200_free(Fsrc); b200_free(Fx); b200_free(Pp0);
+  dev_mats_free(&dm);
+  if (rc == 0) w->setup_time = now_ms() - t0;
   b200_caller_waits(stream);
   return rc;
 }

@@ -568,6 +568,16 @@ extern "C" void b200_aa_reset_dev(B200Aa *a) {
   memset(a->nrm_y_col, 0, sizeof(a->nrm_y_col));
 }
 
+// the state of b200_aa_create: b200_aa_reset_dev and the statistics (ScsInfo.aa_stats) back to zero
+extern "C" void b200_aa_restart_dev(B200Aa *a) {
+  if (!a) return;
+  b200_aa_reset_dev(a);
+  a->n_accept = a->n_reject_lapack = a->n_reject_rank0 = a->n_reject_nonfinite = a->n_reject_weight_cap = 0;
+  a->n_safeguard_reject = a->last_rank = 0;
+  a->last_aa_norm = NAN;
+  a->last_regularization = 0;
+}
+
 // reference solve(), aa.c:422-652
 static double aa_solve(B200Aa *a, double *d_f, int len) {
   const int dim = a->dim;

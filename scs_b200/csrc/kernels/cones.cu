@@ -685,6 +685,18 @@ extern "C" B200Cones *b200_cones_create(int m, int nz, int nl, int bsize, const 
   return c;
 }
 
+// new (already scaled) box bounds, and the Newton warm start back to t = 1: the box state of b200_cones_create
+extern "C" int b200_cones_set_box(B200Cones *c, const double *h_bl, const double *h_bu) {
+  if (c->bsize <= 0) return 0;
+  const double init[8] = {1.0, 0, 0, 0, 0, 0, 0, 0};
+  int rc = b200_h2d(c->d_box, init, sizeof(init)) | b200_memset0(c->d_box_flag, 32);
+  if (c->bsize > 1) {
+    rc |= b200_h2d(c->d_bl, h_bl, (size_t)(c->bsize - 1) * 8);
+    rc |= b200_h2d(c->d_bu, h_bu, (size_t)(c->bsize - 1) * 8);
+  }
+  return rc != 0 || b200_sync() != 0 ? -1 : 0;
+}
+
 extern "C" void b200_cones_destroy(B200Cones *c) {
   if (!c) return;
   b200_sync();

@@ -216,32 +216,21 @@ extern "C" int b200_csc_copy_entries(int rows, int n, long long nnz, const void 
   return rc;
 }
 
-// Both operators from the builder's device CSC of A (m x n; m, n or nnz may be 0; int32 indices, already validated).
-// Returns 0 and sets *A_out (CSR of A) / *At_out (CSR of A' = the CSC arrays); < 0 on failure. The arrays are read
-// only, and may be freed in stream order once this returns.
-extern "C" int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d_Ap, const int *d_Ai,
-                                       const double *d_Ax, B200Spmv **A_out, B200Spmv **At_out) {
-  *A_out = *At_out = nullptr;
-  if (b200_runtime_init() != 0) return -1;
+// The transpose of the builder's device CSC of A (m x n, int32 indices, validated): d_Tp (m + 1), d_Ti, d_Tx (nnz) =
+// the CSR of A, the entries of each row by ascending column. Row counts, scan, then a stable radix sort of (row, entry
+// id): stability keeps the column order of the reference's counting sort. The one transpose of the builder
+// (b200_setup_ops_from_dev) and of the matrix update (scs_b200_update_matrix_device); its temporaries are freed here.
+extern "C" int b200_csc_transpose(int m, int n, long long nnz, const int *d_Ap, const int *d_Ai, const double *d_Ax,
+                                  int *d_Tp, int *d_Ti, double *d_Tx) {
   cudaStream_t st = (cudaStream_t)b200_stream();
-  int *d_Tp = (int *)b200_malloc((size_t)(m + 2) * 4), *d_cnt = (int *)b200_malloc((size_t)(m + 2) * 4);
-  int *d_Ti = (int *)b200_malloc((size_t)nnz * 4);
-  double *d_Tx = (double *)b200_malloc((size_t)nnz * 8);
+  int *d_cnt = (int *)b200_malloc((size_t)(m + 2) * 4);
   int *d_cols = (int *)b200_malloc((size_t)nnz * 4), *d_iota = (int *)b200_malloc((size_t)nnz * 4);
   int *d_keys = (int *)b200_malloc((size_t)nnz * 4), *d_perm = (int *)b200_malloc((size_t)nnz * 4);
   void *d_tmp = nullptr;
-  int rc = -1;
-  B200Spmv *A = nullptr, *At = nullptr;
   const int nsm = b200_num_sms();
-  double t_mark = setup_now_ms();
-  dev_mark("allocations", &t_mark);
+  int rc = -1;
   do {
-    if (!d_Tp || !d_cnt || !d_Ti || !d_Tx || !d_cols || !d_iota || !d_keys || !d_perm) break;
-    // A' first: its CSR is the CSC as given
-    At = b200_spmv_create_dev(n, m, nnz, d_Ap, d_Ai, d_Ax);
-    if (!At) break;
-    dev_mark("operator A' (stream + tiles)", &t_mark);
-    // transpose: row counts -> row pointers; stable sort of (row, entry id) -> entries of each row by ascending column
+    if (!d_cnt || !d_cols || !d_iota || !d_keys || !d_perm) break;
     if (b200_memset0(d_cnt, (size_t)(m + 2) * 4) != 0) break;
     k_count_rows<<<8 * nsm, 256, 0, st>>>(nnz, d_Ai, d_cnt);
     if (b200_dev_exclusive_scan_int(d_cnt, d_Tp, m + 1) != 0) break;
@@ -261,6 +250,34 @@ extern "C" int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d
     k_gather_transposed<<<8 * nsm, 256, 0, st>>>(nnz, d_perm, d_cols, d_Ax, d_Ti, d_Tx);
     b200_count_launch(4);
     if (cudaGetLastError() != cudaSuccess || b200_sync() != 0) break;
+    rc = 0;
+  } while (0);
+  b200_sync();
+  b200_free(d_cnt); b200_free(d_cols); b200_free(d_iota); b200_free(d_keys); b200_free(d_perm); b200_free(d_tmp);
+  return rc;
+}
+
+// Both operators from the builder's device CSC of A (m x n; m, n or nnz may be 0; int32 indices, already validated).
+// Returns 0 and sets *A_out (CSR of A) / *At_out (CSR of A' = the CSC arrays); < 0 on failure. The arrays are read
+// only, and may be freed in stream order once this returns.
+extern "C" int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d_Ap, const int *d_Ai,
+                                       const double *d_Ax, B200Spmv **A_out, B200Spmv **At_out) {
+  *A_out = *At_out = nullptr;
+  if (b200_runtime_init() != 0) return -1;
+  int *d_Tp = (int *)b200_malloc((size_t)(m + 2) * 4);
+  int *d_Ti = (int *)b200_malloc((size_t)nnz * 4);
+  double *d_Tx = (double *)b200_malloc((size_t)nnz * 8);
+  int rc = -1;
+  B200Spmv *A = nullptr, *At = nullptr;
+  double t_mark = setup_now_ms();
+  dev_mark("allocations", &t_mark);
+  do {
+    if (!d_Tp || !d_Ti || !d_Tx) break;
+    // A' first: its CSR is the CSC as given
+    At = b200_spmv_create_dev(n, m, nnz, d_Ap, d_Ai, d_Ax);
+    if (!At) break;
+    dev_mark("operator A' (stream + tiles)", &t_mark);
+    if (b200_csc_transpose(m, n, nnz, d_Ap, d_Ai, d_Ax, d_Tp, d_Ti, d_Tx) != 0) break;
     dev_mark("transpose (count, scan, sort)", &t_mark);
     A = b200_spmv_create_dev(m, n, nnz, d_Tp, d_Ti, d_Tx);
     if (!A) break;
@@ -268,8 +285,7 @@ extern "C" int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d
     rc = 0;
   } while (0);
   b200_sync();
-  b200_free(d_Tp); b200_free(d_cnt); b200_free(d_Ti);
-  b200_free(d_Tx); b200_free(d_cols); b200_free(d_iota); b200_free(d_keys); b200_free(d_perm); b200_free(d_tmp);
+  b200_free(d_Tp); b200_free(d_Ti); b200_free(d_Tx);
   dev_mark("frees", &t_mark);
   if (rc != 0) {
     b200_spmv_destroy(A);
@@ -449,6 +465,15 @@ __global__ void k_sym_values(int n, const int *__restrict__ Fp, const int *__res
     diag[r] = d;
   }
 }
+// the values of the full symmetric P (d_Fx, `full`) and its diagonal (d_diag, n) from the structure above and the
+// values of the upper CSC: what b200_sym_build builds P's operator from, and what the matrix update scatters into it
+extern "C" int b200_sym_values(int n, const int *d_Fp, const int *d_Fi, const int *d_Fsrc, const double *d_Px,
+                               double *d_Fx, double *d_diag) {
+  k_sym_values<<<csc_grid(n), 256, 0, (cudaStream_t)b200_stream()>>>(n, d_Fp, d_Fi, d_Fsrc, d_Px, d_Fx, d_diag);
+  b200_count_launch(1);
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
 // the operator of the full symmetric P (*P_out) and its diagonal (d_diag, n) from the structure above and the values
 // of the upper CSC
 extern "C" int b200_sym_build(int n, long long full, const int *d_Fp, const int *d_Fi, const int *d_Fsrc,
@@ -456,9 +481,8 @@ extern "C" int b200_sym_build(int n, long long full, const int *d_Fp, const int 
   double *d_Fx = (double *)b200_malloc((size_t)full * 8);
   *P_out = nullptr;
   if (!d_Fx) return -1;
-  k_sym_values<<<csc_grid(n), 256, 0, (cudaStream_t)b200_stream()>>>(n, d_Fp, d_Fi, d_Fsrc, d_Px, d_Fx, d_diag);
-  b200_count_launch(1);
-  if (cudaGetLastError() == cudaSuccess) *P_out = b200_spmv_create_dev(n, n, full, d_Fp, d_Fi, d_Fx);
+  if (b200_sym_values(n, d_Fp, d_Fi, d_Fsrc, d_Px, d_Fx, d_diag) == 0)
+    *P_out = b200_spmv_create_dev(n, n, full, d_Fp, d_Fi, d_Fx);
   b200_sync();
   b200_free(d_Fx);
   return *P_out ? 0 : -1;

@@ -801,6 +801,86 @@ extern "C" B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr,
 }
 
 // ---------------------------------------------------------------------------------------------
+// New values on the same pattern (scs_b200_update_matrix_device). The stream of an operator built from a CSR (rp, ci)
+// holds entry k of row r at sp[r] + (k - rp[r]), sp = its stored row pointers: the fill (spmv3_fill_row) writes a row's
+// entries in order from sp[r], a row cut into pieces only gets extra END flags, and an empty row is one SKIP | END
+// entry. So a CSR has the operator's pattern if and only if every row has that stored length (an empty row: one SKIP
+// entry) and every entry's masked column at its position is the CSR's column and not SKIP. The rows of an entry come
+// from a bisection of rp (validated: nondecreasing, rp[0] = 0, rp[nrows] = nnz = the operator's nnz), so every
+// position read lies inside its row's stored range.
+__device__ __forceinline__ int csr_row_of(int nrows, const int *__restrict__ rp, long long k) {
+  int lo = 0, hi = nrows;  // the last row r with rp[r] <= k
+  while (hi - lo > 1) {
+    const int mid = lo + (hi - lo) / 2;
+    if (rp[mid] <= k) lo = mid; else hi = mid;
+  }
+  return lo;
+}
+__global__ void k_check_pattern(int nrows, long long nnz, const int *__restrict__ rp, const int *__restrict__ ci,
+                                const int *__restrict__ sp, const int *__restrict__ oi, unsigned bit,
+                                unsigned *__restrict__ d_bad) {
+  const long long work = nnz > nrows ? nnz : nrows, stride = (long long)gridDim.x * blockDim.x;
+  bool diff = false;
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < work; t += stride) {
+    if (t < nrows) {
+      const int r = (int)t, len = rp[r + 1] - rp[r], slen = sp[r + 1] - sp[r];
+      diff |= len == 0 ? slen != 1 || !((unsigned)oi[sp[r]] & B200_FLAG_SKIP) : slen != len;
+    }
+    if (t < nnz) {
+      const int r = csr_row_of(nrows, rp, t);
+      const int off = (int)(t - rp[r]);
+      if (off < sp[r + 1] - sp[r]) {
+        const unsigned v = (unsigned)oi[sp[r] + off];
+        diff |= (v & B200_FLAG_SKIP) != 0 || (int)(v & B200_COLMASK) != ci[t];
+      } else {
+        diff = true;
+      }
+    }
+  }
+  if (diff) atomicOr(d_bad, bit);
+}
+__global__ void k_scatter_values(int nrows, long long nnz, const int *__restrict__ rp, const double *__restrict__ va,
+                                 const int *__restrict__ sp, double *__restrict__ ov) {
+  for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < nnz; t += (long long)gridDim.x * blockDim.x) {
+    const int r = csr_row_of(nrows, rp, t);
+    ov[sp[r] + (t - rp[r])] = va[t];
+  }
+}
+static int entry_grid(long long work) {
+  const long long g = (work + 255) / 256, cap = 8LL * b200_num_sms();
+  return (int)(g < 1 ? 1 : g > cap ? cap : g);
+}
+// ORs `bit` into *d_bad (device) unless the CSR (d_rp, d_ci: nrows = M's rows, nnz entries) has M's pattern; enqueued
+// only. M must keep its int32 index stream (A, A' and P do; the CG loop's packed copies do not).
+extern "C" int b200_spmv_check_pattern(const B200Spmv *M, const int *d_rp, const int *d_ci, long long nnz, unsigned bit,
+                                       unsigned *d_bad) {
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  if (M->d_colidx == nullptr || M->d_rowptr == nullptr || nnz != M->nnz) {
+    b200_set_error("b200_spmv_check_pattern: the operator has no int32 index stream or another nnz",
+                   cudaErrorInvalidValue, __FILE__, __LINE__);
+    return -1;
+  }
+  const long long work = nnz > M->nrows ? nnz : M->nrows;
+  if (work > 0) {
+    k_check_pattern<<<entry_grid(work), 256, 0, st>>>(M->nrows, nnz, d_rp, d_ci, M->d_rowptr, M->d_colidx, bit, d_bad);
+    b200_count_launch(1);
+  }
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+// the values of the CSR (d_rp, d_va) into M's stream at the positions above, after a clean b200_spmv_check_pattern;
+// M's explicit zeros (empty rows) keep their 0.0
+extern "C" int b200_spmv_scatter_values(B200Spmv *M, const int *d_rp, const double *d_va) {
+  if (M->nnz > 0) {
+    k_scatter_values<<<entry_grid(M->nnz), 256, 0, (cudaStream_t)b200_stream()>>>(M->nrows, M->nnz, d_rp, d_va,
+                                                                                  M->d_rowptr, M->d_vals);
+    b200_count_launch(1);
+  }
+  CUDA_OK(cudaGetLastError());
+  return 0;
+}
+
+// ---------------------------------------------------------------------------------------------
 // Reordered copies for the CG operator (DESIGN.md section 3.1 "Reordering").
 // The m-space ordering INSIDE G = R_x + A' R_y^-1 A is free (tmp = R_y^-1 A p never leaves the operator), so the rows
 // of A can be sorted by their smallest column index: one gather per row of K1 becomes sequential, and the matching

@@ -97,6 +97,7 @@ class SCS:
         self.m, self.n, idx = check_args(data)
         self.device = data["A"].device
         self._long = idx == torch.int64
+        self._has_P = data.get("P") is not None
         spectral = capi.is_spectral(cone)
         self._lib = capi.load(spectral=spectral, long=self._long)
         T = capi.abi(self._long)
@@ -125,8 +126,11 @@ class SCS:
     def _stream(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def update(self, b=None, c=None):
-        """new b and / or c (CUDA float64); None keeps the current vector"""
+    def update(self, b=None, c=None, A=None, P=None):
+        """new b and / or c (CUDA float64) and / or new values of A and P (CUDA sparse-CSC tensors with the pattern the
+        solver was built with: scs_b200_update_matrix_device); None keeps the current one. A solver built with P takes
+        P with every A, and P only with A. The matrices are updated first, then b and c; the previous solution stays
+        the warm start."""
         if b is not None:
             _check_vector("b", b, self.m)
             _check_device("b", b, self.device.index)
@@ -135,6 +139,36 @@ class SCS:
             _check_vector("c", c, self.n)
             _check_device("c", c, self.device.index)
             c = c.contiguous()
+        if P is not None and A is None:
+            raise ValueError("P is updated together with A: pass A as well")
+        if A is not None:
+            if P is None and self._has_P:
+                raise ValueError("this solver was built with P: pass P together with A")
+            if P is not None and not self._has_P:
+                raise ValueError("this solver was built without P; P cannot be added by an update")
+            idx = torch.int64 if self._long else torch.int32
+            for name, M, shape in (("A", A, (self.m, self.n)), ("P", P, (self.n, self.n))):
+                if M is None:
+                    continue
+                _check_csc(name, M, shape)
+                if M.ccol_indices().dtype != idx:
+                    raise ValueError(f"{name} must have {idx} indices, as the solver was built with, "
+                                     f"got {M.ccol_indices().dtype}")
+                _check_device(name, M, self.device.index)
+            keep = []
+
+            def mat(M):
+                p, i, x = M.ccol_indices().contiguous(), M.row_indices().contiguous(), M.values().contiguous()
+                keep.extend((p, i, x))
+                return self._T.ScsMatrix(_dptr(x), _iptr(i, self._T), _iptr(p, self._T), M.shape[0], M.shape[1])
+            Am = mat(A)
+            Pm = mat(P) if P is not None else None
+            rc = self._lib.scs_b200_update_matrix_device(self._work, C.byref(Am),
+                                                         C.byref(Pm) if Pm is not None else None, self._stream())
+            if rc != 0:
+                raise RuntimeError("scs_b200_update_matrix_device refused the matrices (its message is printed above)")
+        if A is not None and b is None and c is None:
+            return
         rc = self._lib.scs_b200_update_device(self._work, _dptr(b) if b is not None else None,
                                               _dptr(c) if c is not None else None, self._stream())
         if rc != 0:
