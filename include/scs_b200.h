@@ -123,7 +123,7 @@ typedef struct {
 #ifdef USE_SPECTRAL_CONES
   /* spectral cones (layout of the reference's USE_SPECTRAL_CONES build, include/scs.h:154-171); only
    * libscs_b200_spectral.so is compiled with this block. Their rows follow the power cones in this order. */
-  scs_int *d;          /* log-det cone orders [dsize]: accepted by the layout, refused by scs_init */
+  scs_int *d;          /* log-det cone orders [dsize] */
   scs_int dsize;
   scs_int *nuc_m, *nuc_n; /* nuclear-norm cones: m x n column-major, 1 <= n <= m, 1 + m n rows each */
   scs_int nucsize;
@@ -231,7 +231,7 @@ scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int r
 
 /* Cone operator: replaces reference src/cones.c:1498-1596 (init_cone /
  * proj_dual_cone / finish_cone) for zero, LP, box, SOC, PSD, exponential and power cones,
- * and in the spectral library also nuclear-norm, l1-norm and sum-of-largest-eigenvalues cones.
+ * and in the spectral library also log-det, nuclear-norm, l1-norm and sum-of-largest-eigenvalues cones.
  * D is the row scaling of the equilibrated problem (length m) or NULL
  * (reference normalize_box_cone, cones.c:1160-1177).  x (length m) and r_y
  * (length m or NULL) are HOST arrays; x is projected in place onto the dual
@@ -241,6 +241,11 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m,
 scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x,
                                 const scs_float *r_y);
 void scs_b200_finish_cone(ScsB200ConeWork *c);
+/* The Newton_stats record (reference ScsConeWork.newton_stats) after the last scs_b200_proj_dual_cone: iter,
+ * newton_success and the three residuals of the last log-det cone projected. Returns 0, or -1 when the workspace
+ * has no log-det cones (always in the default library). */
+scs_int scs_b200_cone_logdet_stats(ScsB200ConeWork *c, scs_int *iter, scs_int *newton_success,
+                                   scs_float *residuals);
 
 /* Anderson acceleration operator: replaces reference src/aa.c:657-979
  * (aa_init / aa_apply / aa_safeguard / aa_reset / aa_finish / aa_get_stats).

@@ -68,7 +68,8 @@ class ScsCone(C.Structure):
 
 class ScsConeSpectral(ScsCone):
     """ScsCone of the reference's USE_SPECTRAL_CONES build (include/scs.h:154-171): 184 bytes, taken by
-    libscs_b200_spectral.so. Log-det cones (d) fit the layout but that library refuses them at scs_init."""
+    libscs_b200_spectral.so, which projects all four spectral cones: log-det (d), nuclear-norm, l1-norm and
+    sum-of-largest-eigenvalues."""
     _fields_ = [
         ("d", c_int_p), ("dsize", C.c_int), ("nuc_m", c_int_p), ("nuc_n", c_int_p), ("nucsize", C.c_int),
         ("ell1", c_int_p), ("ell1_size", C.c_int), ("sl_n", c_int_p), ("sl_k", c_int_p), ("sl_size", C.c_int),
@@ -359,6 +360,8 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_proj_dual_cone.argtypes = [C.c_void_p, c_double_p, c_double_p]
     lib.scs_b200_finish_cone.restype = None
     lib.scs_b200_finish_cone.argtypes = [C.c_void_p]
+    lib.scs_b200_cone_logdet_stats.restype = I
+    lib.scs_b200_cone_logdet_stats.argtypes = [C.c_void_p, IP, IP, c_double_p]
     lib.scs_b200_aa_init.restype = C.c_void_p
     lib.scs_b200_aa_init.argtypes = [I, I, I, I, C.c_double, C.c_double,
                                      C.c_double, C.c_double, I, I]

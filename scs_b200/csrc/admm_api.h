@@ -110,19 +110,30 @@ void b200_cpsd_set_err(B200CpsdCones *c, int *d_err);
 void *b200_solver_acquire(void);
 void b200_solver_release(void *handle);
 int b200_cones_set_complex_psd(B200Cones *c, int cssize, const int *h_cs, int n_triples);
-/* nuclear-norm (nuc_m x nuc_n), l1-norm (ell1) and sum-of-largest-eigenvalues (sl_n, sl_k) cones of the spectral
- * build: the LAST rows of the cone product, in that order (kernels/cones_spectral.cu; reference cones.c:1462-1490).
- * Must be called before b200_cones_set_triples / b200_cones_set_complex_psd. 0 on success (also when all are empty). */
-int b200_cones_set_spectral(B200Cones *c, int nucsize, const int *h_nuc_m, const int *h_nuc_n, int ell1_size,
-                            const int *h_ell1, int sl_size, const int *h_sl_n, const int *h_sl_k);
+/* log-det (d), nuclear-norm (nuc_m x nuc_n), l1-norm (ell1) and sum-of-largest-eigenvalues (sl_n, sl_k) cones of the
+ * spectral build: the LAST rows of the cone product, in that order (kernels/cones_spectral.cu; reference
+ * cones.c:1446-1490). Must be called before b200_cones_set_triples / b200_cones_set_complex_psd. 0 on success (also
+ * when all are empty). */
+int b200_cones_set_spectral(B200Cones *c, int dsize, const int *h_d, int nucsize, const int *h_nuc_m,
+                            const int *h_nuc_n, int ell1_size, const int *h_ell1, int sl_size, const int *h_sl_n,
+                            const int *h_sl_k);
+/* the log-det cones' warm starts and saved projections back to zero, as at creation (0, or -1) */
+int b200_cones_reset_spectral(B200Cones *c);
+/* the Newton_stats record (iter, newton_success, residuals) of the last log-det cone projected; -1 when there are
+ * no log-det cones. Syncs. */
+int b200_cones_logdet_stats(B200Cones *c, int *iter, int *newton_success, double res[3]);
 typedef struct B200SpecCones B200SpecCones;
-B200SpecCones *b200_spec_create(int nucsize, const int *h_nuc_m, const int *h_nuc_n, int ell1_size, const int *h_ell1,
-                                int sl_size, const int *h_sl_n, const int *h_sl_k, long long first_row, int *d_err);
+B200SpecCones *b200_spec_create(int dsize, const int *h_d, int nucsize, const int *h_nuc_m, const int *h_nuc_n,
+                                int ell1_size, const int *h_ell1, int sl_size, const int *h_sl_n, const int *h_sl_k,
+                                long long first_row, int *d_err);
 int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_s, const double *d_ry);
+int b200_spec_reset(B200SpecCones *c);
+int b200_spec_logdet_stats(B200SpecCones *c, int *iter, int *newton_success, double res[3]);
 void b200_spec_destroy(B200SpecCones *c);
 /* shared with kernels/cones_spectral.cu (kernels/cones.cu): the sqrt2-scaled unpack of packed lower triangles, and
- * the DMMA contraction V diag(w) V' with signed weights (mode 1, packed lower output) or its rectangular block
- * (mode 2, dense rows x cols output from V of order ld = rows + cols) */
+ * the DMMA contraction V diag(w) V' with weights max(w, 0) (mode 0, packed lower output; w ascending), signed weights
+ * (mode 1, packed lower output) or its rectangular block (mode 2, dense rows x cols output from V of order
+ * ld = rows + cols) */
 void b200_psd_info_or(int count, const int *d_info, int *d_err);
 void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_x, double *d_mats);
 void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off, const double *d_mats,

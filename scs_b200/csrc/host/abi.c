@@ -127,6 +127,7 @@ int b200_cone_ints(const ScsCone *k, B200ConeInts *c) {
   rc |= narrow(k->s, k->ssize, &c->s);
   rc |= narrow(k->cs, k->cssize, &c->cs);
 #ifdef USE_SPECTRAL_CONES
+  rc |= narrow(k->d, k->dsize, &c->d);
   rc |= narrow(k->nuc_m, k->nucsize, &c->nuc_m);
   rc |= narrow(k->nuc_n, k->nucsize, &c->nuc_n);
   rc |= narrow(k->ell1, k->ell1_size, &c->ell1);
@@ -138,7 +139,7 @@ int b200_cone_ints(const ScsCone *k, B200ConeInts *c) {
 }
 
 void b200_cone_ints_free(B200ConeInts *c) {
-  free(c->q); free(c->s); free(c->cs);
+  free(c->q); free(c->s); free(c->cs); free(c->d);
   free(c->nuc_m); free(c->nuc_n); free(c->ell1); free(c->sl_n); free(c->sl_k);
-  c->q = c->s = c->cs = c->nuc_m = c->nuc_n = c->ell1 = c->sl_n = c->sl_k = SCS_NULL;
+  c->q = c->s = c->cs = c->d = c->nuc_m = c->nuc_n = c->ell1 = c->sl_n = c->sl_k = SCS_NULL;
 }

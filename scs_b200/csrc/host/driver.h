@@ -112,7 +112,7 @@ enum { B200_EQUIL_NONE = 0, B200_EQUIL_PAIR = 1, B200_EQUIL_QP_NO_P = 2, B200_EQ
  * nonzero, and int copies of the cone arrays for the kernel layer */
 int b200_cone_over_limits(const ScsCone *k);
 typedef struct {
-  int *q, *s, *cs, *nuc_m, *nuc_n, *ell1, *sl_n, *sl_k; /* NULL where the cone has none */
+  int *q, *s, *cs, *d, *nuc_m, *nuc_n, *ell1, *sl_n, *sl_k; /* NULL where the cone has none */
 } B200ConeInts;
 int b200_cone_ints(const ScsCone *k, B200ConeInts *c); /* 0, or -1 (out of memory, nothing held) */
 void b200_cone_ints_free(B200ConeInts *c);

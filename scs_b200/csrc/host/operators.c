@@ -31,10 +31,12 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float
   for (j = 0; j < k->cssize; ++j) dims += (long long)k->cs[j] * k->cs[j];
   dims += 3LL * ((long long)k->ep + k->ed + k->psize);
 #ifdef USE_SPECTRAL_CONES
-  if (k->dsize != 0 || k->nucsize < 0 || k->ell1_size < 0 || k->sl_size < 0) return SCS_NULL; /* no log-det cones */
-  if ((k->nucsize > 0 && (!k->nuc_m || !k->nuc_n)) || (k->ell1_size > 0 && !k->ell1) ||
+  if (k->dsize < 0 || k->nucsize < 0 || k->ell1_size < 0 || k->sl_size < 0) return SCS_NULL;
+  if ((k->dsize > 0 && !k->d) || (k->nucsize > 0 && (!k->nuc_m || !k->nuc_n)) || (k->ell1_size > 0 && !k->ell1) ||
       (k->sl_size > 0 && (!k->sl_n || !k->sl_k)))
     return SCS_NULL;
+  for (j = 0; j < k->dsize; ++j)
+    if (k->d[j] < 1) return SCS_NULL;
   for (j = 0; j < k->nucsize; ++j)
     if (k->nuc_m[j] < 1 || k->nuc_n[j] < 1 || k->nuc_n[j] > k->nuc_m[j]) return SCS_NULL;
   for (j = 0; j < k->ell1_size; ++j)
@@ -75,7 +77,7 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float
   bl = bu = SCS_NULL;
   if (!c->cones) goto fail_ints;
 #ifdef USE_SPECTRAL_CONES
-  if (b200_cones_set_spectral(c->cones, (int)k->nucsize, ci.nuc_m, ci.nuc_n, (int)k->ell1_size, ci.ell1,
+  if (b200_cones_set_spectral(c->cones, (int)k->dsize, ci.d, (int)k->nucsize, ci.nuc_m, ci.nuc_n, (int)k->ell1_size, ci.ell1,
                               (int)k->sl_size, ci.sl_n, ci.sl_k) != 0)
     goto fail_ints;
 #endif
@@ -104,6 +106,15 @@ scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x, const scs_floa
   if (b200_d2h(x, c->d_x, bytes) != 0) return -1;
   if (b200_sync() != 0) return -1;
   return b200_cones_check(c->cones); /* a failed eigen-decomposition is an error, like cones.c:1048-1052 */
+}
+
+scs_int scs_b200_cone_logdet_stats(ScsB200ConeWork *c, scs_int *iter, scs_int *newton_success,
+                                   scs_float *residuals) {
+  int it = 0, success = 0;
+  if (!c || b200_cones_logdet_stats(c->cones, &it, &success, residuals) != 0) return -1;
+  *iter = it;
+  *newton_success = success;
+  return 0;
 }
 
 void scs_b200_finish_cone(ScsB200ConeWork *c) {

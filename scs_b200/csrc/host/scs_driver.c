@@ -257,11 +257,6 @@ static int validate_cones(const ScsData *d, const ScsCone *k) {
       printf("sum-of-largest-eigenvalues cone dimension error\n");
       return -1;
     }
-  if (k->dsize > 0) { /* never dropped silently: its rows would go unprojected */
-    printf("log-det cones (dsize = %lli) are not supported: this library projects the nuclear-norm, l1-norm and "
-           "sum-of-largest-eigenvalues spectral cones only\n", (long long)k->dsize);
-    return -1;
-  }
 #endif
   dims = (long long)k->z + k->l + k->bsize;
   for (i = 0; i < k->qsize; ++i) dims += k->q[i];
@@ -272,7 +267,30 @@ static int validate_cones(const ScsData *d, const ScsCone *k) {
   dims += b200_spectral_rows(k);
 #endif
   if (dims != d->m) {
+#ifdef USE_SPECTRAL_CONES
+    /* name the spectral families: a wrong cone array usually comes from one of them */
+    {
+      static const char *names[4] = {"log-det", "nuclear-norm", "l1-norm", "sum-of-largest-eigenvalues"};
+      long long rows[4] = {0, 0, 0, 0};
+      scs_int counts[4];
+      int f, first = 1;
+      for (i = 0; i < k->dsize; ++i) rows[0] += (long long)k->d[i] * (k->d[i] + 1) / 2 + 2;
+      for (i = 0; i < k->nucsize; ++i) rows[1] += (long long)k->nuc_m[i] * k->nuc_n[i] + 1;
+      for (i = 0; i < k->ell1_size; ++i) rows[2] += (long long)k->ell1[i] + 1;
+      for (i = 0; i < k->sl_size; ++i) rows[3] += (long long)k->sl_n[i] * (k->sl_n[i] + 1) / 2 + 1;
+      counts[0] = k->dsize; counts[1] = k->nucsize; counts[2] = k->ell1_size; counts[3] = k->sl_size;
+      printf("Error: Cone dims %li != rows in A %li", (long)dims, (long)d->m);
+      for (f = 0; f < 4; ++f) {
+        if (counts[f] == 0) continue;
+        printf("%s%lli rows in %lli %s cone%s", first ? " (spectral: " : ", ", rows[f], (long long)counts[f],
+               names[f], counts[f] == 1 ? "" : "s");
+        first = 0;
+      }
+      printf("%s\n", first ? "" : ")");
+    }
+#else
     printf("Error: Cone dims %li != rows in A %li\n", (long)dims, (long)d->m);
+#endif
     return -1;
   }
   return 0;
@@ -578,6 +596,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   if (k->cssize > 0) { w->k->cs = (scs_int *)dup_mem(k->cs, (size_t)k->cssize * sizeof(scs_int)); if (!w->k->cs) goto fail; }
   if (k->ssize > 0) { w->k->s = (scs_int *)dup_mem(k->s, (size_t)k->ssize * sizeof(scs_int)); if (!w->k->s) goto fail; }
 #ifdef USE_SPECTRAL_CONES
+  if (k->dsize > 0) { w->k->d = (scs_int *)dup_mem(k->d, (size_t)k->dsize * sizeof(scs_int)); if (!w->k->d) goto fail; }
   if (k->nucsize > 0) {
     w->k->nuc_m = (scs_int *)dup_mem(k->nuc_m, (size_t)k->nucsize * sizeof(scs_int));
     w->k->nuc_n = (scs_int *)dup_mem(k->nuc_n, (size_t)k->nucsize * sizeof(scs_int));
@@ -716,7 +735,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   w->cones = b200_cones_create(m, (int)w->k->z, (int)w->k->l, (int)w->k->bsize, w->k->bl, w->k->bu,
                                (int)w->k->qsize, ci.q, (int)w->k->ssize, ci.s);
 #ifdef USE_SPECTRAL_CONES
-  if (w->cones && b200_cones_set_spectral(w->cones, (int)w->k->nucsize, ci.nuc_m, ci.nuc_n, (int)w->k->ell1_size,
+  if (w->cones && b200_cones_set_spectral(w->cones, (int)w->k->dsize, ci.d, (int)w->k->nucsize, ci.nuc_m, ci.nuc_n, (int)w->k->ell1_size,
                                           ci.ell1, (int)w->k->sl_size, ci.sl_n, ci.sl_k) != 0) {
     printf("ERROR: init_cone failure (spectral cones)\n");
     b200_cone_ints_free(&ci);
@@ -1250,7 +1269,15 @@ static int log_data_to_csv(ScsWork *w, int iter, double t_solve) {
   }
   fprintf(f, "%.16e,%li,%li,", w->aa_norm, (long)w->accepted_accel_steps, (long)w->rejected_accel_steps);
   fprintf(f, "%.16e,", (now_ms() - t_solve) / 1e3);
-  fprintf(f, "0,0,%.16e,%.16e,%.16e,", 0.0, 0.0, 0.0); /* spectral-cone Newton statistics: no spectral cones here */
+  {
+    /* the Newton_stats record of the last log-det cone projected (rw.c:854-858); zeros without log-det cones */
+    int st_iter = 0, st_success = 0;
+    double st_res[3] = {0.0, 0.0, 0.0};
+#ifdef USE_SPECTRAL_CONES
+    if (w->k->dsize > 0 && b200_cones_logdet_stats(w->cones, &st_iter, &st_success, st_res) != 0) return -1;
+#endif
+    fprintf(f, "%i,%i,%.16e,%.16e,%.16e,", st_iter, st_success, st_res[0], st_res[1], st_res[2]);
+  }
   fprintf(f, "\n");
   return 0;
 }
@@ -1724,6 +1751,8 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
       if (w->D) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
     }
     if (b200_cones_set_box(w->cones, w->k->bl, w->k->bu) != 0) goto dev_fail;
+    /* the log-det cones' warm starts and saved projections, as init leaves them */
+    if (b200_cones_reset_spectral(w->cones) != 0) goto dev_fail;
     /* 6. the iterates, the scalar board, AA and the residual caches as init leaves them */
     if (b200_memset0(w->adm.d_cnt, 64) != 0 || b200_memset0(w->adm.d_sc, SC_COUNT * 8) != 0 ||
         b200_memset0(w->adm.d_u, ((size_t)n + m + 1) * 8) != 0 ||

@@ -444,7 +444,9 @@ extern "C" void b200_reconstruct_launch(int mode, int ld, int rows, int cols, in
   cudaStream_t st = (cudaStream_t)b200_stream();
   const int ntr = (rows + PT - 1) / PT, ntc = (cols + PT - 1) / PT;
   dim3 rg(ntc, ntr, count);
-  if (mode == REC_RECT)
+  if (mode == REC_PSD)
+    k_reconstruct_dmma<REC_PSD><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
+  else if (mode == REC_RECT)
     k_reconstruct_dmma<REC_RECT><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
   else
     k_reconstruct_dmma<REC_SIGNED><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
@@ -723,12 +725,13 @@ extern "C" void b200_cones_destroy(B200Cones *c) {
 
 extern "C" double *b200_cones_scratch(B200Cones *c) { return c->d_scratch; }
 
-// nuclear-norm, l1-norm and sum-of-largest-eigenvalues cones occupy the last rows, in that order (reference
-// cones.c:1462-1490). Called before b200_cones_set_triples / _set_complex_psd, whose rows sit just before them.
-extern "C" int b200_cones_set_spectral(B200Cones *c, int nucsize, const int *h_nuc_m, const int *h_nuc_n,
-                                       int ell1_size, const int *h_ell1, int sl_size, const int *h_sl_n,
-                                       const int *h_sl_k) {
+// log-det, nuclear-norm, l1-norm and sum-of-largest-eigenvalues cones occupy the last rows, in that order (reference
+// cones.c:1446-1490). Called before b200_cones_set_triples / _set_complex_psd, whose rows sit just before them.
+extern "C" int b200_cones_set_spectral(B200Cones *c, int dsize, const int *h_d, int nucsize, const int *h_nuc_m,
+                                       const int *h_nuc_n, int ell1_size, const int *h_ell1, int sl_size,
+                                       const int *h_sl_n, const int *h_sl_k) {
   long long rows = 0;
+  for (int i = 0; i < dsize; ++i) rows += 2 + (long long)h_d[i] * (h_d[i] + 1) / 2;
   for (int i = 0; i < nucsize; ++i) rows += 1 + (long long)h_nuc_m[i] * h_nuc_n[i];
   for (int i = 0; i < ell1_size; ++i) rows += 1 + (long long)h_ell1[i];
   for (int i = 0; i < sl_size; ++i) rows += 1 + (long long)h_sl_n[i] * (h_sl_n[i] + 1) / 2;
@@ -739,9 +742,15 @@ extern "C" int b200_cones_set_spectral(B200Cones *c, int nucsize, const int *h_n
     if (!c->d_err || b200_memset0(c->d_err, 64) != 0) return -1;
   }
   c->spec_rows = rows;
-  c->spec = b200_spec_create(nucsize, h_nuc_m, h_nuc_n, ell1_size, h_ell1, sl_size, h_sl_n, h_sl_k,
+  c->spec = b200_spec_create(dsize, h_d, nucsize, h_nuc_m, h_nuc_n, ell1_size, h_ell1, sl_size, h_sl_n, h_sl_k,
                              (long long)c->m - rows, c->d_err);
   return c->spec ? 0 : -1;
+}
+
+extern "C" int b200_cones_reset_spectral(B200Cones *c) { return c->spec ? b200_spec_reset(c->spec) : 0; }
+
+extern "C" int b200_cones_logdet_stats(B200Cones *c, int *iter, int *newton_success, double res[3]) {
+  return c->spec ? b200_spec_logdet_stats(c->spec, iter, newton_success, res) : -1;
 }
 
 // exponential / power cones occupy the 3 (ep + ed + psize) rows before the spectral cones, i.e. the LAST rows when
@@ -858,6 +867,11 @@ extern "C" int b200_cones_check(B200Cones *c) {
   if (!c || !c->d_err) return 0;
   int h = 0;
   if (b200_d2h(&h, c->d_err, sizeof(int)) != 0 || b200_sync() != 0) return -1;
+  if (h & 2) {  // LD_ERR_BIT of kernels/cones_spectral.cu
+    b200_set_error("log-det cone projection failed: Newton and both interior-point variants missed the tolerances",
+                   cudaErrorUnknown, __FILE__, __LINE__);
+    return -1;
+  }
   if (h != 0) {
     b200_set_error("batched syevd reported a failure (info != 0) in a PSD or spectral cone projection",
                    cudaErrorUnknown, __FILE__, __LINE__);
