@@ -275,6 +275,10 @@ scs_int scs_b200_get_stats(const ScsWork *w, ScsB200Stats *out);
 /* Change max_iters of a live workspace (the settings are deep-copied at
  * scs_init; used by bench.py to run W warm-up and then exactly K timed steps). */
 scs_int scs_b200_set_max_iters(ScsWork *w, scs_int max_iters);
+/* 1 if scs_solve reuses g = (R + M)^{-1} [c; -b] from the workspace's previous solve when A, P, b, c and the scale
+ * are unchanged since it was computed (the default), 0 if SCS_B200_G_REUSE=0 makes every scs_solve re-solve it as the
+ * reference does. The environment is read at every scs_solve. */
+scs_int scs_b200_g_reuse(void);
 
 /* Multi-GPU (one process per GPU, row-sharded KKT solve; SURVEY 8e). Rank 0 creates the
  * 128-byte NCCL unique id, the launcher distributes it (bench.py: torch.distributed), every

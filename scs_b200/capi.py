@@ -379,6 +379,8 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_get_stats.argtypes = [C.c_void_p, C.POINTER(ScsB200Stats)]
     lib.scs_b200_set_max_iters.restype = I
     lib.scs_b200_set_max_iters.argtypes = [C.c_void_p, I]
+    lib.scs_b200_g_reuse.restype = I
+    lib.scs_b200_g_reuse.argtypes = []
     lib.scs_b200_comm_unique_id.restype = I
     lib.scs_b200_comm_unique_id.argtypes = [C.c_char_p]
     lib.scs_b200_comm_init.restype = I

@@ -105,6 +105,9 @@ struct SCS_WORK {
   int equil;
   double scale0;
   double *bl_orig, *bu_orig;
+  /* adm.d_g holds (R + M)^{-1} [c; -b] for the current A, P, diag_r, d_b and d_c (DESIGN.md section 3.2, "Reusing g"):
+   * set by update_work_cache, cleared by every path that changes one of them */
+  int g_valid;
 };
 enum { B200_EQUIL_NONE = 0, B200_EQUIL_PAIR = 1, B200_EQUIL_QP_NO_P = 2, B200_EQUIL_QP = 3 };
 

@@ -551,10 +551,12 @@ int b200_linsys_scale_local(ScsLinSysWork *w, const double *d_D, const double *d
 int b200_linsys_solve_dev(ScsLinSysWork *w, double *d_b, const double *d_s, double tol,
                           const double *d_tol) {
   long long max_its = 10LL * w->n; /* reference private.c:307 */
+  int *hint = d_s ? &w->last_admm_its : &w->last_g_its; /* batching only: no result depends on it */
   int its;
   if (max_its > 2000000000LL) max_its = 2000000000LL;
-  its = b200_cg_solve(&w->cg, d_b, d_s, tol, (int)max_its, w->last_cg_its, d_tol);
+  its = b200_cg_solve(&w->cg, d_b, d_s, tol, (int)max_its, *hint, d_tol);
   if (its < 0) return -1;
+  *hint = its;
   w->last_cg_its = its;
   w->tot_cg_its += its;
   w->n_solves += 1;
@@ -591,6 +593,14 @@ scs_int scs_update_lin_sys_diag_r(ScsLinSysWork *w, const scs_float *new_diag_r)
 
 scs_int scs_b200_linsys_last_cg_its(const ScsLinSysWork *w) { return w->last_cg_its; }
 long long scs_b200_linsys_total_cg_its(const ScsLinSysWork *w) { return w->tot_cg_its; }
+
+/* SCS_B200_G_REUSE=0 makes the ADMM driver's update_work re-solve g at every scs_solve, as the reference does, for A/B
+ * runs (DESIGN.md section 3.2). Here rather than in the driver so that every library flavour exports what the header
+ * declares, the plugin-only ones included */
+scs_int scs_b200_g_reuse(void) {
+  const char *e = getenv("SCS_B200_G_REUSE");
+  return !(e && strcmp(e, "0") == 0);
+}
 
 static scs_int accum_generic(ScsLinSysWork *w, const B200Spmv *M, int ncols, int nrows,
                              const scs_float *x, scs_float *y, scs_int accumulate) {

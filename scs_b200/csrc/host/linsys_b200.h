@@ -28,7 +28,10 @@ struct SCS_LIN_SYS_WORK {
   int *d_perm, *d_inv;
   int p_in_exchange; /* cg.d_p points into the peer-mapped exchange allocation (sharded-x mode): not ours to free */
   int *offsets;
-  int last_cg_its;
+  int last_cg_its; /* the last solve of either kind */
+  /* the first CG batch of a solve is sized from the last solve of its kind: warm-started (ADMM, d_s != NULL) solves
+   * take a few dozen iterations, the cold tolerance-1e-12 solves of g a thousand or more */
+  int last_admm_its, last_g_its;
   long long tot_cg_its;
   long long n_solves;
 };

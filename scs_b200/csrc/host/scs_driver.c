@@ -466,6 +466,7 @@ scs_int scs_update(ScsWork *w, scs_float *b, scs_float *c) {
   const double t0 = now_ms();
   const int n = w->n, m = w->m;
   int i;
+  w->g_valid = 0; /* new normalised b and c */
   /* originals last set through scs_b200_update_device and kept here: their host copies are brought up to date */
   if ((!b && w->b_on_dev && b200_d2h(w->b_orig, w->d_b_orig, (size_t)m * 8) != 0) ||
       (!c && w->c_on_dev && b200_d2h(w->c_orig, w->d_c_orig, (size_t)n * 8) != 0) || b200_sync() != 0)
@@ -869,10 +870,14 @@ static int has_converged(const ScsWork *w) {
 }
 
 /* ----------------------------------------------------------------- per-solve setup */
-/* g = (I + M)^{-1} [c; -b]  (scs.c:1118-1128) */
+/* g = (I + M)^{-1} [c; -b]  (scs.c:1118-1128). h lives only in d_g and the CG overwrites it in place, so g is valid only
+ * once the solve has returned */
 static int update_work_cache(ScsWork *w) {
+  w->g_valid = 0;
   if (b200_admm_build_h(&w->adm, w->d_c, w->d_b) != 0) return -1;
-  return b200_linsys_solve_dev(w->p, w->adm.d_g, SCS_NULL, CG_BEST_TOL, SCS_NULL);
+  if (b200_linsys_solve_dev(w->p, w->adm.d_g, SCS_NULL, CG_BEST_TOL, SCS_NULL) != 0) return -1;
+  w->g_valid = 1;
+  return 0;
 }
 
 static int update_work(ScsWork *w, ScsSolution *sol) {
@@ -899,6 +904,8 @@ static int update_work(ScsWork *w, ScsSolution *sol) {
   } else {
     if (b200_admm_cold_start(&w->adm) != 0) return -1;
   }
+  /* g does not depend on the starting point: a solve on unchanged data reuses it (the CG would return the same bits) */
+  if (w->g_valid && scs_b200_g_reuse()) return 0;
   return update_work_cache(w);
 }
 
@@ -927,6 +934,7 @@ static int update_scale(ScsWork *w, int iter) {
     w->n_log_scale_factor = 0;
     w->last_scale_update_iter = iter;
     w->stgs->scale = new_scale;
+    w->g_valid = 0; /* new diag_r; g is re-solved just below */
     set_diag_r_host(w);
     if (b200_admm_set_diag_r(&w->adm, w->k->z, w->stgs->rho_x, w->stgs->scale) != 0) return -1;
     if (b200_linsys_update_diag_r_dev(w->p, w->adm.d_R) != 0) return -1;
@@ -1473,6 +1481,7 @@ scs_int scs_b200_device_ok(void) { return b200_device_ok(); }
 static int update_bc_dev(ScsWork *w) {
   const double t0 = now_ms();
   double mx[4], sigma;
+  w->g_valid = 0; /* new normalised b and c */
   if (b200_normalize_b_c_dev(w->m, w->n, w->d_b_orig, w->d_c_orig, w->D ? w->d_D : SCS_NULL, w->D ? w->d_E : SCS_NULL,
                              w->d_b, w->d_c, mx) != 0)
     return -1;
@@ -1708,6 +1717,7 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
       goto dev_fail;
     init_mark("update: pattern check", &t_mark);
     if (bad) { pattern_differs(bad & 1u ? "A" : "P"); break; }
+    w->g_valid = 0; /* from here on the operators, diag_r, b and c change (d_g is zeroed in step 6) */
     /* 2. the raw values into both orientations of A, equilibrated in place as init did */
     if (b200_spmv_scatter_values(w->p->At, dm.Ap, dm.Ax) != 0 || b200_spmv_scatter_values(w->p->A, Tp, Tx) != 0)
       goto dev_fail;
@@ -1739,7 +1749,7 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
     if (b200_admm_set_diag_r(&w->adm, w->k->z, w->stgs->rho_x, w->stgs->scale) != 0 ||
         b200_linsys_update_diag_r_dev(w->p, w->adm.d_R) != 0)
       goto dev_fail;
-    w->p->last_cg_its = 0;
+    w->p->last_cg_its = w->p->last_admm_its = w->p->last_g_its = 0;
     init_mark("update: preconditioner, CG copy", &t_mark);
     /* 5. D and E on the host (box bounds, CSV log); the box bounds renormalised from the originals */
     if (w->D && (b200_d2h(w->D, w->d_D, (size_t)m * 8) != 0 || b200_d2h(w->E, w->d_E, (size_t)n * 8) != 0 ||

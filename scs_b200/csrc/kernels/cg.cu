@@ -1374,8 +1374,9 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
   CUDA_OK(cudaGetLastError());
 
   // main loop in batches. An iteration enqueued after `done` costs 3 or 4 empty launches (~12 us), a
-  // host poll costs a ~40 us bubble: the first batch is the previous solve's count plus a 6 % margin
-  // (consecutive ADMM iterations need nearly the same number of CG steps), later batches are small.
+  // host poll costs a ~40 us bubble: the first batch is the hint, the previous count of a solve of the same kind
+  // (host/linsys_b200.c), plus a 6 % margin (consecutive ADMM iterations need nearly the same number of CG steps),
+  // later batches are small.
   int batch = its_hint + (its_hint / 16 > 2 ? its_hint / 16 : 2);
   if (batch < 4) batch = 4;
   if (batch > 512) batch = 512;  // a sharp drop of the CG count between two solves wastes at most 512 empty iterations
