@@ -25,7 +25,8 @@ extern "C" {
  * scs_finish take one made here, and these take one made by scs_init. Refused (NULL / -1, with a message): a host
  * pointer or memory of another device, a process that is one of several ranks (multi-GPU), or invalid data. Since
  * -1 is also SCS_UNBOUNDED, a refused scs_b200_solve_device is told apart by info: it is left untouched, while every
- * solve that starts writes info->lin_sys_solver first. Equilibration follows scs_init, SCS_B200_HOST_EQUIL included.
+ * solve that starts writes info->lin_sys_solver first. The operators and the equilibration are built as scs_init builds
+ * them on one GPU, with the same bits.
  * With write_data_filename or log_csv_filename set, the data needed is copied to the host (debugging modes). */
 ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, void *stream);
 scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream);

@@ -58,24 +58,17 @@ typedef struct B200Spmv B200Spmv;
 #define B200_MAX_DIM ((1LL << 30) - 1)
 #define B200_MAX_STORED (2147483647LL - 128)
 
-/* an operator from a host CSR: the arrays are uploaded and the operator is built on the device like every other
- * (b200_spmv_create_dev, kernels/spmv.cu); nrows and nnz may be 0. NULL on failure */
+/* an operator from a host CSR, for the tests (tests/test_linsys_gpu.py): the arrays are uploaded and the operator is
+ * built on the device like every other (b200_spmv_create_dev, kernels/spmv.cu); nrows and nnz may be 0. NULL on
+ * failure */
 B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr, const int *h_colidx,
                            const double *h_vals);
 void b200_spmv_destroy(B200Spmv *M);
-/* both resident orientations built ON THE DEVICE from the host CSC of A (kernels/setup.cu); m, n or nnz may be 0:
- * 0 ok, < 0 error */
-int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax, B200Spmv **A_out,
-                            B200Spmv **At_out);
-/* the same from a CSC with 64-bit column pointers and row indices (the DLONG ABI): they are uploaded and narrowed to
- * int on the device, and the build is refused (< 0) if a pointer decreases, leaves [0, nnz] or p[0] != 0, or a row
- * index leaves [0, m) -- checked before any kernel reads an index. nnz = h_Ap[n] must not exceed B200_MAX_STORED. */
-int b200_setup_ops_from_csc64(int m, int n, const long long *h_Ap, const long long *h_Ai, const double *h_Ax,
-                              B200Spmv **A_out, B200Spmv **At_out);
-/* the same from the builder's own device CSC (int32 indices, validated); the arrays are only read */
+/* both resident orientations built ON THE DEVICE (kernels/setup.cu) from the builder's own device CSC of A (int32
+ * indices, validated); m, n or nnz may be 0, the arrays are only read: 0 ok, < 0 error */
 int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d_Ap, const int *d_Ai, const double *d_Ax,
                             B200Spmv **A_out, B200Spmv **At_out);
-/* The validating copy of a caller's device CSC (idx64: 64-bit indices, narrowed) into the builder's int32 / fp64
+/* The validating copy of a CSC in device memory (idx64: 64-bit indices, narrowed) into the builder's int32 / fp64
  * arrays (kernels/setup.cu). First the pointers: *flags = B200_CSC_BAD_* bits. Only with *flags == 0, the entries:
  * *first = ~0, or (k << 2 | code) of the first entry k that fails (code B200_CSC_BAD_ROW / _UPPER / _VAL, upper != 0
  * for the upper triangle of P); *ndiag = its diagonal entries. d_x and d_Ax may both be NULL. */
@@ -85,8 +78,8 @@ int b200_csc_check_ptrs(int n, long long nnz, const void *d_p, int idx64, int *d
 int b200_csc_copy_entries(int rows, int n, long long nnz, const void *d_i, const double *d_x, int idx64,
                           const int *d_Ap, int upper, int *d_Ai, double *d_Ax, unsigned long long *first,
                           long long *ndiag);
-/* the full symmetric P from its n x n upper CSC on the device, in the CSR of the host's expand_sym_upper: the
- * structure (d_Fp n+1, d_Fi and d_Fsrc `full`: the CSC entry each full entry copies), then, from the CSC's values, the
+/* the full symmetric P from its n x n upper CSC on the device, in CSR (each row: the mirrored entries, then the
+ * direct ones): the structure (d_Fp n+1, d_Fi and d_Fsrc `full`: the CSC entry each full entry copies), then, from the CSC's values, the
  * operator and diag(P) (d_diag, n) */
 int b200_sym_expand_structure(int n, long long nnz, long long full, const int *d_Pp, const int *d_Pi, int *d_Fp,
                               int *d_Fi, int *d_Fsrc);

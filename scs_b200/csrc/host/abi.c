@@ -4,7 +4,8 @@
  * LP64). The kernel layer (dev_api.h, admm_api.h) takes int everywhere. Every count, size or index a caller passes is
  * checked here in scs_int width against the limits of the operators (dev_api.h B200_MAX_DIM, B200_MAX_STORED) and only
  * then narrowed; a value that does not fit is refused with a message that names the limit, never truncated. The
- * matrix indices of A are narrowed on the device (kernels/setup.cu b200_setup_ops_from_csc64). */
+ * matrix indices of A and P are checked and narrowed on the device, by the validating copy (kernels/setup.cu) that
+ * b200_csc_upload (host/linsys_b200.c) runs them through. */
 #include "driver.h"
 #include <stddef.h>
 #include <stdlib.h>

@@ -109,7 +109,7 @@ struct SCS_WORK {
    * set by update_work_cache, cleared by every path that changes one of them */
   int g_valid;
 };
-enum { B200_EQUIL_NONE = 0, B200_EQUIL_PAIR = 1, B200_EQUIL_QP_NO_P = 2, B200_EQUIL_QP = 3 };
+enum { B200_EQUIL_NONE = 0, B200_EQUIL_PAIR = 1, B200_EQUIL_QP = 2 };
 
 /* the integer-width boundary (host/abi.c): checks in scs_int width that print a message naming the limit and return
  * nonzero, and int copies of the cone arrays for the kernel layer */

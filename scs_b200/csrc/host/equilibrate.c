@@ -1,7 +1,8 @@
-/* equilibrate.c -- Ruiz + L2 equilibration of A (and P) on the host at setup,
+/* equilibrate.c -- Ruiz + L2 equilibration of A and P on the host at setup,
  * and the b/c scaling.  Setup path (runs once per scs_init), not part of the
- * per-iteration hot loop; SURVEY.md section 8(f) lists moving it to the GPU as
- * "next".
+ * per-iteration hot loop. The matrix equilibration serves the multi-GPU path
+ * with P != 0 only; one GPU runs its device form, b200_equilibrate_qp_dev
+ * (kernels/equil.cu), with the same bits.
  *
  * Same algorithm and constants as reference linsys/scs_matrix.c:229-496
  * (compute_ruiz_mats / compute_l2_mats / rescale / normalize_a_p: 25 Ruiz

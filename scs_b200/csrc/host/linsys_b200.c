@@ -33,69 +33,6 @@ static int b200_host_threads(long long work_items) {
   return (int)t;
 }
 
-/* expand upper-triangular CSC P into the full symmetric matrix in CSR
- * (reference gpu/indirect/private.c:174-202 does the same for cuSPARSE);
- * also extracts diag(P) for the preconditioner. The input is of scs_int width, the output int: a P whose full
- * symmetric form has more than B200_MAX_STORED entries, or a row index outside [0, n), is refused. */
-static int expand_sym_upper(int n, const scs_int *Pp, const scs_int *Pi, const double *Px, int **Fp_out,
-                            int **Fi_out, double **Fx_out, double *diag) {
-  int *cnt = (int *)calloc((size_t)n + 1, sizeof(int));
-  int *Fp = (int *)calloc((size_t)n + 1, sizeof(int));
-  int *Fi;
-  double *Fx;
-  int i, j, tot = 0;
-  scs_int k;
-  long long full = 0;
-  if (!cnt || !Fp) { free(cnt); free(Fp); return -1; }
-  for (j = 0; j < n; ++j)
-    for (k = Pp[j]; k < Pp[j + 1]; ++k) {
-      if (Pi[k] < 0 || Pi[k] >= n) {
-        fprintf(stderr, "scs_b200: P row index %lld outside [0, %d)\n", (long long)Pi[k], n);
-        free(cnt); free(Fp);
-        return -1;
-      }
-      full += Pi[k] == j ? 1 : 2;
-    }
-  if (full > B200_MAX_STORED) {
-    fprintf(stderr, "scs_b200: the full symmetric P has %lld stored entries, above the limit 2^31 - 129 of one "
-            "operator\n", full);
-    free(cnt); free(Fp);
-    return -1;
-  }
-  for (j = 0; j < n; ++j) diag[j] = 0.0;
-  for (j = 0; j < n; ++j)
-    for (k = Pp[j]; k < Pp[j + 1]; ++k) {
-      i = (int)Pi[k];
-      cnt[i]++;              /* entry (i,j) goes to row i */
-      if (i != j) cnt[j]++;  /* mirrored entry (j,i) goes to row j */
-      else diag[j] += Px[k];
-    }
-  for (i = 0; i < n; ++i) { Fp[i + 1] = Fp[i] + cnt[i]; }
-  tot = Fp[n];
-  Fi = (int *)malloc(((size_t)tot + 1) * sizeof(int));
-  Fx = (double *)malloc(((size_t)tot + 1) * sizeof(double));
-  if (!Fi || !Fx) { free(cnt); free(Fp); free(Fi); free(Fx); return -1; }
-  for (i = 0; i < n; ++i) cnt[i] = Fp[i];
-  /* rows get their entries in ascending column order: first the lower part
-   * (mirrors, columns < row) then the upper part. Two passes keep it sorted. */
-  for (j = 0; j < n; ++j)
-    for (k = Pp[j]; k < Pp[j + 1]; ++k) {
-      i = (int)Pi[k];
-      if (i != j) { /* (i,j) with i<j stored; mirror (j,i): row j, col i < j */
-        const int q = cnt[j]++;
-        Fi[q] = i; Fx[q] = Px[k];
-      }
-    }
-  for (j = 0; j < n; ++j)
-    for (k = Pp[j]; k < Pp[j + 1]; ++k) {
-      i = (int)Pi[k];
-      { const int q = cnt[i]++; Fi[q] = j; Fx[q] = Px[k]; } /* row i, col j >= i */
-    }
-  free(cnt);
-  *Fp_out = Fp; *Fi_out = Fi; *Fx_out = Fx;
-  return 0;
-}
-
 /* Row partition for the sharded KKT solve (SURVEY 8e): contiguous blocks with (nearly) equal
  * numbers of nonzeros. */
 /* generic fork-join over an array of job records (threads that cannot be created run inline) */
@@ -262,24 +199,68 @@ static void setup_mark(const char *what, double *t_last) {
   }
 }
 
-/* Both resident orientations of a CSC matrix, built on the device (kernels/setup.cu): *A_out = the m x n operator
- * (rows of A), *At_out = the n x m one (rows of A' = columns of A). */
-static int build_both_ops(int m, int n, const int *Ap, const int *Ai, const double *Ax, B200Spmv **A_out,
-                          B200Spmv **At_out, double *t_mark) {
-  if (b200_setup_ops_from_csc(m, n, Ap, Ai, Ax, A_out, At_out) != 0) return -1;
-  setup_mark("linsys: both operators built on the device", t_mark);
+/* One upload of a host CSC into the int32 / fp64 device arrays the builder takes: p and i, of 8 bytes (idx64) or 4,
+ * are staged on the device and go through the validating copy (kernels/setup.cu), which narrows them; x is copied as
+ * is and not checked. upper: the upper triangle of P, *ndiag (else NULL) then receives its diagonal entries. Refused
+ * with a message naming `what` when p[0] != 0, a pointer decreases or leaves [0, nnz], or a row index leaves [0, rows)
+ * or, with upper, lies below the diagonal: no kernel reads an index before it has been checked, in its own width (a
+ * truncated 2^32 + 3 would look valid). The staging is freed before this returns, so the builder that runs next does
+ * not hold it too. On success the caller frees *d_p, *d_i and *d_x. */
+int b200_csc_upload(const char *what, int rows, int n, const void *p, const void *i, const double *x, int idx64,
+                    int upper, int **d_p, int **d_i, double **d_x, long long *nnz_out, long long *ndiag) {
+  const size_t w = idx64 ? 8 : 4;
+  const long long nnz = idx64 ? ((const long long *)p)[n] : ((const int *)p)[n];
+  void *s_p = NULL, *s_i = NULL;
+  unsigned flags = 0;
+  unsigned long long first = ~0ULL;
+  long long nd = 0;
+  int rc = -1;
+  *d_p = NULL; *d_i = NULL; *d_x = NULL;
+  if (nnz < 0 || nnz > B200_MAX_STORED) {
+    fprintf(stderr, "scs_b200: %s refused: nnz = %lld must lie in [0, 2^31 - 129]\n", what, nnz);
+    return -1;
+  }
+  s_p = b200_malloc((size_t)(n + 1) * w);
+  s_i = b200_malloc((size_t)nnz * w);
+  *d_p = (int *)b200_malloc((size_t)(n + 1) * 4);
+  *d_i = (int *)b200_malloc((size_t)nnz * 4);
+  *d_x = (double *)b200_malloc((size_t)nnz * 8);
+  if (s_p && s_i && *d_p && *d_i && *d_x && b200_h2d(s_p, p, (size_t)(n + 1) * w) == 0 &&
+      b200_h2d(s_i, i, (size_t)nnz * w) == 0 && b200_csc_check_ptrs(n, nnz, s_p, idx64, *d_p, &flags) == 0) {
+    if (flags == 0 &&
+        b200_csc_copy_entries(rows, n, nnz, s_i, NULL, idx64, *d_p, upper, *d_i, NULL, &first, &nd) == 0 &&
+        first == ~0ULL)
+      rc = 0;
+    if (flags != 0 || first != ~0ULL)
+      fprintf(stderr, "scs_b200: %s refused: column pointers must start at 0 and not decrease, and row indices must "
+              "lie in [0, %s)%s\n", what, upper ? "n" : "m", upper ? " and on or above the diagonal" : "");
+  }
+  b200_free(s_p); /* stream-ordered: the entry pass has read them */
+  b200_free(s_i);
+  if (rc == 0 && b200_h2d(*d_x, x, (size_t)nnz * 8) != 0) rc = -1;
+  if (rc != 0) {
+    b200_free(*d_p); b200_free(*d_i); b200_free(*d_x);
+    *d_p = NULL; *d_i = NULL; *d_x = NULL;
+    return -1;
+  }
+  *nnz_out = nnz;
+  if (ndiag) *ndiag = nd;
   return 0;
 }
-/* the same from the caller's CSC, of scs_int width: with DLONG its 64-bit indices are narrowed on the device */
-static int build_both_ops_user(int m, int n, const scs_int *Ap, const scs_int *Ai, const double *Ax, B200Spmv **A_out,
-                               B200Spmv **At_out, double *t_mark) {
-#ifdef DLONG
-  if (b200_setup_ops_from_csc64(m, n, Ap, Ai, Ax, A_out, At_out) != 0) return -1;
-  setup_mark("linsys: both operators built on the device (64-bit indices narrowed there)", t_mark);
-  return 0;
-#else
-  return build_both_ops(m, n, Ap, Ai, Ax, A_out, At_out, t_mark);
-#endif
+
+/* Both resident orientations of an m x n host CSC (*A_out = the m x n operator, *At_out = the n x m one): one upload,
+ * then the device builder */
+static int ops_from_host(int m, int n, const void *p, const void *i, const double *x, int idx64, B200Spmv **A_out,
+                         B200Spmv **At_out) {
+  int *d_p, *d_i;
+  double *d_x;
+  long long nnz;
+  int rc;
+  *A_out = *At_out = NULL;
+  if (b200_csc_upload("A", m, n, p, i, x, idx64, 0, &d_p, &d_i, &d_x, &nnz, NULL) != 0) return -1;
+  rc = b200_setup_ops_from_dev(m, n, nnz, d_p, d_i, d_x, A_out, At_out);
+  b200_free(d_p); b200_free(d_i); b200_free(d_x); /* stream-ordered */
+  return rc;
 }
 
 /* The reordered pair used inside the CG operator (kernels/spmv.cu "Reordered copies", DESIGN.md section 3.1): the rows
@@ -334,6 +315,7 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
   double t_mark = wall_ms();
   int *Lp = NULL, *Li = NULL;
   double *Lx = NULL;
+  const int idx64 = sizeof(scs_int) == 8;
   int n, m;
   if (!A || b200_matrix_over_limits(A, P)) { /* in scs_int width, before anything is narrowed */
     fprintf(stderr, "scs_b200: init_lin_sys_work refused its input\n");
@@ -363,28 +345,36 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
     if (restrict_rows(n, A->p, A->i, A->x, w->row0, w->row0 + w->mloc, &Lp, &Li, &Lx) != 0) goto fail;
     setup_mark("linsys: row block cut out of A (host)", &t_mark);
     {
-      const int rc = build_both_ops(w->mloc, n, Lp, Li, Lx, &w->A, &w->At, &t_mark);
+      const int rc = ops_from_host(w->mloc, n, Lp, Li, Lx, 0, &w->A, &w->At);
       free(Lp); free(Li); free(Lx);
       if (rc != 0) goto fail;
     }
-  } else if (build_both_ops_user(m, n, A->p, A->i, A->x, &w->A, &w->At, &t_mark) != 0) {
+  } else if (ops_from_host(m, n, A->p, A->i, A->x, idx64, &w->A, &w->At) != 0) {
     goto fail;
   }
-  if (!w->A || !w->At) goto fail;
-  if (P) {
-    int *Fp = NULL, *Fi = NULL;
-    double *Fx = NULL;
-    double *diag = (double *)malloc((size_t)n * sizeof(double));
-    if (!diag || expand_sym_upper(n, P->p, P->i, P->x, &Fp, &Fi, &Fx, diag) != 0) {
-      free(diag);
-      goto fail;
+  setup_mark("linsys: both operators built on the device", &t_mark);
+  if (P) { /* replicated on every rank: the upper CSC uploaded, then expanded to the full symmetric P on the device */
+    int *Pp = NULL, *Pi = NULL, *Fp = NULL, *Fi = NULL, *Fsrc = NULL;
+    double *Px = NULL;
+    long long nnzP = 0, ndiag = 0, full;
+    int rc = -1;
+    if (b200_csc_upload("P", n, n, P->p, P->i, P->x, idx64, 1, &Pp, &Pi, &Px, &nnzP, &ndiag) != 0) goto fail;
+    full = 2 * nnzP - ndiag;
+    if (full > B200_MAX_STORED) {
+      fprintf(stderr, "scs_b200: the full symmetric P has %lld stored entries, above the limit 2^31 - 129 of one "
+              "operator\n", full);
+    } else {
+      Fp = (int *)b200_malloc(((size_t)n + 1) * 4);
+      Fi = (int *)b200_malloc((size_t)full * 4);
+      Fsrc = (int *)b200_malloc((size_t)full * 4);
+      w->d_Pdiag = (double *)b200_malloc((size_t)n * 8);
+      if (Fp && Fi && Fsrc && w->d_Pdiag && b200_sym_expand_structure(n, nnzP, full, Pp, Pi, Fp, Fi, Fsrc) == 0 &&
+          b200_sym_build(n, full, Fp, Fi, Fsrc, Px, w->d_Pdiag, &w->P) == 0)
+        rc = 0;
     }
-    w->P = b200_spmv_create(n, n, Fp, Fi, Fx);
-    w->d_Pdiag = (double *)b200_malloc((size_t)n * 8);
-    if (w->d_Pdiag) b200_h2d(w->d_Pdiag, diag, (size_t)n * 8);
-    free(Fp); free(Fi); free(Fx); free(diag);
-    if (!w->P || !w->d_Pdiag) goto fail;
-    setup_mark("linsys: operator P (host expansion, device build)", &t_mark);
+    b200_free(Pp); b200_free(Pi); b200_free(Px); b200_free(Fp); b200_free(Fi); b200_free(Fsrc); /* stream-ordered */
+    if (rc != 0) goto fail;
+    setup_mark("linsys: operator P (device expansion)", &t_mark);
   }
   if (linsys_vectors(w, diag_r, &t_mark) != 0) goto fail;
   return w;
@@ -534,7 +524,7 @@ int b200_linsys_full_equilibrate(const ScsMatrix *A, const int *bnd, int nbnd, d
   int rc = -1;
   double t_mark = wall_ms();
   B200Spmv *At = NULL, *Ar = NULL;
-  if (build_both_ops_user((int)A->m, (int)A->n, A->p, A->i, A->x, &Ar, &At, &t_mark) == 0)
+  if (ops_from_host((int)A->m, (int)A->n, A->p, A->i, A->x, sizeof(scs_int) == 8, &Ar, &At) == 0)
     rc = b200_equilibrate_dev(Ar, At, bnd, nbnd, d_D, d_E);
   setup_mark("linsys: D, E from a temporary full copy", &t_mark);
   b200_spmv_destroy(Ar);

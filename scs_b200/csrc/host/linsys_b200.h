@@ -42,6 +42,10 @@ int b200_linsys_solve_dev(ScsLinSysWork *w, double *d_b, const double *d_s, doub
 int b200_linsys_update_diag_r_dev(ScsLinSysWork *w, const double *d_diag_r);
 ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B200Spmv *P, double *d_Pdiag,
                                     const scs_float *diag_r);
+/* one upload of a host CSC (p and i of 8 bytes with idx64, else 4) into the builder's validated int32 / fp64 device
+ * arrays; refused (< 0, a message on stderr) when the CSC is malformed. upper: P's upper triangle, counted in *ndiag */
+int b200_csc_upload(const char *what, int rows, int n, const void *p, const void *i, const double *x, int idx64,
+                    int upper, int **d_p, int **d_i, double **d_x, long long *nnz, long long *ndiag);
 int b200_linsys_full_equilibrate(const ScsMatrix *A, const int *bnd, int nbnd, double *d_D, double *d_E);
 int b200_linsys_scale_local(ScsLinSysWork *w, const double *d_D, const double *d_E);
 /* contiguous row blocks balanced by nonzeros; offsets[nranks+1] (also exported for the tests) */

@@ -122,6 +122,21 @@ static void dev_mats_free(DevMats *dm) {
   b200_free(dm->Pp); b200_free(dm->Pi); b200_free(dm->Px);
   memset(dm, 0, sizeof(*dm));
 }
+/* the same blocks from a host A and P that validate_matrix has accepted (scs_init on one GPU) */
+static int dev_mats_from_host(const ScsMatrix *A, const ScsMatrix *P, DevMats *dm) {
+  const int idx64 = sizeof(scs_int) == 8;
+  long long ndiag = 0;
+  if (b200_csc_upload("A", (int)A->m, (int)A->n, A->p, A->i, A->x, idx64, 0, &dm->Ap, &dm->Ai, &dm->Ax, &dm->nnzA,
+                      SCS_NULL) != 0)
+    return -1;
+  if (P) {
+    if (b200_csc_upload("P", (int)P->n, (int)P->n, P->p, P->i, P->x, idx64, 1, &dm->Pp, &dm->Pi, &dm->Px, &dm->nnzP,
+                        &ndiag) != 0)
+      return -1;
+    dm->fullP = 2 * dm->nnzP - ndiag;
+  }
+  return 0;
+}
 static scs_int read_dev_int(const scs_int *d_v) {
   scs_int v = -1;
   if (b200_d2h(&v, d_v, sizeof(scs_int)) != 0 || b200_sync() != 0) return -1;
@@ -521,20 +536,22 @@ static int update_bc_dev(ScsWork *w);
 static int build_ops_dev(ScsWork *w, DevMats *dm);
 static void write_data_dev(const char *filename, const ScsData *d, const ScsCone *k, const ScsSettings *stgs);
 
-/* dm == NULL: scs_init, the data in host memory. Else the device-data entry point: d's arrays are device pointers,
- * validated into dm's blocks, from which the operators are built on the device (build_ops_dev) */
-static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm) {
+/* dev_data: the device-data entry point, d's arrays are device pointers, validated into dm's blocks; else scs_init,
+ * the data in host memory, validated there. On one GPU (dm != NULL) the operators are built on the device from dm's
+ * blocks (build_ops_dev), which scs_init fills from the host A and P. Several GPUs (dm == NULL, scs_init only) cut A
+ * into row blocks on the host (scs_init_lin_sys_work). */
+static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm, int dev_data) {
   ScsWork *w;
   const double t0 = now_ms();
   double t_mark = t0;
-  int n, m, i, dev_equil = 0;
+  int n, m, i, host_copy;
   B200ConeInts ci;
   size_t l;
   if (!d || !k || !stgs) {
     printf("ERROR: Missing ScsData, ScsCone, or ScsSettings input\n");
     return SCS_NULL;
   }
-  if (validate(d, k, stgs, dm) < 0) {
+  if (validate(d, k, stgs, dev_data ? dm : SCS_NULL) < 0) {
     printf("ERROR: Validation returned failure\n");
     return SCS_NULL;
   }
@@ -544,7 +561,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   }
   if (stgs->write_data_filename) { /* reference scs.c:1270-1273 */
     printf("Writing raw problem data to %s\n", stgs->write_data_filename);
-    if (dm) write_data_dev(stgs->write_data_filename, d, k, stgs);
+    if (dev_data) write_data_dev(stgs->write_data_filename, d, k, stgs);
     else scs_b200_write_data(stgs->write_data_filename, d, k, stgs);
   }
   w = (ScsWork *)calloc(1, sizeof(ScsWork));
@@ -558,26 +575,25 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   w->stgs = (ScsSettings *)calloc(1, sizeof(ScsSettings));
   if (!w->d || !w->k || !w->stgs) goto fail;
   w->d->n = n; w->d->m = m;
-  w->nnzA = dm ? dm->nnzA : d->A->p[n];
-  w->nnzP = dm ? dm->nnzP : d->P ? d->P->p[n] : 0;
-  /* Equilibrate on the device when possible (P = 0, single GPU): the user's A is uploaded as
-   * is and both resident orientations are rescaled in place (kernels/equil.cu), so no host
-   * copy of A is needed at all. Otherwise (P != 0 or row-sharded) equilibrate a host copy. */
-  dev_equil = stgs->normalize && !d->P && !getenv("SCS_B200_HOST_EQUIL");
-  /* the device form of each choice, for scs_b200_update_matrix_device: host/equilibrate.c is b200_equilibrate_qp_dev */
-  w->equil = !stgs->normalize ? B200_EQUIL_NONE : d->P ? B200_EQUIL_QP : dev_equil ? B200_EQUIL_PAIR
-                                                                                  : B200_EQUIL_QP_NO_P;
+  w->nnzA = dev_data ? dm->nnzA : d->A->p[n];
+  w->nnzP = dev_data ? dm->nnzP : d->P ? d->P->p[n] : 0;
+  /* the equilibration, for init and for scs_b200_update_matrix_device. One GPU: on the device, the pair of A alone
+   * (P = 0) or with P (b200_equilibrate_qp_dev), so no host copy of A or P is made. Several GPUs: with P = 0 on the
+   * device from temporary full copies of A; otherwise (P != 0, or no equilibration) from a host copy of A and P,
+   * equilibrated there (host/equilibrate.c) */
+  w->equil = !stgs->normalize ? B200_EQUIL_NONE : d->P ? B200_EQUIL_QP : B200_EQUIL_PAIR;
+  host_copy = !dm && w->equil != B200_EQUIL_PAIR;
   w->scale0 = stgs->scale;
-  if (dm) { /* no host copy of A or P; the host copies of b and c are filled when a host call needs them */
+  if (dev_data) { /* the host copies of b and c are filled when a host call needs them */
     w->d->b = (double *)malloc((size_t)m * 8);
     w->d->c = (double *)malloc((size_t)n * 8);
     if (!w->d->b || !w->d->c) goto fail;
   } else {
-    w->d->A = dev_equil ? SCS_NULL : copy_matrix(d->A);
-    w->d->P = d->P ? copy_matrix(d->P) : SCS_NULL;
+    w->d->A = host_copy ? copy_matrix(d->A) : SCS_NULL;
+    w->d->P = host_copy && d->P ? copy_matrix(d->P) : SCS_NULL;
     w->d->b = (double *)dup_mem(d->b, (size_t)m * 8);
     w->d->c = (double *)dup_mem(d->c, (size_t)n * 8);
-    if ((!dev_equil && !w->d->A) || (d->P && !w->d->P) || !w->d->b || !w->d->c) goto fail;
+    if ((host_copy && !w->d->A) || (host_copy && d->P && !w->d->P) || !w->d->b || !w->d->c) goto fail;
   }
   *w->k = *k;
   w->k->bu = w->k->bl = SCS_NULL; w->k->q = SCS_NULL; w->k->s = SCS_NULL;
@@ -633,7 +649,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
     w->D = (double *)malloc((size_t)m * 8);
     w->E = (double *)malloc((size_t)n * 8);
     if (!w->D || !w->E) goto fail;
-    if (!dev_equil && !dm) {
+    if (host_copy) {
       if (b200_equilibrate(w->d->P, w->d->A, w->cone_boundaries, w->cone_boundaries_len, w->D, w->E) != 0)
         goto fail;
       if (w->k->bsize > 1) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
@@ -683,7 +699,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
     w->d_D = (double *)b200_malloc((size_t)m * 8);
     w->d_E = (double *)b200_malloc((size_t)n * 8);
     if (!w->d_D || !w->d_E) goto fail;
-    if (!dev_equil && !dm) {
+    if (host_copy) {
       i |= b200_h2d(w->d_D, w->D, (size_t)m * 8);
       i |= b200_h2d(w->d_E, w->E, (size_t)n * 8);
     }
@@ -691,24 +707,17 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   if (i != 0) goto fail;
   init_mark("init: validate, copies, device vectors", &t_mark);
   if (dm) {
+    if (!dev_data && dev_mats_from_host(d->A, d->P, dm) != 0) goto fail;
     if (build_ops_dev(w, dm) != 0) goto fail;
-    init_mark("init: operators, equilibration and preconditioner from device data", &t_mark);
-  } else if (dev_equil) {
-    /* upload the raw A (both orientations), equilibrate in place on the device */
-    if (b200_comm_nranks() > 1) {
-      /* row-sharded: D, E from temporary full copies, then scale the resident row block once */
-      if (b200_linsys_full_equilibrate(d->A, w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0)
-        goto fail;
-    }
+    init_mark("init: operators, equilibration and preconditioner on the device", &t_mark);
+  } else if (!host_copy) {
+    /* row-sharded, P = 0: D, E from temporary full copies on the device, then the resident row block scaled once */
+    if (b200_linsys_full_equilibrate(d->A, w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0)
+      goto fail;
     w->p = scs_init_lin_sys_work(d->A, SCS_NULL, w->h_diag_r);
     if (!w->p) { printf("ERROR: init_lin_sys_work failure\n"); goto fail; }
     t_mark = now_ms();
-    if (b200_comm_nranks() > 1) {
-      if (b200_linsys_scale_local(w->p, w->d_D, w->d_E) != 0) goto fail;
-    } else if (b200_equilibrate_dev(w->p->A, w->p->At, w->cone_boundaries, w->cone_boundaries_len,
-                                    w->d_D, w->d_E) != 0) {
-      goto fail;
-    }
+    if (b200_linsys_scale_local(w->p, w->d_D, w->d_E) != 0) goto fail;
     if (b200_linsys_update_diag_r_dev(w->p, w->p->d_diag_r) != 0) goto fail; /* preconditioner of D A E */
     if (b200_d2h(w->D, w->d_D, (size_t)m * 8) != 0 || b200_d2h(w->E, w->d_E, (size_t)n * 8) != 0 ||
         b200_sync() != 0)
@@ -717,7 +726,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
     init_mark("init: device equilibration + preconditioner", &t_mark);
   }
   /* b, c: stores *_orig, normalises, uploads */
-  if (dm) {
+  if (dev_data) {
     w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
     w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
     if (!w->d_b_orig || !w->d_c_orig || b200_d2d(w->d_b_orig, d->b, (size_t)m * 8) != 0 ||
@@ -770,7 +779,17 @@ fail:
   return SCS_NULL;
 }
 
-ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) { return init_work(d, k, stgs, SCS_NULL); }
+ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
+  DevMats dm;
+  ScsWork *w;
+  memset(&dm, 0, sizeof(dm));
+  w = init_work(d, k, stgs, b200_comm_nranks() > 1 ? SCS_NULL : &dm, 0);
+  if (dm.Ap) { /* uploaded (a refused input never reaches the GPU): free only once the builder's kernels have run */
+    b200_sync();
+    dev_mats_free(&dm);
+  }
+  return w;
+}
 
 /* ----------------------------------------------------------------- residuals */
 static void compute_residuals(B200Residuals *r, double pd) {
@@ -1503,25 +1522,16 @@ static int update_bc_dev(ScsWork *w) {
 }
 
 /* the linear-system workspace from dm's blocks: both operators of A; with P, the structure of the full P, the
- * P-aware equilibration on the device and then P's operator and diagonal; with P = 0, the equilibration scs_init
- * uses: b200_equilibrate_dev on the built pair, or, where scs_init equilibrates on the host (SCS_B200_HOST_EQUIL),
- * b200_equilibrate_qp_dev with an empty P, which is host/equilibrate.c bit for bit */
+ * P-aware equilibration on the device and then P's operator and diagonal; with P = 0, b200_equilibrate_dev on the
+ * built pair */
 static int build_ops_dev(ScsWork *w, DevMats *dm) {
   const int n = w->n, m = w->m;
   B200Spmv *A = SCS_NULL, *At = SCS_NULL, *P = SCS_NULL;
-  int *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL, *Pp0 = SCS_NULL;
+  int *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL;
   double *d_Pdiag = SCS_NULL;
-  const int host_order = !dm->Pp && w->D && getenv("SCS_B200_HOST_EQUIL");
   int rc = -1;
   do {
     if (b200_setup_ops_from_dev(m, n, dm->nnzA, dm->Ap, dm->Ai, dm->Ax, &A, &At) != 0) break;
-    if (host_order) { /* P = 0 as an n x n matrix without entries: its column and row ranges are all empty */
-      Pp0 = (int *)b200_malloc(((size_t)n + 1) * 4);
-      if (!Pp0 || b200_memset0(Pp0, ((size_t)n + 1) * 4) != 0 ||
-          b200_equilibrate_qp_dev(A, At, Pp0, SCS_NULL, SCS_NULL, Pp0, SCS_NULL, SCS_NULL, w->cone_boundaries,
-                                  w->cone_boundaries_len, w->d_D, w->d_E) != 0)
-        break;
-    }
     if (dm->Pp) {
       Fp = (int *)b200_malloc(((size_t)n + 1) * 4);
       Fi = (int *)b200_malloc((size_t)dm->fullP * 4);
@@ -1539,7 +1549,7 @@ static int build_ops_dev(ScsWork *w, DevMats *dm) {
     A = At = P = SCS_NULL;
     d_Pdiag = SCS_NULL;
     if (!w->p) break;
-    if (w->D && !dm->Pp && !host_order) {
+    if (w->D && !dm->Pp) {
       if (b200_equilibrate_dev(w->p->A, w->p->At, w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0 ||
           b200_linsys_update_diag_r_dev(w->p, w->p->d_diag_r) != 0)
         break;
@@ -1554,7 +1564,7 @@ static int build_ops_dev(ScsWork *w, DevMats *dm) {
   } while (0);
   b200_sync();
   b200_spmv_destroy(A); b200_spmv_destroy(At); b200_spmv_destroy(P);
-  b200_free(Fp); b200_free(Fi); b200_free(Fsrc); b200_free(d_Pdiag); b200_free(Pp0);
+  b200_free(Fp); b200_free(Fi); b200_free(Fsrc); b200_free(d_Pdiag);
   return rc;
 }
 
@@ -1623,7 +1633,7 @@ ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSetti
     return SCS_NULL;
   }
   if (b200_wait_for_caller(stream) != 0) return SCS_NULL;
-  w = init_work(d, k, stgs, &dm);
+  w = init_work(d, k, stgs, &dm, 1);
   b200_sync(); /* the builder's blocks are free only once its kernels have run */
   dev_mats_free(&dm);
   b200_caller_waits(stream);
@@ -1665,7 +1675,7 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
   double t_mark = t0;
   const int n = w ? w->n : 0, m = w ? w->m : 0;
   DevMats dm;
-  int *Tp = SCS_NULL, *Ti = SCS_NULL, *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL, *Pp0 = SCS_NULL;
+  int *Tp = SCS_NULL, *Ti = SCS_NULL, *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL;
   double *Tx = SCS_NULL, *Fx = SCS_NULL;
   unsigned *d_bad = SCS_NULL, bad = ~0u;
   int rc = -1;
@@ -1724,12 +1734,6 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
     if (w->equil == B200_EQUIL_PAIR) {
       if (b200_equilibrate_dev(w->p->A, w->p->At, w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0)
         goto dev_fail;
-    } else if (w->equil == B200_EQUIL_QP_NO_P) { /* P = 0 as an n x n matrix without entries */
-      Pp0 = (int *)b200_malloc(((size_t)n + 1) * 4);
-      if (!Pp0 || b200_memset0(Pp0, ((size_t)n + 1) * 4) != 0 ||
-          b200_equilibrate_qp_dev(w->p->A, w->p->At, Pp0, SCS_NULL, SCS_NULL, Pp0, SCS_NULL, SCS_NULL,
-                                  w->cone_boundaries, w->cone_boundaries_len, w->d_D, w->d_E) != 0)
-        goto dev_fail;
     } else if (w->equil == B200_EQUIL_QP) {
       if (b200_equilibrate_qp_dev(w->p->A, w->p->At, dm.Pp, dm.Pi, dm.Px, Fp, Fi, Fsrc, w->cone_boundaries,
                                   w->cone_boundaries_len, w->d_D, w->d_E) != 0)
@@ -1782,9 +1786,6 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
       goto dev_fail;
     w->b_on_dev = w->c_on_dev = 1;
     if (update_bc_dev(w) != 0) goto dev_fail;
-    /* scs_init's host copies of A and P hold the old values: nothing reads them after init */
-    free_matrix(w->d->A); free_matrix(w->d->P);
-    w->d->A = w->d->P = SCS_NULL;
     init_mark("update: box bounds, resets, b and c", &t_mark);
     rc = 0;
     break;
@@ -1793,7 +1794,7 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
   } while (0);
   b200_sync();
   b200_free(Tp); b200_free(Ti); b200_free(Tx); b200_free(d_bad);
-  b200_free(Fp); b200_free(Fi); b200_free(Fsrc); b200_free(Fx); b200_free(Pp0);
+  b200_free(Fp); b200_free(Fi); b200_free(Fsrc); b200_free(Fx);
   dev_mats_free(&dm);
   if (rc == 0) w->setup_time = now_ms() - t0;
   b200_caller_waits(stream);

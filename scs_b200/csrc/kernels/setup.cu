@@ -1,8 +1,8 @@
 // setup.cu -- device-side construction of the two resident orientations of A at scs_init_lin_sys_work time.
 //
 // Replaces the host transpose of the reference (linsys/cpu/indirect/private.c:7-46: a stable counting sort that leaves
-// the entries of every row in ascending source-column order): the user's CSC arrays are uploaded ONCE, the CSR of A is
-// produced on the device by a STABLE radix sort of the entries by row index (stability = ascending column order inside
+// the entries of every row in ascending source-column order): the caller's CSC arrays are copied ONCE into the
+// builder's int32 / fp64 arrays by the validating copy below, the CSR of A is produced on the device by a STABLE radix sort of the entries by row index (stability = ascending column order inside
 // each row, exactly the reference's order), and both flagged-stream operators are built from device data
 // (b200_spmv_create_dev, kernels/spmv.cu, the builder of every operator). A host transpose took 0.8 s on 8 cores for C2.
 //
@@ -71,54 +71,8 @@ __global__ void k_gather_transposed(long long nnz, const int *__restrict__ perm,
   }
 }
 
-// The 64-bit CSC of the DLONG ABI narrowed to the int32 arrays of the builder, one grid-stride pass over the pointers
-// and the entries. *d_bad receives 1 if p[0] != 0, a pointer decreases or leaves [0, nnz], or a row index leaves [0, m):
-// nothing else checks the plugin path's input, and a truncated index (2^32 + 3 -> 3) would look valid.
-__global__ void k_narrow_csc(int m, int n, long long nnz, const long long *__restrict__ Ap64,
-                             const long long *__restrict__ Ai64, int *__restrict__ Ap, int *__restrict__ Ai,
-                             int *__restrict__ d_bad) {
-  const long long stride = (long long)gridDim.x * blockDim.x;
-  const long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x;
-  bool bad = false;
-  for (long long j = t; j <= n; j += stride) {
-    const long long v = Ap64[j];
-    bad |= v < 0 || v > nnz || (j == 0 && v != 0) || (j < n && Ap64[j + 1] < v);
-    Ap[j] = (int)v;
-  }
-  for (long long k = t; k < nnz; k += stride) {
-    const long long v = Ai64[k];
-    bad |= v < 0 || v >= m;
-    Ai[k] = (int)v;
-  }
-  if (bad) atomicOr(d_bad, 1);
-}
-
-// uploads the 64-bit arrays, narrows them into d_Ap / d_Ai and reads the flag back before anything reads an index
-static int narrow_csc(int m, int n, long long nnz, const long long *h_Ap64, const long long *h_Ai64, int *d_Ap,
-                      int *d_Ai) {
-  long long *d_Ap64 = (long long *)b200_malloc((size_t)(n + 1) * 8);
-  long long *d_Ai64 = (long long *)b200_malloc((size_t)nnz * 8);
-  int *d_bad = (int *)b200_malloc(4);
-  int h_bad = 1, rc = -1;
-  if (d_Ap64 && d_Ai64 && d_bad && b200_h2d(d_Ap64, h_Ap64, (size_t)(n + 1) * 8) == 0 &&
-      b200_h2d(d_Ai64, h_Ai64, (size_t)nnz * 8) == 0 && b200_memset0(d_bad, 4) == 0) {
-    const long long work = nnz > n ? nnz : (long long)n + 1;
-    const long long g = (work + 255) / 256 < 8LL * b200_num_sms() ? (work + 255) / 256 : 8LL * b200_num_sms();
-    k_narrow_csc<<<(int)g, 256, 0, (cudaStream_t)b200_stream()>>>(m, n, nnz, d_Ap64, d_Ai64, d_Ap, d_Ai, d_bad);
-    b200_count_launch(1);
-    if (cudaGetLastError() == cudaSuccess && b200_d2h(&h_bad, d_bad, 4) == 0 && b200_sync() == 0) {
-      rc = h_bad ? -1 : 0;
-      if (h_bad)
-        b200_set_error("b200_setup_ops_from_csc64: column pointers must start at 0 and not decrease, and row indices "
-                       "must lie in [0, m)", cudaErrorInvalidValue, __FILE__, __LINE__);
-    }
-  }
-  b200_sync();
-  b200_free(d_Ap64); b200_free(d_Ai64); b200_free(d_bad);
-  return rc;
-}
-
-// The validating copy of a caller's device CSC (the device-data entry points) into the builder's int32 / fp64 arrays,
+// The validating copy of a CSC in device memory (the caller's, or a host CSC staged there) into the builder's int32 /
+// fp64 arrays,
 // in two grid-stride passes templated on the index width (int, or the 64-bit indices of the DLONG ABI, narrowed as they are copied). The first pass copies the
 // column pointers and sets B200_CSC_BAD_P0 (p[0] != 0) or B200_CSC_BAD_PTR (a pointer decreases or leaves [0, nnz]).
 // The second runs only once the host has read a clean flag, so it may find an entry's column by bisection of the
@@ -292,50 +246,13 @@ extern "C" int b200_setup_ops_from_dev(int m, int n, long long nnz, const int *d
     b200_spmv_destroy(At);
     // a pending CUDA error names the failure; else the failing step has set its own message (e.g. a size limit)
     const cudaError_t e = cudaGetLastError();
-    if (e != cudaSuccess) b200_set_error("b200_setup_ops_from_csc", e, __FILE__, __LINE__);
+    if (e != cudaSuccess) b200_set_error("b200_setup_ops_from_dev", e, __FILE__, __LINE__);
     return rc;
   }
   *A_out = A;
   *At_out = At;
   return 0;
 }
-// the same from the host CSC: int32 arrays (h_Ap, h_Ai) or 64-bit ones (h_Ap64, h_Ai64, narrowed on the device by
-// k_narrow_csc), uploaded into the builder's arrays
-static int setup_ops(int m, int n, long long nnz, const int *h_Ap, const int *h_Ai, const long long *h_Ap64,
-                     const long long *h_Ai64, const double *h_Ax, B200Spmv **A_out, B200Spmv **At_out) {
-  *A_out = *At_out = nullptr;
-  if (b200_runtime_init() != 0) return -1;
-  int *d_Ap = (int *)b200_malloc((size_t)(n + 1) * 4), *d_Ai = (int *)b200_malloc((size_t)nnz * 4);
-  double *d_Ax = (double *)b200_malloc((size_t)nnz * 8);
-  double t_mark = setup_now_ms();
-  int rc = -1;
-  if (d_Ap && d_Ai && d_Ax &&
-      (h_Ap64 ? narrow_csc(m, n, nnz, h_Ap64, h_Ai64, d_Ap, d_Ai)
-              : (b200_h2d(d_Ap, h_Ap, (size_t)(n + 1) * 4) | b200_h2d(d_Ai, h_Ai, (size_t)nnz * 4))) == 0 &&
-      b200_h2d(d_Ax, h_Ax, (size_t)nnz * 8) == 0) {
-    dev_mark("H2D of the CSC arrays", &t_mark);
-    rc = b200_setup_ops_from_dev(m, n, nnz, d_Ap, d_Ai, d_Ax, A_out, At_out);
-  }
-  b200_sync();
-  b200_free(d_Ap); b200_free(d_Ai); b200_free(d_Ax);
-  return rc;
-}
-extern "C" int b200_setup_ops_from_csc(int m, int n, const int *h_Ap, const int *h_Ai, const double *h_Ax,
-                                       B200Spmv **A_out, B200Spmv **At_out) {
-  return setup_ops(m, n, h_Ap[n], h_Ap, h_Ai, nullptr, nullptr, h_Ax, A_out, At_out);
-}
-extern "C" int b200_setup_ops_from_csc64(int m, int n, const long long *h_Ap, const long long *h_Ai,
-                                         const double *h_Ax, B200Spmv **A_out, B200Spmv **At_out) {
-  const long long nnz = h_Ap[n];
-  if (nnz < 0 || nnz > B200_MAX_STORED) {
-    *A_out = *At_out = nullptr;
-    b200_set_error("b200_setup_ops_from_csc64: nnz must lie in [0, 2^31 - 129]", cudaErrorInvalidValue, __FILE__,
-                   __LINE__);
-    return -1;
-  }
-  return setup_ops(m, n, nnz, nullptr, nullptr, h_Ap, h_Ai, h_Ax, A_out, At_out);
-}
-
 // ---------------------------------------------------------------------------------------------
 // Row order for the CG-internal copy of A: rows by their smallest column index (stable, so equal keys keep the
 // original order; empty rows go last). perm[new] = old row; b200_spmv_permuted_rows refines the order and inverts it.
@@ -386,8 +303,7 @@ extern "C" int b200_gather_vec(int n, const int *d_perm, const double *d_src, do
 }
 
 // ---------------------------------------------------------------------------------------------
-// The full symmetric P from its upper-triangular CSC on the device, in exactly the CSR the host's expand_sym_upper
-// (host/linsys_b200.c) produces: row r holds first the mirrors of column r's strict-upper entries in k order, then its
+// The full symmetric P from its upper-triangular CSC on the device, in CSR: row r holds first the mirrors of column r's strict-upper entries in k order, then its
 // direct entries (r, j), j >= r, by ascending j. A stable radix sort by row of the list [every entry's mirror in (j, k)
 // order, then every direct entry in (j, k) order] gives that order; the mirror of a diagonal entry is keyed to row n,
 // which sorts last and is dropped. The structure is built first, with d_Fsrc[q] = the CSC entry that full entry q
@@ -451,7 +367,7 @@ extern "C" int b200_sym_expand_structure(int n, long long nnz, long long full, c
   b200_free(d_tmp);
   return rc;
 }
-// d_Fx[q] = d_Px[d_Fsrc[q]]; d_diag[r] = the sum of row r's diagonal entries in row order (expand_sym_upper's diag)
+// d_Fx[q] = d_Px[d_Fsrc[q]]; d_diag[r] = the sum of row r's diagonal entries in row order
 __global__ void k_sym_values(int n, const int *__restrict__ Fp, const int *__restrict__ Fi,
                              const int *__restrict__ Fsrc, const double *__restrict__ Px, double *__restrict__ Fx,
                              double *__restrict__ diag) {

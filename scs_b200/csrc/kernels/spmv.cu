@@ -704,7 +704,7 @@ static int spmv3_finish(B200Spmv *M, Spmv3Plan &P) {
 
 // ---------------------------------------------------------------------------------------------
 // Construction of a flagged-stream operator from a CSR in HBM, the one builder of every operator (A and A' by
-// kernels/setup.cu, host CSRs such as P through b200_spmv_create): stored row pointers (every row >= 1 entry) by a
+// kernels/setup.cu, P by b200_sym_build there, the tests' host CSRs through b200_spmv_create): stored row pointers (every row >= 1 entry) by a
 // scan, the flagged stream by one fill kernel; only the row pointers travel back to the host for the (sequential,
 // O(rows)) virtual-row and warp-tile passes. Returns NULL on failure, with the reason in b200_last_error().
 __global__ void k_stored_len(int nrows, const int *__restrict__ rp, int *__restrict__ out) {
@@ -784,7 +784,7 @@ extern "C" B200Spmv *b200_spmv_create_dev(int nrows, int ncols, long long nnz, c
   return M;
 }
 
-// an operator from a host CSR (P, the tests): uploaded, then built on the device like every other
+// an operator from a host CSR (the tests only): uploaded, then built on the device like every other
 extern "C" B200Spmv *b200_spmv_create(int nrows, int ncols, const int *h_rowptr, const int *h_colidx,
                                       const double *h_vals) {
   if (b200_runtime_init() != 0) return nullptr;

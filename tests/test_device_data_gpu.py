@@ -193,15 +193,6 @@ def test_int64_indices_equal_the_dlong_host_api(name, max_iters):
     assert_same(host_solve(*prob, long=True, **st), device_solve(*prob, idx=torch.int64, **st))
 
 
-@pytest.mark.parametrize("max_iters", [1, 100000])
-def test_host_equilibration_variable_is_honoured(monkeypatch, max_iters):
-    """with SCS_B200_HOST_EQUIL, P = 0: scs_init equilibrates on the host, the device door in the host's order"""
-    monkeypatch.setenv("SCS_B200_HOST_EQUIL", "1")
-    prob = PROBLEMS["random_prob"]()
-    st = dict(max_iters=max_iters, eps_abs=1e-6, eps_rel=1e-6)
-    assert_same(host_solve(*prob, **st), device_solve(*prob, **st))
-
-
 @pytest.mark.parametrize("name", ["random_prob", "mpc_bug2"])
 def test_update_and_warm_start_sequence_equals_host_api(name):
     A, P, b, c, cone = prob = read_fixture(name)

@@ -195,7 +195,9 @@ def test_plugin_abi_bit_identical(with_p):
         assert_identical(a, b, i)
 
 
-def test_plugin_refuses_a_row_index_that_truncation_would_make_valid(capfd):
+def test_plugin_refuses_a_truncatable_row_index_in_the_validating_copy(capfd):
+    """a 64-bit row index that truncation would make valid is refused by the validating copy's two passes, before any
+    builder kernel runs"""
     llib = capi.load(long=True)
     rng = np.random.default_rng(4)
     m, n = 500, 100
@@ -210,8 +212,8 @@ def test_plugin_refuses_a_row_index_that_truncation_would_make_valid(capfd):
     launches = llib.scs_b200_launch_count()
     w = llib.scs_init_lin_sys_work(C.byref(hp.A), None, capi.dptr(diag_r_scs(n, m, 0)))
     assert not w
-    # the narrowing kernel is the only kernel launched: no builder kernel ever read the refused index
-    assert llib.scs_b200_launch_count() - launches == 1
+    # the two passes of the validating copy are the only kernels launched: no builder kernel ever read the refused index
+    assert llib.scs_b200_launch_count() - launches == 2
     assert "row indices must lie in [0, m)" in capfd.readouterr().err
 
 

@@ -150,15 +150,14 @@ def host_door(A, P, b, c, cone, A2=None, P2=None, **st):
         lib.scs_finish(w)
 
 
-@pytest.mark.parametrize("name,host_equil", [("random_prob", False), ("mpc_bug1", False), ("random_prob", True)])
-def test_host_door_workspaces(monkeypatch, name, host_equil):
-    """scs_init -> update equals a fresh scs_init on A2: P = 0 with device equilibration, P != 0 (host equilibration),
-    and SCS_B200_HOST_EQUIL"""
-    if host_equil:
-        monkeypatch.setenv("SCS_B200_HOST_EQUIL", "1")
+@pytest.mark.parametrize("name,normalize", [("random_prob", 1), ("mpc_bug1", 1), ("mpc_bug1", 0)])
+def test_host_door_workspaces(name, normalize):
+    """scs_init -> update equals a fresh scs_init on A2: P = 0 equilibrated on the pair of A, P != 0 with the P-aware
+    equilibration, and P != 0 without equilibration"""
     A, P, b, c, cone = read_fixture(name)
     A2, P2 = perturbed(A, P)
-    assert_same([host_door(A2, P2, b, c, cone, **ST)], [host_door(A, P, b, c, cone, A2, P2, **ST)])
+    st = dict(ST, normalize=normalize)
+    assert_same([host_door(A2, P2, b, c, cone, **st)], [host_door(A, P, b, c, cone, A2, P2, **st)])
 
 
 @pytest.mark.parametrize("name", ["random_prob", "mpc_bug1"])
