@@ -192,7 +192,15 @@ __device__ __forceinline__ void aa_dmma(double &c0, double &c1, double a, double
                : "d"(a), "d"(b));
 }
 #define AA_BLK 4
-#define AA_WPAD 24
+// W = V'C_tile is staged as AA_BLK rows of stride AA_WPAD, one column per trailing column of the panel. The trailing
+// block is widest right after the first reflector block: NC - 1 <= 2 AA_MAX_MEM columns, which C1 covers with one warp
+// per 8 columns. The stride is that width rounded up to 8 plus 8 doubles: 8 (mod 16) doubles, so the 4 rows x 8
+// columns C2 reads per mma fall on alternate halves of the banks.
+#define AA_NCT_MAX (2 * AA_MAX_MEM)
+#define AA_WPAD (8 * ((AA_NCT_MAX + 7) / 8) + 8)
+static_assert(8 * ((AA_NCT_MAX + 7) / 8) <= AA_WPAD, "W staging narrower than the widest trailing block");
+static_assert((AA_NCT_MAX + 7) / 8 <= AA_THREADS / 32, "C1 needs one warp per 8 trailing columns");
+static_assert(AA_WPAD % 16 == 8, "W row stride: rows on alternate bank halves");
 __device__ void tsqr_eliminate_blocked(double *P, int ld, int len, int NC, double *s_tmp, double *Vt /*[4][128]*/,
                                        double *Tm /*[16]*/, double *Wm /*[4][AA_WPAD]*/) {
   const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;

@@ -42,8 +42,14 @@ def contraction(dim, seed):
     return F
 
 
+def steps(mem):
+    """40 map applications, and more for long memories: the first solve comes at the mem-th apply (min_len = mem)"""
+    return max(40, mem + 30)
+
+
 @pytest.mark.parametrize("dim,mem,type1,relax", [
     (50, 5, 1, 1.0), (5000, 10, 1, 1.0), (5000, 10, 0, 1.0), (3001, 7, 1, 0.8), (200000, 10, 1, 1.0),
+    (4099, 14, 1, 1.0), (4099, 31, 1, 1.0), (4099, 31, 0, 1.0), (50000, 20, 1, 1.5),
 ])
 def test_aa_sequence_matches_reference(lib, reflib, dim, mem, type1, relax):
     decl_ref(reflib)
@@ -56,7 +62,7 @@ def test_aa_sequence_matches_reference(lib, reflib, dim, mem, type1, relax):
     xr = np.zeros(dim)
     worst = 0.0
     n_acc = 0
-    for i in range(40):
+    for i in range(steps(mem)):
         # same driver as the reference's documented usage pattern (include/aa.h:66-84)
         if i > 0:
             nm = lib.scs_b200_aa_apply(mine, capi.dptr(xm), capi.dptr(xm_prev))
@@ -78,5 +84,54 @@ def test_aa_sequence_matches_reference(lib, reflib, dim, mem, type1, relax):
     assert worst <= 1e-9
     st = lib.scs_b200_aa_get_stats(mine)
     assert st.n_accept == n_acc
+    lib.scs_b200_aa_finish(mine)
+    reflib.aa_finish(ref)
+
+
+def test_aa_rank_deficient_history_matches_reference(lib, reflib):
+    """One apply handed the inputs of the apply before it: its S, D and Y columns are exactly zero. Without
+    regularization the pivoted QR then truncates the rank (last_rank < len) until a reset or until that column is
+    overwritten mem applies later; the truncated solve is not the exact one, so only the reference can check it."""
+    decl_ref(reflib)
+    dim, mem, repeat = 3001, 8, 12
+    F = contraction(dim, 77)
+    mine = lib.scs_b200_aa_init(dim, mem, mem, 1, 0.0, 1.0, 1.0, 1e10, 5, 0)
+    ref = reflib.aa_init(dim, mem, mem, 1, 0.0, 1.0, 1.0, 1e10, 5, 0)
+    assert mine and ref
+    xm = np.zeros(dim)
+    xr = np.zeros(dim)
+    worst = 0.0
+    n_acc = 0
+    truncated = []
+    for i in range(40):
+        if i > 0:
+            if i == repeat:
+                fm, fr = xm.copy(), xr.copy()   # the same inputs once more right after: a zero history column
+                nm = lib.scs_b200_aa_apply(mine, capi.dptr(fm), capi.dptr(xm_prev))
+                nr = reflib.aa_apply(capi.dptr(fr), capi.dptr(xr_prev), ref)
+                assert (nm > 0) == (nr > 0), (i, nm, nr)
+                n_acc += nr > 0
+            nm = lib.scs_b200_aa_apply(mine, capi.dptr(xm), capi.dptr(xm_prev))
+            nr = reflib.aa_apply(capi.dptr(xr), capi.dptr(xr_prev), ref)
+            xr = known_or(xr, xm)
+            assert (nm > 0) == (nr > 0), (i, nm, nr)
+            if nr > 0:
+                n_acc += 1
+                assert abs(nm - nr) <= 1e-6 * abs(nr), (i, nm, nr)
+            st = lib.scs_b200_aa_get_stats(mine)
+            if nm > 0 and st.last_rank < min(st.iter - 1, mem):
+                truncated.append((i, st.last_rank))
+        xm_prev, xr_prev = xm.copy(), xr.copy()
+        xm, xr = F(xm), F(xr)
+        sm = lib.scs_b200_aa_safeguard(mine, capi.dptr(xm), capi.dptr(xm_prev))
+        sr = reflib.aa_safeguard(capi.dptr(xr), capi.dptr(xr_prev), ref)
+        assert sm == sr, (i, sm, sr)
+        worst = max(worst, rel(xm, xr, 1e-300))
+        xr = known_or(xr, xm)
+    print(f"\n[rank-deficient history] accepted={n_acc} truncated (step, rank) {truncated} worst rel diff {worst:.3e}")
+    assert truncated and truncated[0] == (repeat, mem - 1)
+    assert n_acc > 10
+    assert worst <= 1e-9
+    assert lib.scs_b200_aa_get_stats(mine).n_accept == n_acc
     lib.scs_b200_aa_finish(mine)
     reflib.aa_finish(ref)
