@@ -34,5 +34,5 @@ for k, nm in enumerate(("K1 A p /R_y", "K2 A' tmp + R_x p, dot", "K3 update", "K
     print(f"{nm:28s}: {ms[k]*1e3:7.1f} us  {by[k]/ms[k]/1e6:6.0f} GB/s")
 ab = C.c_double()
 t = lib.scs_b200_time_cg_iter(w, reps, C.byref(ab))
-print(f"{'iteration (no events inside)':28s}: {t*1e3:7.1f} us  {ab.value/t/1e6:6.0f} GB/s   PDL={os.environ.get('SCS_B200_PDL', '1')}")
+print(f"{'iteration (no events inside)':28s}: {t*1e3:7.1f} us  {ab.value/t/1e6:6.0f} GB/s")
 lib.scs_free_lin_sys_work(w)

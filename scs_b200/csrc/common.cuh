@@ -4,6 +4,7 @@
 // * "last block finishes" grid reductions: every block writes its partial to a
 //   fixed slot, the last block to arrive sums the slots in index order, so a
 //   launch with a fixed grid is bit-reproducible (no fp64 atomics anywhere)
+// * the fp64 tensor-core mma (mma.sync m8n8k4 .f64 -> SASS DMMA)
 // * sm_90a TMA 1-D bulk copy + mbarrier wrappers (cp.async.bulk -> SASS UBLKCP)
 #pragma once
 #include <cuda_runtime.h>
@@ -129,6 +130,15 @@ __device__ __forceinline__ bool grid_finish(double (&mine)[NV], double *partials
     __threadfence();
   }
   return true;
+}
+
+// ---------------------------------------------------------------- fp64 tensor core (SASS DMMA)
+// One m8n8k4 fp64 mma accumulated in place: {c0, c1} += A B over the warp, with this lane's A[g][t] in a, B[t][g]
+// in b and C[g][2t], C[g][2t+1] in c0, c1 (g = lane >> 2, t = lane & 3).
+__device__ __forceinline__ void dmma_m8n8k4(double &c0, double &c1, double a, double b) {
+  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
+               : "+d"(c0), "+d"(c1)
+               : "d"(a), "d"(b));
 }
 
 // ---------------------------------------------------------------- TMA / mbarrier (sm_90a)

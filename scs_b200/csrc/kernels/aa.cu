@@ -126,56 +126,9 @@ k_aa_diffnorm(long long dim, const double *__restrict__ a, const double *__restr
 
 // ------------------------------------------------------------------ TSQR
 // Shared panel P (ld = len + AA_TILE_ROWS), column-major, NC columns. Rows [0,len) hold the
-// running triangle [R | Z]; rows [len, len+rows) the fresh tile. Eliminates the tile rows
+// running triangle [R | Z]; rows [len, ld) the fresh tile. Eliminates the tile rows
 // below the triangle with `len` Householder reflectors whose support is {j} U tile rows.
-__device__ void tsqr_eliminate(double *P, int ld, int len, int NC, int rows, double *s_tmp) {
-  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, nw = blockDim.x >> 5;
-  for (int j = 0; j < len; ++j) {
-    double *cj = P + (size_t)j * ld;
-    // sigma = sum over tile rows of column j (warp 0)
-    if (wid == 0) {
-      double sg = 0.0;
-      for (int i = lane; i < rows; i += 32) {
-        const double t = cj[len + i];
-        sg = fma(t, t, sg);
-      }
-      sg = warp_sum(sg);
-      if (lane == 0) {
-        const double alpha = cj[j];
-        double tau = 0.0, scale = 0.0, beta = alpha;
-        if (sg != 0.0) {
-          const double nrm = sqrt(fma(alpha, alpha, sg));
-          beta = (alpha >= 0.0) ? -nrm : nrm;
-          tau = (beta - alpha) / beta;
-          scale = 1.0 / (alpha - beta);
-        }
-        s_tmp[0] = tau;
-        s_tmp[1] = scale;
-        s_tmp[2] = beta;
-      }
-    }
-    __syncthreads();
-    const double tau = s_tmp[0], scale = s_tmp[1];
-    if (tau != 0.0) {
-      // trailing columns c in (j, NC): w = tau * (P[j,c] + sum_i v_i P[len+i,c]), v_i = scale * cj[len+i]
-      for (int c = j + 1 + wid; c < NC; c += nw) {
-        double *cc = P + (size_t)c * ld;
-        double w = 0.0;
-        for (int i = lane; i < rows; i += 32) w = fma(cj[len + i] * scale, cc[len + i], w);
-        w = warp_sum(w);
-        w = tau * (cc[j] + w);
-        for (int i = lane; i < rows; i += 32) cc[len + i] = fma(-w, cj[len + i] * scale, cc[len + i]);
-        if (lane == 0) cc[j] -= w;
-      }
-    }
-    __syncthreads();
-    if (tid == 0 && tau != 0.0) cj[j] = s_tmp[2];
-    // tile part of column j is now (implicitly) zero; it is never read again
-    __syncthreads();
-  }
-}
-
-// ---- the same elimination, BLOCKED (compact WY, blocks of 4 reflectors) so that the trailing update is two small
+// The elimination is BLOCKED (compact WY, blocks of 4 reflectors) so that the trailing update is two small
 // GEMMs on the fp64 tensor-core path (mma.sync.aligned.m8n8k4.f64, SASS DMMA) -- north_star "small tensor-core QR".
 // Reflector j of this TSQR step has support {row j of the triangle} U {tile rows}: the top parts of the block's
 // reflectors are distinct unit vectors, so with V = the 128 x nb matrix of their (normalised) tile parts
@@ -184,13 +137,8 @@ __device__ void tsqr_eliminate(double *P, int ld, int len, int NC, int rows, dou
 //   W = T' W
 //   C_top -= W ;  C_tile -= V W   [DMMA: M = 128 tile rows, N = trailing columns, K = 4 = the m8n8k4 depth]
 // Inside a block the reflectors are still generated and applied one at a time (to the <= 3 later columns of the
-// block). Checked against the reflector-at-a-time version in numpy (1e-16) and by the AA parity tests. Tile rows
+// block). Checked against a reflector-at-a-time elimination in numpy (1e-16) and by the AA parity tests. Tile rows
 // beyond `rows` are zero-filled by the callers, so the block always works on all AA_TILE_ROWS rows.
-__device__ __forceinline__ void aa_dmma(double &c0, double &c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
 #define AA_BLK 4
 // W = V'C_tile is staged as AA_BLK rows of stride AA_WPAD, one column per trailing column of the panel. The trailing
 // block is widest right after the first reflector block: NC - 1 <= 2 AA_MAX_MEM columns, which C1 covers with one warp
@@ -283,7 +231,7 @@ __device__ void tsqr_eliminate_blocked(double *P, int ld, int len, int NC, doubl
       for (int k0 = 0; k0 < AA_TILE_ROWS; k0 += 4) {
         const double a = (g < nb) ? Vt[g * AA_TILE_ROWS + k0 + t] : 0.0;
         const double b = (col < NC) ? bc[k0 + t] : 0.0;
-        aa_dmma(a0, a1, a, b);
+        dmma_m8n8k4(a0, a1, a, b);
       }
       if (g < nb) {
         Wm[g * AA_WPAD + 8 * wid + 2 * t] = a0;
@@ -316,7 +264,7 @@ __device__ void tsqr_eliminate_blocked(double *P, int ld, int len, int NC, doubl
       double *pa = P + (size_t)(ca < NC ? ca : 0) * ld + len + 8 * mt + g;
       double *pb = P + (size_t)(cb < NC ? cb : 0) * ld + len + 8 * mt + g;
       double x0 = (ca < NC) ? *pa : 0.0, x1 = (cb < NC) ? *pb : 0.0;
-      aa_dmma(x0, x1, a, b);
+      dmma_m8n8k4(x0, x1, a, b);
       if (ca < NC) *pa = x0;
       if (cb < NC) *pb = x1;
     }
@@ -335,7 +283,7 @@ __device__ __forceinline__ const double *aa_col(int c, int len, int type1, const
 __global__ void __launch_bounds__(AA_THREADS)
 k_aa_tsqr_local(long long dim, int len, int type1, const double *__restrict__ A_src,
                 const double *__restrict__ Y, const double *__restrict__ g,
-                double *__restrict__ cta_R, int blocked) {
+                double *__restrict__ cta_R) {
   extern __shared__ double P[];
   __shared__ double s_tmp[4];
   __shared__ double s_Vt[AA_BLK * AA_TILE_ROWS], s_Tm[AA_BLK * AA_BLK], s_Wm[AA_BLK * AA_WPAD];
@@ -353,8 +301,7 @@ k_aa_tsqr_local(long long dim, int len, int type1, const double *__restrict__ A_
       P[(size_t)c * ld + len + i] = (i < rows) ? col[r0 + i] : 0.0;
     }
     __syncthreads();
-    if (blocked) tsqr_eliminate_blocked(P, ld, len, NC, s_tmp, s_Vt, s_Tm, s_Wm);
-    else tsqr_eliminate(P, ld, len, NC, rows, s_tmp);
+    tsqr_eliminate_blocked(P, ld, len, NC, s_tmp, s_Vt, s_Tm, s_Wm);
   }
   for (int e = threadIdx.x; e < len * NC; e += blockDim.x) {
     const int i = e % len, c = e / len;
@@ -364,7 +311,7 @@ k_aa_tsqr_local(long long dim, int len, int type1, const double *__restrict__ A_
 // single CTA: combine `nblk` triangles (each len x NC, column-major, ld = len)
 __global__ void __launch_bounds__(AA_THREADS)
 k_aa_tsqr_combine(int nblk, int len, int NC, const double *__restrict__ cta_R,
-                  double *__restrict__ out, int blocked) {
+                  double *__restrict__ out) {
   extern __shared__ double P[];
   __shared__ double s_tmp[4];
   __shared__ double s_Vt[AA_BLK * AA_TILE_ROWS], s_Tm[AA_BLK * AA_BLK], s_Wm[AA_BLK * AA_WPAD];
@@ -385,8 +332,7 @@ k_aa_tsqr_combine(int nblk, int len, int NC, const double *__restrict__ cta_R,
       P[(size_t)c * ld + len + i] = v;
     }
     __syncthreads();
-    if (blocked) tsqr_eliminate_blocked(P, ld, len, NC, s_tmp, s_Vt, s_Tm, s_Wm);
-    else tsqr_eliminate(P, ld, len, NC, rows, s_tmp);
+    tsqr_eliminate_blocked(P, ld, len, NC, s_tmp, s_Vt, s_Tm, s_Wm);
   }
   for (int e = threadIdx.x; e < len * NC; e += blockDim.x) {
     const int i = e % len, c = e / len;
@@ -607,14 +553,9 @@ static double aa_solve(B200Aa *a, double *d_f, int len) {
   // 1. device TSQR of [A | Y | g]
   const double *A_src = type1 ? a->d_S : a->d_Y;
   const size_t smem = (size_t)(len + AA_TILE_ROWS) * NC * 8;
-  static int aa_fma = -1;  // SCS_B200_AA_FMA=1: reflector-at-a-time elimination on the FMA pipe (A/B of the DMMA path)
-  if (aa_fma < 0) {
-    const char *e = getenv("SCS_B200_AA_FMA");
-    aa_fma = (e && atoi(e) != 0) ? 1 : 0;
-  }
   k_aa_tsqr_local<<<a->grid, AA_THREADS, smem, ST>>>((long long)dim, len, type1, A_src, a->d_Y,
-                                                      a->d_g, a->d_cta_R, aa_fma ? 0 : 1);
-  k_aa_tsqr_combine<<<1, AA_THREADS, smem, ST>>>(a->grid, len, NC, a->d_cta_R, a->d_final_R, aa_fma ? 0 : 1);
+                                                      a->d_g, a->d_cta_R);
+  k_aa_tsqr_combine<<<1, AA_THREADS, smem, ST>>>(a->grid, len, NC, a->d_cta_R, a->d_final_R);
   b200_count_launch(2);
   if (cudaGetLastError() != cudaSuccess) info = -1;
   if (info == 0 && (b200_d2h(a->h_final_R, a->d_final_R, (size_t)len * NC * 8) != 0 || b200_sync() != 0))

@@ -970,16 +970,6 @@ extern "C" int b200_cg_set_preconditioner(const B200Cg *cg, const double *d_Pdia
   return 0;
 }
 
-// programmatic dependent launch of the CG loop's kernels (SCS_B200_PDL=0 turns it off for A/B measurements)
-static int g_pdl = -1;
-static bool cg_pdl_enabled() {
-  if (g_pdl < 0) {
-    const char *e = getenv("SCS_B200_PDL");
-    g_pdl = (e && atoi(e) == 0) ? 0 : 1;
-  }
-  return g_pdl == 1;
-}
-
 // peer-memory reduction: 0 = automatic (one pass for 2 ranks, two-phase for more), 1 = one pass, 2 = two-phase
 static int g_p2p_mode = -1;
 extern "C" void scs_b200_set_p2p_mode(int mode) { g_p2p_mode = mode; }
@@ -1066,8 +1056,8 @@ static int mat_vec(B200Cg *cg, const double *d_x, double *d_y, int with_dot, con
   const B200Spmv *A = re ? cg->A_cg : cg->A, *At = re ? cg->At_cg : cg->At;
   B200SpmvArgs a;
   memset(&a, 0, sizeof(a));
-  // K1: tmp = (A x) ./ R_y
-  a.pdl = cg_pdl_enabled() ? 1 : 0;
+  // K1: tmp = (A x) ./ R_y; every kernel of the CG loop is a programmatic dependent of its predecessor
+  a.pdl = 1;
   a.d_x = d_x; a.d_y = cg->d_tmp; a.d_init = nullptr; a.init_sign = 1.0;
   a.post = B200_POST_MUL; a.d_v = nullptr; a.d_dot = nullptr;
   k1_operand(cg, re, a);
@@ -1110,7 +1100,7 @@ static int cg_iteration_shard_x(B200Cg *cg, double *d_x, cudaEvent_t *ev = nullp
   B200SpmvArgs a;
   memset(&a, 0, sizeof(a));
   // K1 (local rows): tmp_g = (A_g p) ./ R_g
-  a.pdl = cg_pdl_enabled() ? 1 : 0;
+  a.pdl = 1;
   a.d_x = cg->d_p; a.d_y = cg->d_tmp + cg->row0; a.init_sign = 1.0; a.post = B200_POST_MUL;
   a.d_d = cg->d_ry_inv + cg->row0; a.d_skip = d_skip;
   if (b200_spmv(cg->A, &a) != 0) return -1;
@@ -1142,7 +1132,7 @@ static int cg_iteration_shard_x(B200Cg *cg, double *d_x, cudaEvent_t *ev = nullp
   const long long slice = ((long long)cg->n + G - 1) / G;
   const long long want = (slice + VEC_THREADS - 1) / VEC_THREADS;
   if (want < g) g = (int)(want < 1 ? 1 : want);
-  CUDA_OK(b200_launch(k_cgx_iteration, dim3(g), dim3(VEC_THREADS), 0, st, cg_pdl_enabled(), cg->n, pv, seq,
+  CUDA_OK(b200_launch(k_cgx_iteration, dim3(g), dim3(VEC_THREADS), 0, st, true, cg->n, pv, seq,
                       (int)(cg->P != nullptr), (const double *)cg->d_rx, (const double *)cg->d_M, cg->d_p, cg->d_Gp,
                       d_x, cg->d_r, cg->d_z, cg->d_ctl, cg->d_partials, cg->d_counter));
   if (ev) cudaEventRecord(ev[3], st);
@@ -1175,18 +1165,17 @@ static int cg_iteration(B200Cg *cg, double *d_x) {
   const int n = cg->n;
   const int g = k34_grid(n);
   if (mat_vec(cg, cg->d_p, cg->d_Gp, 1, &cg->d_ctl->done) != 0) return -1;
-  const bool pdl = cg_pdl_enabled();
   if (cg->k34_fused) {
-    CUDA_OK(b200_launch(k_cg_update_p, dim3(g), dim3(VEC_THREADS), 0, st, pdl, n, d_x, cg->d_r, cg->d_p,
+    CUDA_OK(b200_launch(k_cg_update_p, dim3(g), dim3(VEC_THREADS), 0, st, true, n, d_x, cg->d_r, cg->d_p,
                         (const double *)cg->d_Gp, (const double *)cg->d_M, cg->d_ctl, cg->d_partials, cg->d_counter,
                         (unsigned long long *)nullptr));
     b200_count_launch(1);
     return 0;
   }
-  CUDA_OK(b200_launch(k_cg_update, dim3(g), dim3(VEC_THREADS), 0, st, pdl, n, d_x, cg->d_r, (const double *)cg->d_p,
+  CUDA_OK(b200_launch(k_cg_update, dim3(g), dim3(VEC_THREADS), 0, st, true, n, d_x, cg->d_r, (const double *)cg->d_p,
                       (const double *)cg->d_Gp, (const double *)cg->d_M, cg->d_z, cg->d_ctl, cg->d_partials,
                       cg->d_counter));
-  CUDA_OK(b200_launch(k_cg_pupdate, dim3(g), dim3(VEC_THREADS), 0, st, pdl, n, cg->d_p, (const double *)cg->d_z,
+  CUDA_OK(b200_launch(k_cg_pupdate, dim3(g), dim3(VEC_THREADS), 0, st, true, n, cg->d_p, (const double *)cg->d_z,
                       (const B200CgCtl *)cg->d_ctl));
   b200_count_launch(2);
   return 0;

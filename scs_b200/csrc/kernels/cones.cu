@@ -283,60 +283,8 @@ __global__ void k_psd_unpack(int k, int count, const int *__restrict__ off,
     M[e] = (i == j) ? v * sqrt2 : v;
   }
 }
-// X = sum_{lambda_c > 0} lambda_c v_c v_c' ; write packed lower triangle (diag / sqrt2) with
-// post-scaling. One CTA per (block, 32x32 output tile with ti >= tj).
-#define PT 32
-__global__ void __launch_bounds__(PT * 8)
-k_psd_reconstruct(int k, int count, const int *__restrict__ off, const double *__restrict__ mats,
-                  const double *__restrict__ evals, double *__restrict__ x, const double *sv,
-                  const double *ry) {
-  __shared__ double sA[PT][PT + 1];  // V[i0+ii, c] * lambda_c
-  __shared__ double sB[PT][PT + 1];  // V[j0+jj, c]
-  const int b = blockIdx.z;
-  const int ti = blockIdx.y, tj = blockIdx.x;
-  if (tj > ti) return;
-  const double *V = mats + (size_t)b * k * k;
-  const double *lam = evals + (size_t)b * k;
-  const int i0 = ti * PT, j0 = tj * PT;
-  const int tx = threadIdx.x % PT, ty = threadIdx.x / PT;  // ty in 0..7 ; each thread 4 rows
-  double acc[4] = {0, 0, 0, 0};
-  for (int c0 = 0; c0 < k; c0 += PT) {
-    // load tiles: sA[ii][cc] = V[i0+ii + (c0+cc)*k] * max(lam,0); sB[jj][cc] = V[j0+jj + (c0+cc)*k]
-    for (int e = threadIdx.x; e < PT * PT; e += blockDim.x) {
-      const int rr = e % PT, cc = e / PT;
-      const int c = c0 + cc;
-      double la = 0.0, va = 0.0, vb = 0.0;
-      if (c < k) {
-        la = lam[c];
-        la = la > 0.0 ? la : 0.0;
-        if (i0 + rr < k) va = V[(size_t)(i0 + rr) + (size_t)c * k];
-        if (j0 + rr < k) vb = V[(size_t)(j0 + rr) + (size_t)c * k];
-      }
-      sA[rr][cc] = va * la;
-      sB[rr][cc] = vb;
-    }
-    __syncthreads();
-#pragma unroll 8
-    for (int cc = 0; cc < PT; ++cc) {
-      const double bj = sB[tx][cc];
-#pragma unroll
-      for (int r = 0; r < 4; ++r) acc[r] = fma(sA[ty * 4 + r][cc], bj, acc[r]);
-    }
-    __syncthreads();
-  }
-  const double inv_sqrt2 = 1.0 / sqrt(2.0);
-  const long long base = off[b];
-#pragma unroll
-  for (int r = 0; r < 4; ++r) {
-    const int i = i0 + ty * 4 + r, j = j0 + tx;
-    if (i < k && j < k && i >= j) {
-      const double val = (i == j) ? acc[r] * inv_sqrt2 : acc[r];
-      const long long row = base + packed_idx(i, j, k);
-      x[row] = post_scale(val, ry, sv, row);
-    }
-  }
-}
-// Same contraction on the fp64 TENSOR-CORE path: mma.sync.aligned.m8n8k4.row.col.f64 (DMMA; SASS "DMMA").
+// X = sum_{lambda_c > 0} lambda_c v_c v_c', written as a packed lower triangle (diag / sqrt2) with post-scaling,
+// on the fp64 TENSOR-CORE path: mma.sync.aligned.m8n8k4.row.col.f64 (DMMA; SASS "DMMA").
 // wgmma has no fp64 kind, so this is the tensor pipe an fp64 contraction at 1e-13 parity can use on sm_90a
 // (north_star: "tensor-core GEMM for the dense Z+ Z+' contraction", reference cones.c:1058-1062 dsyrk).
 // CTA = 4 warps = one 32x32 output tile (ti >= tj) of one block; warp w owns the 16x16 quadrant (w >> 1, w & 1)
@@ -351,13 +299,9 @@ k_psd_reconstruct(int k, int count, const int *__restrict__ off, const double *_
 //  REC_RECT    V of order ld = rows + cols, output the dense column-major rows x cols block
 //              V[0:rows, :] diag(w) V[rows:ld, :]' (nuclear-norm cone, from the symmetric embedding); only the
 //              last `cols` columns of V carry weight, so the chunk loop starts at the chunk holding column ld - cols.
+#define PT 32
 #define PTD 36
 enum { REC_PSD = 0, REC_SIGNED = 1, REC_RECT = 2 };
-__device__ __forceinline__ void dmma_m8n8k4(double &c0, double &c1, double a, double b) {
-  asm volatile("mma.sync.aligned.m8n8k4.row.col.f64.f64.f64.f64 {%0,%1}, {%2}, {%3}, {%0,%1};"
-               : "+d"(c0), "+d"(c1)
-               : "d"(a), "d"(b));
-}
 template <int MODE>
 __global__ void __launch_bounds__(128)
 k_reconstruct_dmma(int ld, int rows, int cols, int count, const int *__restrict__ off,
@@ -836,16 +780,7 @@ extern "C" int b200_cones_project_rest(B200Cones *c, double *d_x, const double *
       b200_psd_info_or(g.count, g.d_info, c->d_err);
       const int nt = (k + PT - 1) / PT;
       dim3 rg(nt, nt, g.count);
-      static int psd_fma = -1;  // SCS_B200_PSD_FMA=1: the plain fp64 FMA contraction (A/B measurement of the DMMA path)
-      if (psd_fma < 0) {
-        const char *e = getenv("SCS_B200_PSD_FMA");
-        psd_fma = (e && atoi(e) != 0) ? 1 : 0;
-      }
-      if (psd_fma)
-        k_psd_reconstruct<<<rg, PT * 8, 0, st>>>(k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
-      else
-        k_reconstruct_dmma<REC_PSD><<<rg, 128, 0, st>>>(k, k, k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s,
-                                                         d_ry);
+      k_reconstruct_dmma<REC_PSD><<<rg, 128, 0, st>>>(k, k, k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
       b200_count_launch(1);
     }
   }

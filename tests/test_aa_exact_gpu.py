@@ -19,10 +19,7 @@ One sequence of mem + 6 applies with min_len = 1 solves every len from 1 to mem 
 aa_safeguard is not called (a reset would restart the history); test_aa_gpu.py covers it against the reference.
 """
 import ctypes as C
-import json
 import os
-import subprocess
-import sys
 from fractions import Fraction
 
 import mpmath
@@ -210,33 +207,6 @@ def test_tile_and_grid_edges(lib, mem, where):
 @pytest.mark.parametrize("type1", [1, 0])
 def test_regularization_and_relaxation(lib, type1, reg, relax):
     check(lib, 2500, 20, type1, reg=reg, relax=relax)
-
-
-FMA_CHILD = """
-import json, sys
-sys.path[:0] = [{root!r}, {tests!r}]
-from scs_b200 import capi
-import test_aa_exact_gpu as t
-out = []
-for dim in (129, t.tiles_past_grid(3)):
-    results, fails = t.run_sequence(capi.load(), dim, t.MAX_MEM, 1)
-    out.append(dict(dim=dim, lens=sorted({{n for n, _ in results}}), worst=max(r for _, r in results), fails=fails))
-print("RESULT " + json.dumps(out))
-"""
-
-
-def test_fma_elimination_every_len():
-    """SCS_B200_AA_FMA=1 (the reflector-at-a-time elimination) is read once per process: a child process runs the
-    mem 31 type-I sequences with it"""
-    env = dict(os.environ, SCS_B200_AA_FMA="1")
-    code = FMA_CHILD.format(root=ROOT, tests=os.path.join(ROOT, "tests"))
-    p = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=1200)
-    assert p.returncode == 0, p.stderr[-4000:]
-    line = next(s for s in p.stdout.splitlines() if s.startswith("RESULT "))
-    for case in json.loads(line[len("RESULT "):]):
-        print(f"\n[aa exact FMA dim={case['dim']} mem=31 typeI] worst observed/gate {case['worst']:.3e}")
-        assert case["lens"] == list(range(1, MAX_MEM + 1))
-        assert not case["fails"], case["fails"][:3]
 
 
 # ---- solver level: long memories inside scs()
