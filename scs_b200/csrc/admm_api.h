@@ -138,6 +138,19 @@ void b200_psd_info_or(int count, const int *d_info, int *d_err);
 void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_x, double *d_mats);
 void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off, const double *d_mats,
                              const double *d_w, double *d_x, const double *d_s, const double *d_ry);
+/* Every launcher of the eigen-decomposition cones, and every batched eigensolver call, covers a group of one order in
+ * sub-batches of at most B200_EIG_BATCH blocks, and the eigensolver workspace is sized for min(count, B200_EIG_BATCH).
+ * The per-block kernels take the block index from gridDim.y or gridDim.z, which stop at 65535; and
+ * cusolverDnXsyevBatched asks for about 0.5 MB of workspace per matrix whatever its order (measured on an H100 with
+ * cuSOLVER 11.7.5: 35 GB for 65535 matrices of order 2), while cuSOLVER 11.7.3 (CUDA 12.8, the build PyTorch wheels
+ * bundle) refuses the workspace query from 32767 matrices on (16384 pass). 4096 keeps the workspace near 2 GB. */
+#define B200_EIG_BATCH 4096
+/* cusolverDnXsyevBatched (eigenvectors, lower triangle) on count matrices of order n, sub-batch by sub-batch, then
+ * the status words ORed into d_err; solver / params: cusolverDnHandle_t / cusolverDnParams_t. 0, or -1 with the error
+ * recorded as `what`. */
+int b200_syevd_batched(void *solver, void *params, int n, double *d_mats, double *d_evals, void *d_work,
+                       size_t work_bytes, void *h_work, size_t h_work_bytes, int *d_info, int count, int *d_err,
+                       const char *what);
 void b200_cones_destroy(B200Cones *c);
 /* new box bounds (HOST arrays of bsize - 1, already scaled) and the box Newton warm start back to 1, as at creation */
 int b200_cones_set_box(B200Cones *c, const double *h_bl, const double *h_bu);

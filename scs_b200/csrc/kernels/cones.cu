@@ -377,24 +377,50 @@ k_reconstruct_dmma(int ld, int rows, int cols, int count, const int *__restrict_
       }
 }
 // Launchers for kernels/cones_spectral.cu (count blocks; off[b] = first row of block b's matrix)
+// (blocks b0 .. b0 + nb - 1 of a sub-batch: offset pointers, the kernels index the sub-batch from 0)
 extern "C" void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_x, double *d_mats) {
-  dim3 ug((k * k + 255) / 256, count);
-  k_psd_unpack<<<ug, 256, 0, (cudaStream_t)b200_stream()>>>(k, count, d_off, d_x, d_mats);
-  b200_count_launch(1);
+  for (int b0 = 0; b0 < count; b0 += B200_EIG_BATCH) {
+    const int nb = std::min(B200_EIG_BATCH, count - b0);
+    dim3 ug((k * k + 255) / 256, nb);
+    k_psd_unpack<<<ug, 256, 0, (cudaStream_t)b200_stream()>>>(k, nb, d_off + b0, d_x, d_mats + (size_t)b0 * k * k);
+    b200_count_launch(1);
+  }
 }
 extern "C" void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off,
                                         const double *d_mats, const double *d_w, double *d_x, const double *d_s,
                                         const double *d_ry) {
   cudaStream_t st = (cudaStream_t)b200_stream();
   const int ntr = (rows + PT - 1) / PT, ntc = (cols + PT - 1) / PT;
-  dim3 rg(ntc, ntr, count);
-  if (mode == REC_PSD)
-    k_reconstruct_dmma<REC_PSD><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
-  else if (mode == REC_RECT)
-    k_reconstruct_dmma<REC_RECT><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
-  else
-    k_reconstruct_dmma<REC_SIGNED><<<rg, 128, 0, st>>>(ld, rows, cols, count, d_off, d_mats, d_w, d_x, d_s, d_ry);
-  b200_count_launch(1);
+  for (int b0 = 0; b0 < count; b0 += B200_EIG_BATCH) {
+    const int nb = std::min(B200_EIG_BATCH, count - b0);
+    const int *off = d_off + b0;
+    const double *V = d_mats + (size_t)b0 * ld * ld, *w = d_w + (size_t)b0 * ld;
+    dim3 rg(ntc, ntr, nb);
+    if (mode == REC_PSD)
+      k_reconstruct_dmma<REC_PSD><<<rg, 128, 0, st>>>(ld, rows, cols, nb, off, V, w, d_x, d_s, d_ry);
+    else if (mode == REC_RECT)
+      k_reconstruct_dmma<REC_RECT><<<rg, 128, 0, st>>>(ld, rows, cols, nb, off, V, w, d_x, d_s, d_ry);
+    else
+      k_reconstruct_dmma<REC_SIGNED><<<rg, 128, 0, st>>>(ld, rows, cols, nb, off, V, w, d_x, d_s, d_ry);
+    b200_count_launch(1);
+  }
+}
+extern "C" int b200_syevd_batched(void *solver, void *params, int n, double *d_mats, double *d_evals, void *d_work,
+                                  size_t work_bytes, void *h_work, size_t h_work_bytes, int *d_info, int count,
+                                  int *d_err, const char *what) {
+  for (int b0 = 0; b0 < count; b0 += B200_EIG_BATCH) {
+    const int nb = std::min(B200_EIG_BATCH, count - b0);
+    const cusolverStatus_t cs = cusolverDnXsyevBatched(
+        (cusolverDnHandle_t)solver, (cusolverDnParams_t)params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, n,
+        CUDA_R_64F, d_mats + (size_t)b0 * n * n, n, CUDA_R_64F, d_evals + (size_t)b0 * n, CUDA_R_64F, d_work,
+        work_bytes, h_work, h_work_bytes, d_info + b0, nb);
+    if (cs != CUSOLVER_STATUS_SUCCESS) {
+      b200_set_error(what, cudaErrorUnknown, __FILE__, __LINE__);
+      return -1;
+    }
+  }
+  b200_psd_info_or(count, d_info, d_err);
+  return 0;
 }
 __global__ void k_psd_order1(int count, const int *__restrict__ off, double *__restrict__ x,
                              const double *sv, const double *ry) {
@@ -612,10 +638,14 @@ extern "C" B200Cones *b200_cones_create(int m, int nz, int nl, int bsize, const 
       rc |= b200_h2d(g.d_off, kv.second.data(), (size_t)count * 4);
       rc |= b200_sync();
       size_t wd = 0, wh = 0;
-      if (cusolverDnXsyevBatched_bufferSize(c->solver, c->solver_params, CUSOLVER_EIG_MODE_VECTOR,
-                                            CUBLAS_FILL_MODE_LOWER, k, CUDA_R_64F, g.d_mats, k,
-                                            CUDA_R_64F, g.d_evals, CUDA_R_64F, &wd, &wh,
-                                            count) != CUSOLVER_STATUS_SUCCESS) {
+      const cusolverStatus_t bs = cusolverDnXsyevBatched_bufferSize(
+          c->solver, c->solver_params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, k, CUDA_R_64F, g.d_mats, k,
+          CUDA_R_64F, g.d_evals, CUDA_R_64F, &wd, &wh, std::min(count, B200_EIG_BATCH));
+      if (bs != CUSOLVER_STATUS_SUCCESS) {
+        char what[112];
+        snprintf(what, sizeof(what), "cusolverDnXsyevBatched_bufferSize (order %d, %d blocks): status %d", k,
+                 std::min(count, B200_EIG_BATCH), (int)bs);
+        b200_set_error(what, cudaErrorUnknown, __FILE__, __LINE__);
         drop_group();
         return nullptr;
       }
@@ -766,22 +796,11 @@ extern "C" int b200_cones_project_rest(B200Cones *c, double *d_x, const double *
   if (c->groups) {
     for (auto &g : *c->groups) {
       const int k = g.k;
-      dim3 ug((k * k + 255) / 256, g.count);
-      k_psd_unpack<<<ug, 256, 0, st>>>(k, g.count, g.d_off, d_x, g.d_mats);
-      b200_count_launch(1);
-      cusolverStatus_t cs = cusolverDnXsyevBatched(
-          c->solver, c->solver_params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, k,
-          CUDA_R_64F, g.d_mats, k, CUDA_R_64F, g.d_evals, CUDA_R_64F, g.d_work, g.work_bytes,
-          g.h_work, g.h_work_bytes, g.d_info, g.count);
-      if (cs != CUSOLVER_STATUS_SUCCESS) {
-        b200_set_error("cusolverDnXsyevBatched", cudaErrorUnknown, __FILE__, __LINE__);
+      b200_psd_unpack_launch(k, g.count, g.d_off, d_x, g.d_mats);
+      if (b200_syevd_batched(c->solver, c->solver_params, k, g.d_mats, g.d_evals, g.d_work, g.work_bytes, g.h_work,
+                             g.h_work_bytes, g.d_info, g.count, c->d_err, "cusolverDnXsyevBatched") != 0)
         return -1;
-      }
-      b200_psd_info_or(g.count, g.d_info, c->d_err);
-      const int nt = (k + PT - 1) / PT;
-      dim3 rg(nt, nt, g.count);
-      k_reconstruct_dmma<REC_PSD><<<rg, 128, 0, st>>>(k, k, k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
-      b200_count_launch(1);
+      b200_reconstruct_launch(REC_PSD, k, k, k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
     }
   }
   // ---- complex PSD

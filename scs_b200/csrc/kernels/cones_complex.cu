@@ -19,6 +19,7 @@
 #include "../common.cuh"
 #include "../admm_api.h"
 #include <cusolverDn.h>
+#include <algorithm>
 #include <map>
 #include <math.h>
 #include <stdlib.h>
@@ -150,7 +151,6 @@ struct B200CpsdCones {
   cusolverDnParams_t params;
   int *d_err;  // sticky "an eigen-decomposition failed" flag, owned by B200Cones (cones.cu)
 };
-extern "C" void b200_psd_info_or(int count, const int *d_info, int *d_err);  // cones.cu
 extern "C" void b200_cpsd_set_err(B200CpsdCones *c, int *d_err) { c->d_err = d_err; }
 
 extern "C" void b200_cpsd_destroy(B200CpsdCones *c) {
@@ -199,7 +199,7 @@ extern "C" B200CpsdCones *b200_cpsd_create(int cssize, const int *h_cs, long lon
     ok = ok && cusolverDnXsyevBatched_bufferSize(c->solver, c->params, CUSOLVER_EIG_MODE_VECTOR,
                                                  CUBLAS_FILL_MODE_LOWER, g.K, CUDA_R_64F, g.d_mats, g.K,
                                                  CUDA_R_64F, g.d_evals, CUDA_R_64F, &wd, &wh,
-                                                 g.count) == CUSOLVER_STATUS_SUCCESS;
+                                                 std::min(g.count, B200_EIG_BATCH)) == CUSOLVER_STATUS_SUCCESS;
     if (ok) {
       g.work_bytes = wd;
       g.h_work_bytes = wh;
@@ -220,21 +220,25 @@ extern "C" B200CpsdCones *b200_cpsd_create(int cssize, const int *h_cs, long lon
 extern "C" int b200_cpsd_project(B200CpsdCones *c, double *d_x, const double *d_s, const double *d_ry) {
   cudaStream_t st = (cudaStream_t)b200_stream();
   for (auto &g : c->groups) {
-    dim3 ug((g.K * g.K + 255) / 256, g.count);
-    k_cpsd_unpack<<<ug, 256, 0, st>>>(g.kc, g.count, g.d_off, d_x, g.d_mats);
-    cusolverStatus_t cs = cusolverDnXsyevBatched(
-        c->solver, c->params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, g.K, CUDA_R_64F, g.d_mats,
-        g.K, CUDA_R_64F, g.d_evals, CUDA_R_64F, g.d_work, g.work_bytes, g.h_work, g.h_work_bytes, g.d_info,
-        g.count);
-    if (cs != CUSOLVER_STATUS_SUCCESS) {
-      b200_set_error("cusolverDnXsyevBatched (complex PSD embedding)", cudaErrorUnknown, __FILE__, __LINE__);
-      return -1;
+    const size_t KK = (size_t)g.K * g.K;
+    for (int b0 = 0; b0 < g.count; b0 += B200_EIG_BATCH) {
+      const int nb = std::min(B200_EIG_BATCH, g.count - b0);
+      dim3 ug((g.K * g.K + 255) / 256, nb);
+      k_cpsd_unpack<<<ug, 256, 0, st>>>(g.kc, nb, g.d_off + b0, d_x, g.d_mats + b0 * KK);
+      b200_count_launch(1);
     }
+    if (b200_syevd_batched(c->solver, c->params, g.K, g.d_mats, g.d_evals, g.d_work, g.work_bytes, g.h_work,
+                           g.h_work_bytes, g.d_info, g.count, c->d_err,
+                           "cusolverDnXsyevBatched (complex PSD embedding)") != 0)
+      return -1;
     const int nt = (g.K + CPT - 1) / CPT;
-    b200_psd_info_or(g.count, g.d_info, c->d_err);
-    dim3 rg(nt, nt, g.count);
-    k_cpsd_reconstruct<<<rg, CPT * 8, 0, st>>>(g.kc, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
-    b200_count_launch(2);
+    for (int b0 = 0; b0 < g.count; b0 += B200_EIG_BATCH) {
+      const int nb = std::min(B200_EIG_BATCH, g.count - b0);
+      dim3 rg(nt, nt, nb);
+      k_cpsd_reconstruct<<<rg, CPT * 8, 0, st>>>(g.kc, nb, g.d_off + b0, g.d_mats + b0 * KK,
+                                                 g.d_evals + (size_t)b0 * g.K, d_x, d_s, d_ry);
+      b200_count_launch(1);
+    }
   }
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -36,6 +36,7 @@
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
+#include <algorithm>
 #include <map>
 #include <utility>
 #include <vector>
@@ -1030,7 +1031,7 @@ static bool init_group(B200SpecCones *c, EigGroup &g, const std::vector<int> &of
   size_t wd = 0, wh = 0;
   ok = ok && cusolverDnXsyevBatched_bufferSize(c->solver, c->params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER,
                                                g.N, CUDA_R_64F, g.d_mats, g.N, CUDA_R_64F, g.d_evals, CUDA_R_64F,
-                                               &wd, &wh, g.count) == CUSOLVER_STATUS_SUCCESS;
+                                               &wd, &wh, std::min(g.count, B200_EIG_BATCH)) == CUSOLVER_STATUS_SUCCESS;
   if (ok) {
     g.work_bytes = wd;
     g.h_work_bytes = wh;
@@ -1183,15 +1184,8 @@ extern "C" B200SpecCones *b200_spec_create(int dsize, const int *h_d, int nucsiz
 }
 
 static int syevd(B200SpecCones *c, EigGroup &g, const char *what) {
-  const cusolverStatus_t cs = cusolverDnXsyevBatched(
-      c->solver, c->params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, g.N, CUDA_R_64F, g.d_mats, g.N,
-      CUDA_R_64F, g.d_evals, CUDA_R_64F, g.d_work, g.work_bytes, g.h_work, g.h_work_bytes, g.d_info, g.count);
-  if (cs != CUSOLVER_STATUS_SUCCESS) {
-    b200_set_error(what, cudaErrorUnknown, __FILE__, __LINE__);
-    return -1;
-  }
-  b200_psd_info_or(g.count, g.d_info, c->d_err);
-  return 0;
+  return b200_syevd_batched(c->solver, c->params, g.N, g.d_mats, g.d_evals, g.d_work, g.work_bytes, g.h_work,
+                            g.h_work_bytes, g.d_info, g.count, c->d_err, what);
 }
 
 extern "C" int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_s, const double *d_ry) {
@@ -1214,9 +1208,12 @@ extern "C" int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_
   }
   // ---- nuclear-norm cones
   for (auto &g : c->nuc) {
-    dim3 eg((g.N * g.N + 255) / 256, g.count);
-    k_nuc_embed<<<eg, 256, 0, st>>>(g.m, g.n, g.count, g.d_off, d_x, g.d_mats);
-    b200_count_launch(1);
+    for (int b0 = 0; b0 < g.count; b0 += B200_EIG_BATCH) {
+      const int nb = std::min(B200_EIG_BATCH, g.count - b0);
+      dim3 eg((g.N * g.N + 255) / 256, nb);
+      k_nuc_embed<<<eg, 256, 0, st>>>(g.m, g.n, nb, g.d_off + b0, d_x, g.d_mats + (size_t)b0 * g.N * g.N);
+      b200_count_launch(1);
+    }
     if (syevd(c, g, "cusolverDnXsyevBatched (nuclear-norm cone embedding)") != 0) return -1;
     k_nuc_vector<<<g.count, NUC_T, 0, st>>>(g.m, g.n, g.count, g.d_off, g.d_evals, d_x, d_s, d_ry);
     b200_count_launch(1);
