@@ -100,15 +100,6 @@ int b200_cones_set_triples(B200Cones *c, int ep, int ed, int psize, const double
 int b200_cone_triples_project(int n_exp_primal, int n_exp_dual, int n_pow, long long exp_off,
                               const double *d_pow, double *d_x, const double *d_s, const double *d_ry);
 /* complex PSD blocks (kernels/cones_complex.cu; reference cones.c:1072-1156). n_triples = ep + ed + psize. */
-typedef struct B200CpsdCones B200CpsdCones;
-B200CpsdCones *b200_cpsd_create(int cssize, const int *h_cs, long long first_row);
-int b200_cpsd_project(B200CpsdCones *c, double *d_x, const double *d_s, const double *d_ry);
-void b200_cpsd_destroy(B200CpsdCones *c);
-void b200_cpsd_set_err(B200CpsdCones *c, int *d_err);
-/* cuSOLVER handles are expensive to create (a cuBLAS handle + workspace each): workspaces borrow them from a small
- * per-device cache and hand them back at destroy (kernels/cones.cu). The pointer is a cusolverDnHandle_t. */
-void *b200_solver_acquire(void);
-void b200_solver_release(void *handle);
 int b200_cones_set_complex_psd(B200Cones *c, int cssize, const int *h_cs, int n_triples);
 /* log-det (d), nuclear-norm (nuc_m x nuc_n), l1-norm (ell1) and sum-of-largest-eigenvalues (sl_n, sl_k) cones of the
  * spectral build: the LAST rows of the cone product, in that order (kernels/cones_spectral.cu; reference
@@ -122,35 +113,6 @@ int b200_cones_reset_spectral(B200Cones *c);
 /* the Newton_stats record (iter, newton_success, residuals) of the last log-det cone projected; -1 when there are
  * no log-det cones. Syncs. */
 int b200_cones_logdet_stats(B200Cones *c, int *iter, int *newton_success, double res[3]);
-typedef struct B200SpecCones B200SpecCones;
-B200SpecCones *b200_spec_create(int dsize, const int *h_d, int nucsize, const int *h_nuc_m, const int *h_nuc_n,
-                                int ell1_size, const int *h_ell1, int sl_size, const int *h_sl_n, const int *h_sl_k,
-                                long long first_row, int *d_err);
-int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_s, const double *d_ry);
-int b200_spec_reset(B200SpecCones *c);
-int b200_spec_logdet_stats(B200SpecCones *c, int *iter, int *newton_success, double res[3]);
-void b200_spec_destroy(B200SpecCones *c);
-/* shared with kernels/cones_spectral.cu (kernels/cones.cu): the sqrt2-scaled unpack of packed lower triangles, and
- * the DMMA contraction V diag(w) V' with weights max(w, 0) (mode 0, packed lower output; w ascending), signed weights
- * (mode 1, packed lower output) or its rectangular block (mode 2, dense rows x cols output from V of order
- * ld = rows + cols) */
-void b200_psd_info_or(int count, const int *d_info, int *d_err);
-void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_x, double *d_mats);
-void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off, const double *d_mats,
-                             const double *d_w, double *d_x, const double *d_s, const double *d_ry);
-/* Every launcher of the eigen-decomposition cones, and every batched eigensolver call, covers a group of one order in
- * sub-batches of at most B200_EIG_BATCH blocks, and the eigensolver workspace is sized for min(count, B200_EIG_BATCH).
- * The per-block kernels take the block index from gridDim.y or gridDim.z, which stop at 65535; and
- * cusolverDnXsyevBatched asks for about 0.5 MB of workspace per matrix whatever its order (measured on an H100 with
- * cuSOLVER 11.7.5: 35 GB for 65535 matrices of order 2), while cuSOLVER 11.7.3 (CUDA 12.8, the build PyTorch wheels
- * bundle) refuses the workspace query from 32767 matrices on (16384 pass). 4096 keeps the workspace near 2 GB. */
-#define B200_EIG_BATCH 4096
-/* cusolverDnXsyevBatched (eigenvectors, lower triangle) on count matrices of order n, sub-batch by sub-batch, then
- * the status words ORed into d_err; solver / params: cusolverDnHandle_t / cusolverDnParams_t. 0, or -1 with the error
- * recorded as `what`. */
-int b200_syevd_batched(void *solver, void *params, int n, double *d_mats, double *d_evals, void *d_work,
-                       size_t work_bytes, void *h_work, size_t h_work_bytes, int *d_info, int count, int *d_err,
-                       const char *what);
 void b200_cones_destroy(B200Cones *c);
 /* new box bounds (HOST arrays of bsize - 1, already scaled) and the box Newton warm start back to 1, as at creation */
 int b200_cones_set_box(B200Cones *c, const double *h_bl, const double *h_bu);

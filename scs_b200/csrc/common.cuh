@@ -132,6 +132,13 @@ __device__ __forceinline__ bool grid_finish(double (&mine)[NV], double *partials
   return true;
 }
 
+// ---------------------------------------------------------------- Moreau post-scaling (cones)
+// Every cone projection writes Pi(x) / r + s: the wrapper of reference cones.c:1583-1592, fused into its last pass.
+// ry NULL => x + s; sv NULL => the bare projection (cone-operator tests).
+__device__ __forceinline__ double moreau_post(double x, const double *ry, const double *sv, long long row) {
+  return sv == nullptr ? x : ry ? x / ry[row] + sv[row] : x + sv[row];
+}
+
 // ---------------------------------------------------------------- fp64 tensor core (SASS DMMA)
 // One m8n8k4 fp64 mma accumulated in place: {c0, c1} += A B over the warp, with this lane's A[g][t] in a, B[t][g]
 // in b and C[g][2t], C[g][2t+1] in c0, c1 (g = lane >> 2, t = lane & 3).

@@ -266,12 +266,6 @@ HD void project_pow(double &v0, double &v1, double &v2, double a) {
   v2 = (v2 < 0) ? -r : r;
 }
 
-__device__ __forceinline__ double finish(double xnew, const double *ry, const double *sv, long long row) {
-  // Moreau post-scaling of the wrapper (cones.c:1583-1592): x / r + s; sv NULL => bare projection
-  if (sv == nullptr) return xnew;
-  return (ry != nullptr) ? xnew / ry[row] + sv[row] : xnew + sv[row];
-}
-
 __global__ void k_exp_triples(int n_primal, int n_total, long long off, double *__restrict__ x,
                               const double *sv, const double *ry) {
   for (int i = blockIdx.x * blockDim.x + threadIdx.x; i < n_total; i += gridDim.x * blockDim.x) {
@@ -279,9 +273,9 @@ __global__ void k_exp_triples(int n_primal, int n_total, long long off, double *
     V3 v;
     v.r = x[b]; v.s = x[b + 1]; v.t = x[b + 2];
     project_exp(v, i < n_primal);
-    x[b] = finish(v.r, ry, sv, b);
-    x[b + 1] = finish(v.s, ry, sv, b + 1);
-    x[b + 2] = finish(v.t, ry, sv, b + 2);
+    x[b] = moreau_post(v.r, ry, sv, b);
+    x[b + 1] = moreau_post(v.s, ry, sv, b + 1);
+    x[b + 2] = moreau_post(v.t, ry, sv, b + 2);
   }
 }
 __global__ void k_pow_triples(int n, long long off, const double *__restrict__ pw, double *__restrict__ x,
@@ -298,9 +292,9 @@ __global__ void k_pow_triples(int n, long long off, const double *__restrict__ p
       project_pow(w0, w1, w2, -a);
       v0 += w0; v1 += w1; v2 += w2;
     }
-    x[b] = finish(v0, ry, sv, b);
-    x[b + 1] = finish(v1, ry, sv, b + 1);
-    x[b + 2] = finish(v2, ry, sv, b + 2);
+    x[b] = moreau_post(v0, ry, sv, b);
+    x[b + 1] = moreau_post(v1, ry, sv, b + 1);
+    x[b + 2] = moreau_post(v2, ry, sv, b + 2);
   }
 }
 

@@ -19,7 +19,7 @@
 //    shared-memory GEMM -> repack with the post-scaling fused.
 #include "../common.cuh"
 #include "../admm_api.h"
-#include <cusolverDn.h>
+#include "../eigen.cuh"
 #include <math.h>
 #include <stdio.h>
 #include <stdlib.h>
@@ -33,19 +33,6 @@
 #define SOC_BATCH_ROWS 4096
 #define BOX_MAX_ITERS 25
 #define CT 256
-
-struct PsdGroup {
-  int k;            // matrix order
-  int count;        // number of blocks
-  int *d_off;       // offset of each block inside the m-vector (count)
-  double *d_mats;   // count * k * k  (column-major, eigenvectors on exit)
-  double *d_evals;  // count * k
-  void *d_work;
-  size_t work_bytes;
-  void *h_work;
-  size_t h_work_bytes;
-  int *d_info;      // count
-};
 
 struct B200Cones {
   int m, nz, nl, bsize, qsize, ssize;
@@ -67,11 +54,9 @@ struct B200Cones {
   double *d_chunk_part;
   double *d_head_a0;
   // PSD
-  std::vector<PsdGroup> *groups;
+  std::vector<B200EigGroup> *groups;  // one per order k > 1
   int *d_psd1_off;  // offsets of the order-1 blocks
   int n_psd1;
-  cusolverDnHandle_t solver;
-  cusolverDnParams_t solver_params;
   double *d_scratch;  // m
   // three-dimensional cones (kernels/cone_triples.cu): ep primal exp, ed dual exp, psize power
   int n_ep, n_ed, n_pow;
@@ -80,9 +65,7 @@ struct B200Cones {
   B200CpsdCones *cpsd;  // complex PSD blocks (kernels/cones_complex.cu), or NULL
   B200SpecCones *spec;  // nuclear / l1 / sum-of-largest cones (kernels/cones_spectral.cu), or NULL
   long long spec_rows;  // rows of the spectral cones: the last rows of the m-vector
-  // sticky device flag: OR of every per-matrix `info` the batched eigen-solver has returned (reference
-  // cones.c:1048-1052 propagates a failed syevr as "error in project_cones"); read by b200_cones_check
-  int *d_err;
+  B200Eig eig;          // the eigensolver of the PSD, complex PSD and spectral groups
 };
 
 // OR the eigen-solver's per-matrix status words into the sticky flag (tiny; runs after every batched syevd)
@@ -92,7 +75,7 @@ __global__ void k_psd_info_or(int count, const int *__restrict__ info, int *err)
     if (info[b] != 0) bad = 1;
   if (bad) atomicOr(err, 1);
 }
-extern "C" void b200_psd_info_or(int count, const int *d_info, int *d_err) {
+static void psd_info_or(int count, const int *d_info, int *d_err) {
   if (!d_err || count <= 0) return;
   k_psd_info_or<<<(count + 255) / 256 > 64 ? 64 : (count + 255) / 256, 256, 0, (cudaStream_t)b200_stream()>>>(
       count, d_info, d_err);
@@ -114,12 +97,6 @@ __device__ __forceinline__ void soc_decide(double v1, double s, double &a0, doub
     scale = alpha / s;
   }
 }
-__device__ __forceinline__ double post_scale(double xnew, const double *ry, const double *sv,
-                                             long long row) {
-  // x / r + s  (or x + s when r is NULL); sv NULL => plain projection output
-  if (sv == nullptr) return xnew;
-  return (ry != nullptr) ? xnew / ry[row] + sv[row] : xnew + sv[row];
-}
 
 __global__ void __launch_bounds__(CT)
 k_soc_small(const int4 *__restrict__ items, const int *__restrict__ q_off, int soc_off,
@@ -131,7 +108,7 @@ k_soc_small(const int4 *__restrict__ items, const int *__restrict__ q_off, int s
     if (q <= 0) continue;
     const long long base = (long long)soc_off + off;
     if (q == 1) {
-      if (lane == 0) x[base] = post_scale(fmax(x[base], 0.0), ry, sv, base);
+      if (lane == 0) x[base] = moreau_post(fmax(x[base], 0.0), ry, sv, base);
       continue;
     }
     double acc = 0.0;
@@ -148,7 +125,7 @@ k_soc_small(const int4 *__restrict__ items, const int *__restrict__ q_off, int s
     for (int j = lane; j < q; j += 32) {
       const double xv = x[base + j];
       const double xn = (j == 0) ? a0 : (scale == 1.0 ? xv : (scale == 0.0 ? 0.0 : xv * scale));
-      x[base + j] = post_scale(xn, ry, sv, base + j);
+      x[base + j] = moreau_post(xn, ry, sv, base + j);
     }
   }
 }
@@ -195,7 +172,7 @@ k_soc_big_apply(const int4 *__restrict__ chunks, const int4 *__restrict__ big, i
   for (int j = threadIdx.x + (ch.w ? 1 : 0); j < ch.z; j += blockDim.x) {
     const double xv = x[base + j];
     const double xn = (scale == 1.0) ? xv : (scale == 0.0 ? 0.0 : xv * scale);
-    x[base + j] = post_scale(xn, ry, sv, base + j);
+    x[base + j] = moreau_post(xn, ry, sv, base + j);
   }
 }
 // element 0 of every big cone, written after all chunks have read it
@@ -205,7 +182,7 @@ __global__ void k_soc_big_heads(int n_big, const int4 *__restrict__ big, int soc
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= n_big) return;
   const long long row = (long long)soc_off + big[b].z;
-  x[row] = post_scale(head_a0[b], ry, sv, row);
+  x[row] = moreau_post(head_a0[b], ry, sv, row);
 }
 
 // ------------------------------------------------------------------ box kernels
@@ -261,7 +238,7 @@ __global__ void k_box_apply(int bsize, int box_off, double *__restrict__ x,
       if (xv > t * u) xn = t * u;
       else if (xv < t * l) xn = t * l;
     }
-    x[row] = post_scale(xn, ry, sv, row);
+    x[row] = moreau_post(xn, ry, sv, row);
   }
 }
 
@@ -367,32 +344,30 @@ k_reconstruct_dmma(int ld, int rows, int cols, int count, const int *__restrict_
         if (MODE == REC_RECT) {
           if (i < rows && j < cols) {
             const long long row = base + i + (long long)j * rows;
-            x[row] = post_scale(acc[a][c][q], ry, sv, row);
+            x[row] = moreau_post(acc[a][c][q], ry, sv, row);
           }
         } else if (i < rows && j < rows && i >= j) {
           const double val = (i == j) ? acc[a][c][q] * inv_sqrt2 : acc[a][c][q];
           const long long row = base + packed_idx(i, j, rows);
-          x[row] = post_scale(val, ry, sv, row);
+          x[row] = moreau_post(val, ry, sv, row);
         }
       }
 }
 // Launchers for kernels/cones_spectral.cu (count blocks; off[b] = first row of block b's matrix)
 // (blocks b0 .. b0 + nb - 1 of a sub-batch: offset pointers, the kernels index the sub-batch from 0)
 extern "C" void b200_psd_unpack_launch(int k, int count, const int *d_off, const double *d_x, double *d_mats) {
-  for (int b0 = 0; b0 < count; b0 += B200_EIG_BATCH) {
-    const int nb = std::min(B200_EIG_BATCH, count - b0);
+  eig_sub_batches(count, [&](int b0, int nb) {
     dim3 ug((k * k + 255) / 256, nb);
     k_psd_unpack<<<ug, 256, 0, (cudaStream_t)b200_stream()>>>(k, nb, d_off + b0, d_x, d_mats + (size_t)b0 * k * k);
     b200_count_launch(1);
-  }
+  });
 }
 extern "C" void b200_reconstruct_launch(int mode, int ld, int rows, int cols, int count, const int *d_off,
                                         const double *d_mats, const double *d_w, double *d_x, const double *d_s,
                                         const double *d_ry) {
   cudaStream_t st = (cudaStream_t)b200_stream();
   const int ntr = (rows + PT - 1) / PT, ntc = (cols + PT - 1) / PT;
-  for (int b0 = 0; b0 < count; b0 += B200_EIG_BATCH) {
-    const int nb = std::min(B200_EIG_BATCH, count - b0);
+  eig_sub_batches(count, [&](int b0, int nb) {
     const int *off = d_off + b0;
     const double *V = d_mats + (size_t)b0 * ld * ld, *w = d_w + (size_t)b0 * ld;
     dim3 rg(ntc, ntr, nb);
@@ -403,31 +378,14 @@ extern "C" void b200_reconstruct_launch(int mode, int ld, int rows, int cols, in
     else
       k_reconstruct_dmma<REC_SIGNED><<<rg, 128, 0, st>>>(ld, rows, cols, nb, off, V, w, d_x, d_s, d_ry);
     b200_count_launch(1);
-  }
-}
-extern "C" int b200_syevd_batched(void *solver, void *params, int n, double *d_mats, double *d_evals, void *d_work,
-                                  size_t work_bytes, void *h_work, size_t h_work_bytes, int *d_info, int count,
-                                  int *d_err, const char *what) {
-  for (int b0 = 0; b0 < count; b0 += B200_EIG_BATCH) {
-    const int nb = std::min(B200_EIG_BATCH, count - b0);
-    const cusolverStatus_t cs = cusolverDnXsyevBatched(
-        (cusolverDnHandle_t)solver, (cusolverDnParams_t)params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, n,
-        CUDA_R_64F, d_mats + (size_t)b0 * n * n, n, CUDA_R_64F, d_evals + (size_t)b0 * n, CUDA_R_64F, d_work,
-        work_bytes, h_work, h_work_bytes, d_info + b0, nb);
-    if (cs != CUSOLVER_STATUS_SUCCESS) {
-      b200_set_error(what, cudaErrorUnknown, __FILE__, __LINE__);
-      return -1;
-    }
-  }
-  b200_psd_info_or(count, d_info, d_err);
-  return 0;
+  });
 }
 __global__ void k_psd_order1(int count, const int *__restrict__ off, double *__restrict__ x,
                              const double *sv, const double *ry) {
   const int b = blockIdx.x * blockDim.x + threadIdx.x;
   if (b >= count) return;
   const long long row = off[b];
-  x[row] = post_scale(fmax(x[row], 0.0), ry, sv, row);
+  x[row] = moreau_post(fmax(x[row], 0.0), ry, sv, row);
 }
 
 // ------------------------------------------------------------------ Moreau wrapper kernels (operator API)
@@ -455,11 +413,12 @@ __global__ void k_moreau_pre(int m, int nz, int nl, double *__restrict__ x, doub
 
 // ------------------------------------------------------------------ host side
 // ---- cuSOLVER handle cache (per device, at most 4 parked): scs_init of a PSD problem no longer pays cusolverDnCreate
+// (a cuBLAS handle and workspace each)
 #include <mutex>
 static std::mutex g_solver_mu;
 static std::vector<std::pair<int, cusolverDnHandle_t>> g_solver_free;
 
-extern "C" void *b200_solver_acquire(void) {
+static cusolverDnHandle_t b200_solver_acquire(void) {
   int dev = 0;
   if (cudaGetDevice(&dev) != cudaSuccess) return nullptr;
   cusolverDnHandle_t h = nullptr;
@@ -477,20 +436,96 @@ extern "C" void *b200_solver_acquire(void) {
     cusolverDnDestroy(h);
     return nullptr;
   }
-  return (void *)h;
+  return h;
 }
 
-extern "C" void b200_solver_release(void *handle) {
+static void b200_solver_release(cusolverDnHandle_t handle) {
   if (!handle) return;
   int dev = 0;
   if (cudaGetDevice(&dev) == cudaSuccess) {
     std::lock_guard<std::mutex> lk(g_solver_mu);
     if (g_solver_free.size() < 4) {
-      g_solver_free.emplace_back(dev, (cusolverDnHandle_t)handle);
+      g_solver_free.emplace_back(dev, handle);
       return;
     }
   }
-  cusolverDnDestroy((cusolverDnHandle_t)handle);
+  cusolverDnDestroy(handle);
+}
+
+// ---- the eigensolver context (eigen.cuh)
+int eig_group_add(B200Eig *e, B200EigGroup &g, int N, const std::vector<int> &offs) {
+  if (!e->solver) {  // the first group of any family creates the context
+    e->solver = b200_solver_acquire();
+    if (!e->solver || cusolverDnCreateParams(&e->params) != CUSOLVER_STATUS_SUCCESS) return -1;
+    e->d_err = (int *)b200_malloc(64);
+    if (!e->d_err || b200_memset0(e->d_err, 64) != 0) return -1;
+  }
+  g.N = N;
+  g.count = (int)offs.size();
+  g.d_off = (int *)b200_malloc((size_t)g.count * 4);
+  g.d_mats = (double *)b200_malloc((size_t)g.count * N * N * 8);
+  g.d_evals = (double *)b200_malloc((size_t)g.count * N * 8);
+  if (!g.d_off || !g.d_mats || !g.d_evals || b200_h2d(g.d_off, offs.data(), (size_t)g.count * 4) != 0 ||
+      b200_sync() != 0)
+    return -1;
+  if (N == 1) return 0;  // order-1 log-det cones: the matrix is its own eigenvalue (kernels/cones_spectral.cu)
+  const int nb = std::min(g.count, B200_EIG_BATCH);
+  const cusolverStatus_t bs = cusolverDnXsyevBatched_bufferSize(
+      e->solver, e->params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, N, CUDA_R_64F, g.d_mats, N, CUDA_R_64F,
+      g.d_evals, CUDA_R_64F, &g.work_bytes, &g.h_work_bytes, nb);
+  if (bs != CUSOLVER_STATUS_SUCCESS) {
+    char what[112];
+    snprintf(what, sizeof(what), "cusolverDnXsyevBatched_bufferSize (order %d, %d blocks): status %d", N, nb, (int)bs);
+    b200_set_error(what, cudaErrorUnknown, __FILE__, __LINE__);
+    return -1;
+  }
+  if (!e->d_work || g.work_bytes > e->d_work_bytes) {
+    b200_free(e->d_work);
+    e->d_work_bytes = g.work_bytes;
+    e->d_work = b200_malloc(g.work_bytes);
+    if (!e->d_work) return -1;
+  }
+  if (g.h_work_bytes > e->h_work_bytes) {
+    free(e->h_work);
+    e->h_work_bytes = g.h_work_bytes;
+    e->h_work = malloc(g.h_work_bytes);
+    if (!e->h_work) return -1;
+  }
+  if (g.count > e->info_count) {
+    b200_free(e->d_info);
+    e->info_count = g.count;
+    e->d_info = (int *)b200_malloc((size_t)g.count * 4);
+    if (!e->d_info) return -1;
+  }
+  return 0;
+}
+
+void eig_group_free(B200EigGroup &g) {
+  b200_free(g.d_off); b200_free(g.d_mats); b200_free(g.d_evals);
+}
+
+void eig_destroy(B200Eig *e) {
+  b200_free(e->d_work); free(e->h_work); b200_free(e->d_info); b200_free(e->d_err);
+  if (e->params) cusolverDnDestroyParams(e->params);
+  b200_solver_release(e->solver);
+}
+
+int eig_syevd(B200Eig *e, const B200EigGroup &g, const char *what) {
+  const int n = g.N;
+  cusolverStatus_t cs = CUSOLVER_STATUS_SUCCESS;
+  eig_sub_batches(g.count, [&](int b0, int nb) {
+    if (cs == CUSOLVER_STATUS_SUCCESS)
+      cs = cusolverDnXsyevBatched(e->solver, e->params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, n,
+                                  CUDA_R_64F, g.d_mats + (size_t)b0 * n * n, n, CUDA_R_64F,
+                                  g.d_evals + (size_t)b0 * n, CUDA_R_64F, e->d_work, g.work_bytes,
+                                  g.h_work_bytes ? e->h_work : nullptr, g.h_work_bytes, e->d_info + b0, nb);
+  });
+  if (cs != CUSOLVER_STATUS_SUCCESS) {
+    b200_set_error(what, cudaErrorUnknown, __FILE__, __LINE__);
+    return -1;
+  }
+  psd_info_or(g.count, e->d_info, e->d_err);
+  return 0;
 }
 
 static int grid_for(long long n, int threads) {
@@ -513,7 +548,7 @@ extern "C" B200Cones *b200_cones_create(int m, int nz, int nl, int bsize, const 
   long long qtot = 0;
   for (int i = 0; i < qsize; ++i) qtot += h_q[i];
   c->psd_off = c->soc_off + (int)qtot;
-  c->groups = new std::vector<PsdGroup>();
+  c->groups = new std::vector<B200EigGroup>();
   int rc = 0;
   c->d_part = (double *)b200_malloc(8 * 2048 * 8);
   c->d_cnt = (unsigned int *)b200_malloc(64);
@@ -604,13 +639,6 @@ extern "C" B200Cones *b200_cones_create(int m, int nz, int nl, int bsize, const 
       if (k > 0) by_k[k].push_back((int)off);
       off += (long long)k * (k + 1) / 2;
     }
-    c->solver = (cusolverDnHandle_t)b200_solver_acquire();
-    if (!c->solver || cusolverDnCreateParams(&c->solver_params) != CUSOLVER_STATUS_SUCCESS) {
-      b200_cones_destroy(c);
-      return nullptr;
-    }
-    c->d_err = (int *)b200_malloc(64);
-    if (!c->d_err || b200_memset0(c->d_err, 64) != 0) { b200_cones_destroy(c); return nullptr; }
     for (auto &kv : by_k) {
       const int k = kv.first;
       const int count = (int)kv.second.size();
@@ -622,39 +650,8 @@ extern "C" B200Cones *b200_cones_create(int m, int nz, int nl, int bsize, const 
         rc |= b200_sync();
         continue;
       }
-      PsdGroup g;
-      memset(&g, 0, sizeof(g));
-      g.k = k; g.count = count;
-      g.d_off = (int *)b200_malloc((size_t)count * 4);
-      g.d_mats = (double *)b200_malloc((size_t)count * k * k * 8);
-      g.d_evals = (double *)b200_malloc((size_t)count * k * 8);
-      g.d_info = (int *)b200_malloc((size_t)count * 4);
-      auto drop_group = [&]() {
-        b200_free(g.d_off); b200_free(g.d_mats); b200_free(g.d_evals); b200_free(g.d_info);
-        b200_free(g.d_work); free(g.h_work);
-        b200_cones_destroy(c);
-      };
-      if (!g.d_off || !g.d_mats || !g.d_evals || !g.d_info) { drop_group(); return nullptr; }
-      rc |= b200_h2d(g.d_off, kv.second.data(), (size_t)count * 4);
-      rc |= b200_sync();
-      size_t wd = 0, wh = 0;
-      const cusolverStatus_t bs = cusolverDnXsyevBatched_bufferSize(
-          c->solver, c->solver_params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER, k, CUDA_R_64F, g.d_mats, k,
-          CUDA_R_64F, g.d_evals, CUDA_R_64F, &wd, &wh, std::min(count, B200_EIG_BATCH));
-      if (bs != CUSOLVER_STATUS_SUCCESS) {
-        char what[112];
-        snprintf(what, sizeof(what), "cusolverDnXsyevBatched_bufferSize (order %d, %d blocks): status %d", k,
-                 std::min(count, B200_EIG_BATCH), (int)bs);
-        b200_set_error(what, cudaErrorUnknown, __FILE__, __LINE__);
-        drop_group();
-        return nullptr;
-      }
-      g.work_bytes = wd;
-      g.h_work_bytes = wh;
-      g.d_work = b200_malloc(wd ? wd : 16);
-      g.h_work = wh ? malloc(wh) : nullptr;
-      if (!g.d_work || (wh && !g.h_work)) { drop_group(); return nullptr; }
-      c->groups->push_back(g);
+      c->groups->push_back(B200EigGroup());  // pushed first so that destroy releases what was allocated
+      if (eig_group_add(&c->eig, c->groups->back(), k, kv.second) != 0) { b200_cones_destroy(c); return nullptr; }
     }
   }
   if (rc != 0 || b200_sync() != 0) { b200_cones_destroy(c); return nullptr; }
@@ -682,18 +679,13 @@ extern "C" void b200_cones_destroy(B200Cones *c) {
   b200_free(c->d_big); b200_free(c->d_chunk_part); b200_free(c->d_head_a0); b200_free(c->d_psd1_off);
   b200_free(c->d_scratch);
   b200_free(c->d_pow);
-  b200_free(c->d_err);
   b200_cpsd_destroy(c->cpsd);
   b200_spec_destroy(c->spec);
   if (c->groups) {
-    for (auto &g : *c->groups) {
-      b200_free(g.d_off); b200_free(g.d_mats); b200_free(g.d_evals); b200_free(g.d_info);
-      b200_free(g.d_work); free(g.h_work);
-    }
+    for (auto &g : *c->groups) eig_group_free(g);
     delete c->groups;
   }
-  if (c->solver_params) cusolverDnDestroyParams(c->solver_params);
-  b200_solver_release((void *)c->solver);
+  eig_destroy(&c->eig);
   free(c);
 }
 
@@ -711,13 +703,9 @@ extern "C" int b200_cones_set_spectral(B200Cones *c, int dsize, const int *h_d, 
   for (int i = 0; i < sl_size; ++i) rows += 1 + (long long)h_sl_n[i] * (h_sl_n[i] + 1) / 2;
   if (rows == 0) return 0;
   if (rows > c->m) return -1;
-  if (!c->d_err) {
-    c->d_err = (int *)b200_malloc(64);
-    if (!c->d_err || b200_memset0(c->d_err, 64) != 0) return -1;
-  }
   c->spec_rows = rows;
   c->spec = b200_spec_create(dsize, h_d, nucsize, h_nuc_m, h_nuc_n, ell1_size, h_ell1, sl_size, h_sl_n, h_sl_k,
-                             (long long)c->m - rows, c->d_err);
+                             (long long)c->m - rows, &c->eig);
   return c->spec ? 0 : -1;
 }
 
@@ -747,12 +735,7 @@ extern "C" int b200_cones_set_complex_psd(B200Cones *c, int cssize, const int *h
   if (rows == 0) return 0;
   const long long first = (long long)c->m - c->spec_rows - 3LL * n_triples - rows;
   if (first < 0) return -1;
-  if (!c->d_err) {
-    c->d_err = (int *)b200_malloc(64);
-    if (!c->d_err || b200_memset0(c->d_err, 64) != 0) return -1;
-  }
-  c->cpsd = b200_cpsd_create(cssize, h_cs, first);
-  if (c->cpsd) b200_cpsd_set_err(c->cpsd, c->d_err);
+  c->cpsd = b200_cpsd_create(cssize, h_cs, first, &c->eig);
   return c->cpsd ? 0 : -1;
 }
 
@@ -795,11 +778,9 @@ extern "C" int b200_cones_project_rest(B200Cones *c, double *d_x, const double *
   }
   if (c->groups) {
     for (auto &g : *c->groups) {
-      const int k = g.k;
+      const int k = g.N;
       b200_psd_unpack_launch(k, g.count, g.d_off, d_x, g.d_mats);
-      if (b200_syevd_batched(c->solver, c->solver_params, k, g.d_mats, g.d_evals, g.d_work, g.work_bytes, g.h_work,
-                             g.h_work_bytes, g.d_info, g.count, c->d_err, "cusolverDnXsyevBatched") != 0)
-        return -1;
+      if (eig_syevd(&c->eig, g, "cusolverDnXsyevBatched") != 0) return -1;
       b200_reconstruct_launch(REC_PSD, k, k, k, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
     }
   }
@@ -818,9 +799,9 @@ extern "C" int b200_cones_project_rest(B200Cones *c, double *d_x, const double *
 
 // 0: every eigen-decomposition so far reported success; -1: at least one did not (sticky). Syncs the stream.
 extern "C" int b200_cones_check(B200Cones *c) {
-  if (!c || !c->d_err) return 0;
+  if (!c || !c->eig.d_err) return 0;
   int h = 0;
-  if (b200_d2h(&h, c->d_err, sizeof(int)) != 0 || b200_sync() != 0) return -1;
+  if (b200_d2h(&h, c->eig.d_err, sizeof(int)) != 0 || b200_sync() != 0) return -1;
   if (h & 2) {  // LD_ERR_BIT of kernels/cones_spectral.cu
     b200_set_error("log-det cone projection failed: Newton and both interior-point variants missed the tolerances",
                    cudaErrorUnknown, __FILE__, __LINE__);

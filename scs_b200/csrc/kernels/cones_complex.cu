@@ -18,31 +18,12 @@
 // and A+ (top-left) and B+ (bottom-left) are packed back with the Moreau post-scaling fused.
 #include "../common.cuh"
 #include "../admm_api.h"
-#include <cusolverDn.h>
-#include <algorithm>
+#include "../eigen.cuh"
 #include <map>
 #include <math.h>
-#include <stdlib.h>
-#include <string.h>
 #include <vector>
 
 namespace {
-
-struct CGroup {
-  int kc;      // complex order
-  int K;       // embedding order 2 kc
-  int count;   // blocks of this order
-  int *d_off;  // first row of each block in the m-vector
-  double *d_mats, *d_evals;
-  int *d_info;
-  void *d_work, *h_work;
-  size_t work_bytes, h_work_bytes;
-};
-
-__device__ __forceinline__ double finish(double xnew, const double *ry, const double *sv, long long row) {
-  if (sv == nullptr) return xnew;
-  return (ry != nullptr) ? xnew / ry[row] + sv[row] : xnew + sv[row];
-}
 
 // (re, im) of the sqrt(2)-scaled Hermitian matrix at (i, j), i >= j, from the packed block p
 __device__ __forceinline__ void packed_entry(const double *p, int kc, int i, int j, double &re, double &im) {
@@ -128,16 +109,16 @@ k_cpsd_reconstruct(int kc, int count, const int *__restrict__ off, const double 
     const long long col = base + (long long)J * (2 * kc - J);
     if (I < kc) {  // real part of H+(I, J)
       if (I == J) {
-        x[col] = finish(acc[r] * 0.7071067811865476, ry, sv, col);
+        x[col] = moreau_post(acc[r] * 0.7071067811865476, ry, sv, col);
       } else {
         const long long row = col + 1 + 2 * (I - J - 1);
-        x[row] = finish(acc[r], ry, sv, row);
+        x[row] = moreau_post(acc[r], ry, sv, row);
       }
     } else {  // imaginary part of H+(I - kc, J), strictly lower triangle only
       const int i = I - kc;
       if (i > J) {
         const long long row = col + 2 + 2 * (i - J - 1);
-        x[row] = finish(acc[r], ry, sv, row);
+        x[row] = moreau_post(acc[r], ry, sv, row);
       }
     }
   }
@@ -146,69 +127,31 @@ k_cpsd_reconstruct(int kc, int count, const int *__restrict__ off, const double 
 }  // namespace
 
 struct B200CpsdCones {
-  std::vector<CGroup> groups;
-  cusolverDnHandle_t solver;
-  cusolverDnParams_t params;
-  int *d_err;  // sticky "an eigen-decomposition failed" flag, owned by B200Cones (cones.cu)
+  std::vector<B200EigGroup> groups;  // one per complex order kc, of embedding order N = 2 kc
+  B200Eig *eig;                      // owned by B200Cones (kernels/cones.cu)
 };
-extern "C" void b200_cpsd_set_err(B200CpsdCones *c, int *d_err) { c->d_err = d_err; }
 
 extern "C" void b200_cpsd_destroy(B200CpsdCones *c) {
   if (!c) return;
   b200_sync();
-  for (auto &g : c->groups) {
-    b200_free(g.d_off); b200_free(g.d_mats); b200_free(g.d_evals); b200_free(g.d_info);
-    b200_free(g.d_work); free(g.h_work);
-  }
-  if (c->params) cusolverDnDestroyParams(c->params);
-  b200_solver_release((void *)c->solver);
+  for (auto &g : c->groups) eig_group_free(g);
   delete c;
 }
 
 // h_cs: complex PSD orders; first_row: row of the first complex block inside the m-vector
-extern "C" B200CpsdCones *b200_cpsd_create(int cssize, const int *h_cs, long long first_row) {
+extern "C" B200CpsdCones *b200_cpsd_create(int cssize, const int *h_cs, long long first_row, B200Eig *eig) {
   if (b200_runtime_init() != 0) return nullptr;
   B200CpsdCones *c = new B200CpsdCones();
-  c->solver = nullptr;
-  c->params = nullptr;
+  c->eig = eig;
   std::map<int, std::vector<int>> by_k;
   long long off = first_row;
   for (int i = 0; i < cssize; ++i) {
     if (h_cs[i] > 0) by_k[h_cs[i]].push_back((int)off);
     off += (long long)h_cs[i] * h_cs[i];
   }
-  if (by_k.empty()) return c;
-  c->solver = (cusolverDnHandle_t)b200_solver_acquire();
-  if (!c->solver || cusolverDnCreateParams(&c->params) != CUSOLVER_STATUS_SUCCESS) {
-    b200_cpsd_destroy(c);
-    return nullptr;
-  }
   for (auto &kv : by_k) {
-    CGroup g;
-    memset(&g, 0, sizeof(g));
-    g.kc = kv.first;
-    g.K = 2 * kv.first;
-    g.count = (int)kv.second.size();
-    g.d_off = (int *)b200_malloc((size_t)g.count * 4);
-    g.d_mats = (double *)b200_malloc((size_t)g.count * g.K * g.K * 8);
-    g.d_evals = (double *)b200_malloc((size_t)g.count * g.K * 8);
-    g.d_info = (int *)b200_malloc((size_t)g.count * 4);
-    bool ok = g.d_off && g.d_mats && g.d_evals && g.d_info &&
-              b200_h2d(g.d_off, kv.second.data(), (size_t)g.count * 4) == 0 && b200_sync() == 0;
-    size_t wd = 0, wh = 0;
-    ok = ok && cusolverDnXsyevBatched_bufferSize(c->solver, c->params, CUSOLVER_EIG_MODE_VECTOR,
-                                                 CUBLAS_FILL_MODE_LOWER, g.K, CUDA_R_64F, g.d_mats, g.K,
-                                                 CUDA_R_64F, g.d_evals, CUDA_R_64F, &wd, &wh,
-                                                 std::min(g.count, B200_EIG_BATCH)) == CUSOLVER_STATUS_SUCCESS;
-    if (ok) {
-      g.work_bytes = wd;
-      g.h_work_bytes = wh;
-      g.d_work = b200_malloc(wd ? wd : 16);
-      g.h_work = wh ? malloc(wh) : nullptr;
-      ok = g.d_work != nullptr && (wh == 0 || g.h_work != nullptr);
-    }
-    c->groups.push_back(g);  // pushed before the check so that destroy releases what was allocated
-    if (!ok) {
+    c->groups.push_back(B200EigGroup());  // pushed first so that destroy releases what was allocated
+    if (eig_group_add(eig, c->groups.back(), 2 * kv.first, kv.second) != 0) {
       b200_cpsd_destroy(c);
       return nullptr;
     }
@@ -220,25 +163,21 @@ extern "C" B200CpsdCones *b200_cpsd_create(int cssize, const int *h_cs, long lon
 extern "C" int b200_cpsd_project(B200CpsdCones *c, double *d_x, const double *d_s, const double *d_ry) {
   cudaStream_t st = (cudaStream_t)b200_stream();
   for (auto &g : c->groups) {
-    const size_t KK = (size_t)g.K * g.K;
-    for (int b0 = 0; b0 < g.count; b0 += B200_EIG_BATCH) {
-      const int nb = std::min(B200_EIG_BATCH, g.count - b0);
-      dim3 ug((g.K * g.K + 255) / 256, nb);
-      k_cpsd_unpack<<<ug, 256, 0, st>>>(g.kc, nb, g.d_off + b0, d_x, g.d_mats + b0 * KK);
+    const int K = g.N, kc = K / 2;
+    const size_t KK = (size_t)K * K;
+    eig_sub_batches(g.count, [&](int b0, int nb) {
+      dim3 ug((K * K + 255) / 256, nb);
+      k_cpsd_unpack<<<ug, 256, 0, st>>>(kc, nb, g.d_off + b0, d_x, g.d_mats + b0 * KK);
       b200_count_launch(1);
-    }
-    if (b200_syevd_batched(c->solver, c->params, g.K, g.d_mats, g.d_evals, g.d_work, g.work_bytes, g.h_work,
-                           g.h_work_bytes, g.d_info, g.count, c->d_err,
-                           "cusolverDnXsyevBatched (complex PSD embedding)") != 0)
-      return -1;
-    const int nt = (g.K + CPT - 1) / CPT;
-    for (int b0 = 0; b0 < g.count; b0 += B200_EIG_BATCH) {
-      const int nb = std::min(B200_EIG_BATCH, g.count - b0);
+    });
+    if (eig_syevd(c->eig, g, "cusolverDnXsyevBatched (complex PSD embedding)") != 0) return -1;
+    const int nt = (K + CPT - 1) / CPT;
+    eig_sub_batches(g.count, [&](int b0, int nb) {
       dim3 rg(nt, nt, nb);
-      k_cpsd_reconstruct<<<rg, CPT * 8, 0, st>>>(g.kc, nb, g.d_off + b0, g.d_mats + b0 * KK,
-                                                 g.d_evals + (size_t)b0 * g.K, d_x, d_s, d_ry);
+      k_cpsd_reconstruct<<<rg, CPT * 8, 0, st>>>(kc, nb, g.d_off + b0, g.d_mats + b0 * KK,
+                                                 g.d_evals + (size_t)b0 * K, d_x, d_s, d_ry);
       b200_count_launch(1);
-    }
+    });
   }
   CUDA_OK(cudaGetLastError());
   return 0;

@@ -32,10 +32,9 @@
 // kernels/cones.cu (b200_cones_check).
 #include "../common.cuh"
 #include "../admm_api.h"
-#include <cusolverDn.h>
+#include "../eigen.cuh"
 #include <math.h>
 #include <stdlib.h>
-#include <string.h>
 #include <algorithm>
 #include <map>
 #include <utility>
@@ -49,11 +48,6 @@
 #define TOL_LARGEST_CONE 1e-9  // reference sum_largest_cone.c:9
 
 namespace {
-
-__device__ __forceinline__ double finish(double xnew, const double *ry, const double *sv, long long row) {
-  if (sv == nullptr) return xnew;
-  return (ry != nullptr) ? xnew / ry[row] + sv[row] : xnew + sv[row];
-}
 
 // Threshold of the l1-norm cone projection of (t0, v), returned in every thread of the CTA:
 //   Pi(t0, v) = (t0 + mu, sign(v) max(|v| - mu, 0)),   mu >= 0 the root of  sum_i max(|v_i| - mu, 0) = t0 + mu.
@@ -123,13 +117,13 @@ __global__ void k_ell1_cones(const int *__restrict__ off, const int *__restrict_
   if (n <= ELL1_INLINE) {
     for (int i = threadIdx.x; i < n; i += blockDim.x) {
       const long long row = base + 1 + i;
-      x[row] = finish(ell1_apply(x[row], mu, diff), ry, sv, row);
+      x[row] = moreau_post(ell1_apply(x[row], mu, diff), ry, sv, row);
     }
   } else if (threadIdx.x == 0) {
     par[2 * b] = mu;
     par[2 * b + 1] = diff;
   }
-  if (threadIdx.x == 0) x[base] = finish(tn, ry, sv, base);
+  if (threadIdx.x == 0) x[base] = moreau_post(tn, ry, sv, base);
 }
 
 // chunks of the big l1 cones: (index into par, first row, rows, -)
@@ -139,7 +133,7 @@ __global__ void k_ell1_chunks(const int4 *__restrict__ chunks, const double *__r
   const double mu = par[2 * ch.x], diff = par[2 * ch.x + 1];
   for (int i = threadIdx.x; i < ch.z; i += blockDim.x) {
     const long long row = (long long)ch.y + i;
-    x[row] = finish(ell1_apply(x[row], mu, diff), ry, sv, row);
+    x[row] = moreau_post(ell1_apply(x[row], mu, diff), ry, sv, row);
   }
 }
 
@@ -182,7 +176,7 @@ __global__ void k_nuc_vector(int m, int n, int count, const int *__restrict__ of
     }
     lam[c] = wgt;
   }
-  if (threadIdx.x == 0) x[trow] = finish(tn, ry, sv, trow);
+  if (threadIdx.x == 0) x[trow] = moreau_post(tn, ry, sv, trow);
 }
 
 // sum-of-largest cone, vector step: one thread per cone, the reference's sorted algorithm
@@ -221,7 +215,7 @@ __global__ void k_sl_vector(int n, int count, const int *__restrict__ off, const
   nt -= 1;
   for (int i = 0; i < nu; ++i) X(i) -= eta;
   for (int i = nu; i < nu + nt; ++i) X(i) = a_t;
-  x[trow] = finish(t * (1.0 / sqrt2), ry, sv, trow);
+  x[trow] = moreau_post(t * (1.0 / sqrt2), ry, sv, trow);
 }
 
 // ---------------------------------------------------------------------------------------------- log-det cone
@@ -940,8 +934,8 @@ __global__ void __launch_bounds__(LD_T) k_logdet_vector(int n, const int *__rest
   if (lane == 0) {
     warm[cone] = wflag;
     const double inv = 1.0 / sqrt2;
-    x[trow] = finish(inv * u[0], ry, sv, trow);
-    x[trow + 1] = finish(inv * u[1], ry, sv, trow + 1);
+    x[trow] = moreau_post(inv * u[0], ry, sv, trow);
+    x[trow + 1] = moreau_post(inv * u[1], ry, sv, trow + 1);
     if (status != 0) atomicOr(err, LD_ERR_BIT);
     if (cone == last) {
       stats->iter = st.iter;
@@ -961,25 +955,18 @@ __global__ void k_logdet_order1(int count, double *__restrict__ mats, double *__
   mats[b] = 1.0;
 }
 
-// one batch of equally shaped matrices for cusolverDnXsyevBatched
-struct EigGroup {
-  int m, n;    // nuclear: X is m x n (order m + n); sum-of-largest: order n (m = 0)
-  int N;       // order of the decomposed matrices
-  int count;
-  int *d_off;  // first row of each block's matrix (the row after t)
-  int *d_k;    // sum-of-largest: k of each cone; log-det: the cone's index among the log-det cones
+// the eigensolver group of one family and shape (d_off: the row after t), with the family's own arrays
+struct SpecGroup : B200EigGroup {
+  int m, n;  // nuclear: X is m x n (N = m + n); log-det, sum-of-largest: order n = N (m = 0)
+  int *d_k;  // sum-of-largest: k of each cone; log-det: the cone's index among the log-det cones
   long long *d_poff;  // log-det: offset of each cone's saved projection in B200SpecCones::d_ld_proj
   double *d_scratch;  // log-det: LD_VECS n doubles per cone
-  double *d_mats, *d_evals;
-  int *d_info;
-  void *d_work, *h_work;
-  size_t work_bytes, h_work_bytes;
 };
 
 }  // namespace
 
 struct B200SpecCones {
-  std::vector<EigGroup> ld, nuc, sl;
+  std::vector<SpecGroup> ld, nuc, sl;
   // log-det state, kept across projections and solves like the reference's ScsConeWork: the warm-start flag of each
   // cone, its previous projection (2 + d doubles, at offsets 2 i + sum_{j<i} d_j) and the stats of the last cone
   int ld_count;
@@ -991,55 +978,20 @@ struct B200SpecCones {
   int *d_ell1_off, *d_ell1_len;  // small cones first, then big ones
   double *d_par;                 // 2 per big cone
   int4 *d_chunks;
-  cusolverDnHandle_t solver;
-  cusolverDnParams_t params;
-  int *d_err;  // owned by B200Cones
+  B200Eig *eig;  // owned by B200Cones (kernels/cones.cu)
 };
-
-static void free_group(EigGroup &g) {
-  b200_free(g.d_off); b200_free(g.d_k); b200_free(g.d_poff); b200_free(g.d_scratch); b200_free(g.d_mats); b200_free(g.d_evals); b200_free(g.d_info);
-  b200_free(g.d_work); free(g.h_work);
-}
 
 extern "C" void b200_spec_destroy(B200SpecCones *c) {
   if (!c) return;
   b200_sync();
-  for (auto &g : c->ld) free_group(g);
-  for (auto &g : c->nuc) free_group(g);
-  for (auto &g : c->sl) free_group(g);
+  for (auto *family : {&c->ld, &c->nuc, &c->sl})
+    for (auto &g : *family) {
+      eig_group_free(g);
+      b200_free(g.d_k); b200_free(g.d_poff); b200_free(g.d_scratch);
+    }
   b200_free(c->d_ld_warm); b200_free(c->d_ld_proj); b200_free(c->d_ld_stats);
   b200_free(c->d_ell1_off); b200_free(c->d_ell1_len); b200_free(c->d_par); b200_free(c->d_chunks);
-  if (c->params) cusolverDnDestroyParams(c->params);
-  b200_solver_release((void *)c->solver);
   delete c;
-}
-
-// offsets / ks: host arrays of the group; allocates the eigensolver batch of order g.N
-static bool init_group(B200SpecCones *c, EigGroup &g, const std::vector<int> &offs, const std::vector<int> *ks) {
-  g.count = (int)offs.size();
-  g.d_off = (int *)b200_malloc((size_t)g.count * 4);
-  g.d_mats = (double *)b200_malloc((size_t)g.count * g.N * g.N * 8);
-  g.d_evals = (double *)b200_malloc((size_t)g.count * g.N * 8);
-  g.d_info = (int *)b200_malloc((size_t)g.count * 4);
-  bool ok = g.d_off && g.d_mats && g.d_evals && g.d_info && b200_h2d(g.d_off, offs.data(), offs.size() * 4) == 0;
-  if (ok && ks) {
-    g.d_k = (int *)b200_malloc((size_t)g.count * 4);
-    ok = g.d_k && b200_h2d(g.d_k, ks->data(), ks->size() * 4) == 0;
-  }
-  ok = ok && b200_sync() == 0;
-  if (g.N == 1) return ok;  // order-1 log-det cones need no eigensolver (k_logdet_order1)
-  size_t wd = 0, wh = 0;
-  ok = ok && cusolverDnXsyevBatched_bufferSize(c->solver, c->params, CUSOLVER_EIG_MODE_VECTOR, CUBLAS_FILL_MODE_LOWER,
-                                               g.N, CUDA_R_64F, g.d_mats, g.N, CUDA_R_64F, g.d_evals, CUDA_R_64F,
-                                               &wd, &wh, std::min(g.count, B200_EIG_BATCH)) == CUSOLVER_STATUS_SUCCESS;
-  if (ok) {
-    g.work_bytes = wd;
-    g.h_work_bytes = wh;
-    g.d_work = b200_malloc(wd ? wd : 16);
-    g.h_work = wh ? malloc(wh) : nullptr;
-    ok = g.d_work != nullptr && (wh == 0 || g.h_work != nullptr);
-  }
-  return ok;
 }
 
 // zeroes the log-det warm starts, saved projections and stats: the state of a fresh b200_spec_create
@@ -1063,10 +1015,10 @@ extern "C" int b200_spec_logdet_stats(B200SpecCones *c, int *iter, int *newton_s
 
 extern "C" B200SpecCones *b200_spec_create(int dsize, const int *h_d, int nucsize, const int *h_nuc_m,
                                            const int *h_nuc_n, int ell1_size, const int *h_ell1, int sl_size,
-                                           const int *h_sl_n, const int *h_sl_k, long long first_row, int *d_err) {
+                                           const int *h_sl_n, const int *h_sl_k, long long first_row, B200Eig *eig) {
   if (b200_runtime_init() != 0) return nullptr;
   B200SpecCones *c = new B200SpecCones();  // value-initialised: counts and pointers start at 0
-  c->d_err = d_err;
+  c->eig = eig;
   long long row = first_row;
   // log-det cones come first (reference cones.c:1449): (t, v, X), 2 + d(d+1)/2 rows; grouped by order
   struct LdCones { std::vector<int> off, idx; std::vector<long long> poff; };
@@ -1140,52 +1092,41 @@ extern "C" B200SpecCones *b200_spec_create(int dsize, const int *h_d, int nucsiz
       return nullptr;
     }
   }
-  // ---- eigensolver batches
-  if (!ld_by.empty() || !nuc_by.empty() || !sl_by.empty()) {
-    c->solver = (cusolverDnHandle_t)b200_solver_acquire();
-    if (!c->solver || cusolverDnCreateParams(&c->params) != CUSOLVER_STATUS_SUCCESS) {
+  // ---- eigensolver groups, each pushed before its allocations so that destroy releases them
+  auto upload_ints = [](int *&d, const std::vector<int> &h) {
+    d = (int *)b200_malloc(h.size() * 4);
+    return d && b200_h2d(d, h.data(), h.size() * 4) == 0;
+  };
+  for (auto &kv : ld_by) {
+    c->ld.push_back(SpecGroup());
+    SpecGroup &g = c->ld.back();
+    g.n = kv.first;
+    bool ok = eig_group_add(eig, g, g.n, kv.second.off) == 0 && upload_ints(g.d_k, kv.second.idx);
+    if (ok) {
+      g.d_poff = (long long *)b200_malloc((size_t)g.count * 8);
+      g.d_scratch = (double *)b200_malloc((size_t)g.count * (LD_VECS * g.n + LD_KEEP) * 8);
+      ok = g.d_poff && g.d_scratch && b200_h2d(g.d_poff, kv.second.poff.data(), (size_t)g.count * 8) == 0;
+    }
+    if (!ok || b200_sync() != 0) { b200_spec_destroy(c); return nullptr; }
+  }
+  for (auto &kv : nuc_by) {
+    c->nuc.push_back(SpecGroup());
+    SpecGroup &g = c->nuc.back();
+    g.m = kv.first.first;
+    g.n = kv.first.second;
+    if (eig_group_add(eig, g, g.m + g.n, kv.second) != 0) { b200_spec_destroy(c); return nullptr; }
+  }
+  for (auto &kv : sl_by) {
+    c->sl.push_back(SpecGroup());
+    SpecGroup &g = c->sl.back();
+    g.n = kv.first;
+    if (eig_group_add(eig, g, g.n, kv.second.first) != 0 || !upload_ints(g.d_k, kv.second.second) ||
+        b200_sync() != 0) {
       b200_spec_destroy(c);
       return nullptr;
     }
   }
-  for (auto &kv : ld_by) {
-    EigGroup g;
-    memset(&g, 0, sizeof(g));
-    g.n = g.N = kv.first;
-    bool ok = init_group(c, g, kv.second.off, &kv.second.idx);
-    if (ok) {
-      g.d_poff = (long long *)b200_malloc((size_t)g.count * 8);
-      g.d_scratch = (double *)b200_malloc((size_t)g.count * (LD_VECS * g.n + LD_KEEP) * 8);
-      ok = g.d_poff && g.d_scratch && b200_h2d(g.d_poff, kv.second.poff.data(), (size_t)g.count * 8) == 0 &&
-           b200_sync() == 0;
-    }
-    c->ld.push_back(g);
-    if (!ok) { b200_spec_destroy(c); return nullptr; }
-  }
-  for (auto &kv : nuc_by) {
-    EigGroup g;
-    memset(&g, 0, sizeof(g));
-    g.m = kv.first.first;
-    g.n = kv.first.second;
-    g.N = g.m + g.n;
-    const bool ok = init_group(c, g, kv.second, nullptr);
-    c->nuc.push_back(g);  // pushed before the check so that destroy releases what was allocated
-    if (!ok) { b200_spec_destroy(c); return nullptr; }
-  }
-  for (auto &kv : sl_by) {
-    EigGroup g;
-    memset(&g, 0, sizeof(g));
-    g.n = g.N = kv.first;
-    const bool ok = init_group(c, g, kv.second.first, &kv.second.second);
-    c->sl.push_back(g);
-    if (!ok) { b200_spec_destroy(c); return nullptr; }
-  }
   return c;
-}
-
-static int syevd(B200SpecCones *c, EigGroup &g, const char *what) {
-  return b200_syevd_batched(c->solver, c->params, g.N, g.d_mats, g.d_evals, g.d_work, g.work_bytes, g.h_work,
-                            g.h_work_bytes, g.d_info, g.count, c->d_err, what);
 }
 
 extern "C" int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_s, const double *d_ry) {
@@ -1197,24 +1138,23 @@ extern "C" int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_
     if (g.N == 1) {
       k_logdet_order1<<<(g.count + 127) / 128, 128, 0, st>>>(g.count, g.d_mats, g.d_evals);
       b200_count_launch(1);
-    } else if (syevd(c, g, "cusolverDnXsyevBatched (log-det cone)") != 0) {
+    } else if (eig_syevd(c->eig, g, "cusolverDnXsyevBatched (log-det cone)") != 0) {
       return -1;
     }
     k_logdet_vector<<<g.count, LD_T, 0, st>>>(g.n, g.d_off, g.d_k, g.d_poff, g.d_evals, d_x, d_s, d_ry,
                                               c->d_ld_proj, c->d_ld_warm, g.d_scratch, c->ld_count - 1,
-                                              c->d_ld_stats, c->d_err);
+                                              c->d_ld_stats, c->eig->d_err);
     b200_count_launch(1);
     b200_reconstruct_launch(0, g.n, g.n, g.n, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
   }
   // ---- nuclear-norm cones
   for (auto &g : c->nuc) {
-    for (int b0 = 0; b0 < g.count; b0 += B200_EIG_BATCH) {
-      const int nb = std::min(B200_EIG_BATCH, g.count - b0);
+    eig_sub_batches(g.count, [&](int b0, int nb) {
       dim3 eg((g.N * g.N + 255) / 256, nb);
       k_nuc_embed<<<eg, 256, 0, st>>>(g.m, g.n, nb, g.d_off + b0, d_x, g.d_mats + (size_t)b0 * g.N * g.N);
       b200_count_launch(1);
-    }
-    if (syevd(c, g, "cusolverDnXsyevBatched (nuclear-norm cone embedding)") != 0) return -1;
+    });
+    if (eig_syevd(c->eig, g, "cusolverDnXsyevBatched (nuclear-norm cone embedding)") != 0) return -1;
     k_nuc_vector<<<g.count, NUC_T, 0, st>>>(g.m, g.n, g.count, g.d_off, g.d_evals, d_x, d_s, d_ry);
     b200_count_launch(1);
     b200_reconstruct_launch(2, g.N, g.m, g.n, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);
@@ -1233,7 +1173,7 @@ extern "C" int b200_spec_project(B200SpecCones *c, double *d_x, const double *d_
   // ---- sum-of-largest-eigenvalues cones
   for (auto &g : c->sl) {
     b200_psd_unpack_launch(g.n, g.count, g.d_off, d_x, g.d_mats);
-    if (syevd(c, g, "cusolverDnXsyevBatched (sum-of-largest-eigenvalues cone)") != 0) return -1;
+    if (eig_syevd(c->eig, g, "cusolverDnXsyevBatched (sum-of-largest-eigenvalues cone)") != 0) return -1;
     k_sl_vector<<<(g.count + 127) / 128, 128, 0, st>>>(g.n, g.count, g.d_off, g.d_k, g.d_evals, d_x, d_s, d_ry);
     b200_count_launch(1);
     b200_reconstruct_launch(1, g.n, g.n, g.n, g.count, g.d_off, g.d_mats, g.d_evals, d_x, d_s, d_ry);

@@ -31,7 +31,7 @@ from scs_b200 import capi
 pytestmark = pytest.mark.gpu
 SQRT2 = np.sqrt(2.0)
 GRID_YZ = 65535  # largest gridDim.y / gridDim.z
-SUB_BATCH = 4096  # B200_EIG_BATCH (scs_b200/csrc/admm_api.h)
+SUB_BATCH = 4096  # B200_EIG_BATCH (scs_b200/csrc/eigen.cuh)
 
 
 @pytest.fixture(scope="module")
