@@ -37,11 +37,15 @@
  * fallback: every entry point fails (NULL / nonzero / SCS_FAILED) when no CUDA
  * device is usable.
  *
- * Threading: one process drives ONE GPU (SCS_B200_DEVICE / LOCAL_RANK) through ONE stream.  Entry points may be
- * called from any host thread (each binds the calling thread to the library's device; the pinned staging buffer of
- * pageable copies is mutex-protected), but work of different workspaces is ordered by that single stream and the
- * kernel-launch sequence of a solve is not re-entrant: run one scs_solve / scs_solve_lin_sys at a time per
- * process (the reference is re-entrant per ScsWork; this library is re-entrant per process).
+ * Threading: one process drives ONE GPU (SCS_B200_DEVICE / LOCAL_RANK).  Like the reference, the library is
+ * re-entrant per workspace: two threads may call scs_solve (or any other entry point) on two different workspaces at
+ * the same time.  Every workspace -- ScsWork, a ScsLinSysWork made by scs_init_lin_sys_work, ScsB200ConeWork,
+ * ScsB200AaWork -- owns an execution context (a CUDA stream of its own, its timers and its cached device blocks),
+ * and every entry point binds it to the calling thread for the length of the call; each solve returns the same bits
+ * as when run alone, also when the threads use different library flavours (int, DLONG, spectral): they share the
+ * one libscs_b200_token.so of the process.  One workspace must not be used by two threads at once.  Processes with several ranks
+ * (scs_b200_comm_init, nranks > 1) keep one solve at a time per process: their CG kernels wait on flags that peers
+ * set and need the whole GPU.
  */
 #ifndef SCS_B200_H
 #define SCS_B200_H
@@ -267,7 +271,7 @@ AaStats scs_b200_aa_get_stats(const ScsB200AaWork *a);
 typedef struct {
   long long cg_iters;        /* total CG iterations */
   long long lin_sys_solves;  /* scs_solve_lin_sys calls */
-  long long kernel_launches; /* kernels of this library launched */
+  long long kernel_launches; /* kernels this workspace's solve launched */
   double spmv_ms;            /* reserved */
   scs_int n_gpus;
 } ScsB200Stats;
@@ -305,13 +309,18 @@ scs_int scs_b200_write_data(const char *filename, const ScsData *d, const ScsCon
 scs_int scs_b200_read_data(const char *filename, ScsData **d, ScsCone **k, ScsSettings **stgs);
 void scs_b200_free_data(ScsData *d, ScsCone *k, ScsSettings *stgs);
 
-/* Number of kernels this library has launched in this process. */
+/* The KKT solves of the last scs_solve on this workspace that ran the CG loop's fused K3 + K4 kernel (out[0]) and
+ * that ran its two-kernel pair (out[1]); both compute the same bits. A fused kernel of more than one block runs
+ * only while no other solve of the process runs one (DESIGN.md, "Concurrent solves"). 0, or -1 for NULL input. */
+scs_int scs_b200_cg_k34_paths(const ScsWork *w, long long out[2]);
+/* Number of kernels this library has launched in this process, over all threads. */
 long long scs_b200_launch_count(void);
 /* 1 if a CUDA device of compute capability 10.x is usable, else 0. */
 scs_int scs_b200_device_ok(void);
 /* Device memory is cached across workspaces (a freed block is handed to the next allocation of the same size instead of
  * going back to the driver: cudaMalloc / cudaFree cost milliseconds each and cudaFree synchronises the device). This
- * returns every cached block to the driver; SCS_B200_POOL=0 disables the caching altogether. */
+ * returns every cached block to the driver, also those a live workspace has cached (it waits for that workspace's
+ * stream first); SCS_B200_POOL=0 disables the caching altogether. */
 void scs_b200_release_memory(void);
 
 #ifdef __cplusplus

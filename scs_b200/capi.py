@@ -399,6 +399,8 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_transfer_stats.restype = None
     lib.scs_b200_transfer_stats.argtypes = [C.POINTER(C.c_longlong)]
     lib.scs_b200_transfer_stats_reset.restype = None
+    lib.scs_b200_cg_k34_paths.restype = I
+    lib.scs_b200_cg_k34_paths.argtypes = [C.c_void_p, C.POINTER(C.c_longlong)]
     lib.scs_b200_launch_count.restype = C.c_longlong
     lib.scs_b200_device_ok.restype = I
     lib.scs_b200_release_memory.restype = None

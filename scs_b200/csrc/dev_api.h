@@ -26,8 +26,19 @@ int b200_d2h(void *dst, const void *d_src, size_t bytes);  /* async on stream */
 int b200_d2d(void *d_dst, const void *d_src, size_t bytes);
 int b200_memset0(void *d_dst, size_t bytes);
 int b200_sync(void);
-long long b200_launches(void);
-/* CUDA-event timing on the library stream */
+long long b200_launches(void);         /* process-wide */
+/* Execution contexts (kernels/runtime.cu): a stream of its own, the timer and join events, the section timers, a
+ * launch counter and the free lists of the blocks freed under it. Every call below acts on the context bound to the
+ * calling thread, or on the process context when none is. A workspace owns a context (or shares its parent's) and
+ * every entry point brackets its work with enter / leave. */
+typedef struct B200Ctx B200Ctx;
+B200Ctx *b200_ctx_create(void);        /* a parked context or a new one; NULL on failure */
+void b200_ctx_release(B200Ctx *c);     /* syncs its stream, gives its free lists to the shared pool, parks it */
+B200Ctx *b200_ctx_enter(B200Ctx *c);   /* binds c (NULL: the process context) to the thread; returns the previous */
+void b200_ctx_leave(B200Ctx *prev);    /* restores what b200_ctx_enter returned */
+B200Ctx *b200_ctx_bound(void);         /* the context bound to the thread, NULL if none */
+long long b200_ctx_launches(void);     /* kernels launched under the current context */
+/* CUDA-event timing on the current context's stream */
 int b200_timer_start(void);
 double b200_timer_stop_ms(void);       /* syncs; <0 on error */
 /* device-side section timers (ScsInfo.lin_sys_time / cone_time / accel_time): CUDA events on the library
@@ -222,6 +233,7 @@ typedef struct {
   B200P2pRoute *d_p2p_route; /* device copy of the push-routing table (sharded-x mode); d_p then lives in the
                                 peer-mapped exchange allocation */
   int k34_fused;       /* 1: K3 and K4 run as one kernel (k_cg_update_p); set by b200_cg_plan_k34 */
+  long long k34_solves[2]; /* KKT solves run with the fused kernel / with the pair k_cg_update + k_cg_pupdate */
 } B200Cg;
 
 /* M_j = 1 / (R_x,j + P_jj + sum_k A_kj^2 / R_y,k)   (private.c:50-82) */
@@ -229,7 +241,12 @@ int b200_cg_set_preconditioner(const B200Cg *cg, const double *d_Pdiag);
 /* after b200_cg_set_preconditioner, with the reordered pair and d_perm (its rows) in place: fills d_diag_tab and
  * d_ry_mask and sets ry_form / rx_form (one 4-byte read-back) */
 int b200_cg_classify_diag(B200Cg *cg, const int *d_perm);
-/* single GPU: sets k34_fused when n <= 2 SMs * 4096 and the fused kernel's grid is co-resident on the device */
+/* single GPU: sets k34_fused when n <= 2 SMs * 4096 and the fused kernel's grid is co-resident on the device. A solve
+ * whose fused grid has more than one block runs it only while it holds the process-wide token (kernels/cg.cu) */
+/* that token (token/k34_token.c, libscs_b200_token.so: one per process whatever flavours are loaded): take returns 1
+ * when the caller now holds it, 0 when another solve does, and never waits */
+int b200_k34_token_take(void);
+void b200_k34_token_give_back(void);
 int b200_cg_plan_k34(B200Cg *cg);
 /* Full device solve of [[R_x+P, A'],[A, -R_y]] [x;y] = b in place on d_b (n+m),
  * warm start d_s (n) or NULL; returns CG iterations (>=0) or <0 on error.

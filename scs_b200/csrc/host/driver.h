@@ -88,8 +88,10 @@ struct SCS_WORK {
   /* AA */
   double aa_norm;
   int rejected_accel_steps, accepted_accel_steps;
-  /* stats of the last solve */
-  long long stat_cg_iters, stat_solves, stat_launches;
+  /* stats of the last solve; stat_k34: its KKT solves with the fused K3 + K4 kernel and with the pair */
+  long long stat_cg_iters, stat_solves, stat_launches, stat_k34[2];
+  /* the execution context (stream, events, timers, free lists) every entry point binds; shared by p, cones, accel */
+  B200Ctx *ctx;
   /* per-iteration CSV trace (ScsSettings.log_csv_filename, reference src/rw.c:707-861): debugging mode, the
    * iterates are copied to the host every iteration and every column is recomputed there */
   char *log_csv_name; /* deep copy of ScsSettings.log_csv_filename */

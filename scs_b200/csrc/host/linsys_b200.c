@@ -12,6 +12,7 @@
  * plus device-pointer variants (b200_linsys_*_dev) used by the device-resident
  * ADMM driver (host/scs_driver.c) so that the hot loop never crosses PCIe.
  */
+#include "driver.h" /* ScsWork, for scs_b200_cg_k34_paths */
 #include "linsys_b200.h"
 #include <pthread.h>
 #include <stdio.h>
@@ -309,8 +310,7 @@ static int cg_ops_refresh(ScsLinSysWork *w) {
 
 static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_mark_p);
 
-ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
-                                     const scs_float *diag_r) {
+static ScsLinSysWork *init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P, const scs_float *diag_r) {
   ScsLinSysWork *w;
   double t_mark = wall_ms();
   int *Lp = NULL, *Li = NULL;
@@ -329,6 +329,7 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
   }
   w = (ScsLinSysWork *)calloc(1, sizeof(ScsLinSysWork));
   if (!w) return SCS_NULL;
+  w->ctx = b200_ctx_bound();
   w->n = n; w->m = m;
   w->nnz = A->p[n];
   w->nranks = b200_comm_nranks();
@@ -384,6 +385,25 @@ fail:
   return SCS_NULL;
 }
 
+/* Inside scs_init the workspace shares the ScsWork's execution context; called as a plugin it gets one of its own, so
+ * that linear-system workspaces of different threads solve on different streams. */
+ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
+                                     const scs_float *diag_r) {
+  B200Ctx *own = SCS_NULL, *prev = SCS_NULL;
+  ScsLinSysWork *w;
+  if (!b200_ctx_bound()) {
+    own = b200_ctx_create();
+    prev = b200_ctx_enter(own);
+  }
+  w = init_lin_sys_work(A, P, diag_r);
+  if (w) w->own_ctx = own != SCS_NULL;
+  if (own) {
+    b200_ctx_leave(prev);
+    if (!w) b200_ctx_release(own);
+  }
+  return w;
+}
+
 /* single GPU, from operators built on the device (the device-data entry points, host/scs_driver.c): the workspace takes
  * A, At, P and d_Pdiag over, also when it fails */
 ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B200Spmv *P, double *d_Pdiag,
@@ -394,6 +414,7 @@ ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B20
     b200_spmv_destroy(A); b200_spmv_destroy(At); b200_spmv_destroy(P); b200_free(d_Pdiag);
     return SCS_NULL;
   }
+  w->ctx = b200_ctx_bound();
   w->n = n; w->m = m;
   w->nnz = b200_spmv_nnz(At);
   w->nranks = 1;
@@ -482,8 +503,7 @@ static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_m
   return 0;
 }
 
-void scs_free_lin_sys_work(ScsLinSysWork *w) {
-  if (!w) return;
+static void free_lin_sys_work(ScsLinSysWork *w) {
   b200_sync();
   b200_spmv_destroy(w->At_cg); /* a view of At: before At itself */
   b200_spmv_destroy(w->A_cg);
@@ -516,6 +536,15 @@ void scs_free_lin_sys_work(ScsLinSysWork *w) {
   b200_host_free(w->cg.h_ctl);
   free(w->offsets);
   free(w);
+}
+void scs_free_lin_sys_work(ScsLinSysWork *w) {
+  B200Ctx *prev, *own;
+  if (!w) return;
+  own = w->own_ctx ? w->ctx : SCS_NULL;
+  prev = b200_ctx_enter(w->ctx);
+  free_lin_sys_work(w);
+  b200_ctx_leave(prev);
+  b200_ctx_release(own);
 }
 
 /* Row-sharded setup: D, E of the FULL matrix are computed on every rank from temporary full
@@ -561,7 +590,7 @@ int b200_linsys_update_diag_r_dev(ScsLinSysWork *w, const double *d_diag_r) {
   return cg_ops_refresh(w); /* the operators may have been rescaled in place; R_y has changed */
 }
 
-scs_int scs_solve_lin_sys(ScsLinSysWork *w, scs_float *b, const scs_float *s, scs_float tol) {
+static scs_int solve_lin_sys(ScsLinSysWork *w, scs_float *b, const scs_float *s, scs_float tol) {
   const size_t nm = (size_t)w->n + w->m;
   if (tol <= 0.) {
     fprintf(stderr, "Warning: tol = %4f <= 0, likely compiled without setting INDIRECT flag.\n",
@@ -574,11 +603,23 @@ scs_int scs_solve_lin_sys(ScsLinSysWork *w, scs_float *b, const scs_float *s, sc
   if (b200_sync() != 0) return -1;
   return 0;
 }
+scs_int scs_solve_lin_sys(ScsLinSysWork *w, scs_float *b, const scs_float *s, scs_float tol) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const scs_int rc = solve_lin_sys(w, b, s, tol);
+  b200_ctx_leave(prev);
+  return rc;
+}
 
-scs_int scs_update_lin_sys_diag_r(ScsLinSysWork *w, const scs_float *new_diag_r) {
+static scs_int update_lin_sys_diag_r(ScsLinSysWork *w, const scs_float *new_diag_r) {
   if (b200_h2d(w->d_diag_r, new_diag_r, ((size_t)w->n + w->m) * 8) != 0) return -1;
   if (b200_linsys_update_diag_r_dev(w, w->d_diag_r) != 0) return -1;
   return b200_sync() == 0 ? 0 : -1;
+}
+scs_int scs_update_lin_sys_diag_r(ScsLinSysWork *w, const scs_float *new_diag_r) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const scs_int rc = update_lin_sys_diag_r(w, new_diag_r);
+  b200_ctx_leave(prev);
+  return rc;
 }
 
 scs_int scs_b200_linsys_last_cg_its(const ScsLinSysWork *w) { return w->last_cg_its; }
@@ -592,13 +633,23 @@ scs_int scs_b200_g_reuse(void) {
   return !(e && strcmp(e, "0") == 0);
 }
 
+/* the CG path counts of the last scs_solve (host/scs_driver.c fills them); here rather than in the driver for the same
+ * reason as scs_b200_g_reuse */
+scs_int scs_b200_cg_k34_paths(const ScsWork *w, long long out[2]) {
+  if (!w || !out) return -1;
+  out[0] = w->stat_k34[0];
+  out[1] = w->stat_k34[1];
+  return 0;
+}
+
 static scs_int accum_generic(ScsLinSysWork *w, const B200Spmv *M, int ncols, int nrows,
                              const scs_float *x, scs_float *y, scs_int accumulate) {
   B200SpmvArgs a;
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
   double *d_x = (double *)b200_malloc((size_t)ncols * 8);
   double *d_y = (double *)b200_malloc((size_t)nrows * 8);
   int rc = -1;
-  if (w->nranks > 1) { b200_free(d_x); b200_free(d_y); return -1; } /* operator-level API is single-GPU */
+  if (w->nranks > 1) goto out; /* operator-level API is single-GPU */
   if (!d_x || !d_y) goto out;
   if (b200_h2d(d_x, x, (size_t)ncols * 8) != 0) goto out;
   if (accumulate && b200_h2d(d_y, y, (size_t)nrows * 8) != 0) goto out;
@@ -612,6 +663,7 @@ static scs_int accum_generic(ScsLinSysWork *w, const B200Spmv *M, int ncols, int
 out:
   b200_free(d_x);
   b200_free(d_y);
+  b200_ctx_leave(prev);
   return rc;
 }
 
@@ -627,7 +679,10 @@ scs_int scs_b200_accum_by_atrans(ScsLinSysWork *w, const scs_float *x, scs_float
 /* --- device timing helpers for bench.py (inputs resident in HBM) --------- */
 double scs_b200_time_spmv(ScsLinSysWork *w, scs_int op, scs_int reps, double *alg_bytes) {
   double ms[2] = {-1.0, -1.0};
-  if (b200_spmv_time_pair(w->A, w->At, reps, ms) != 0) return -1.0;
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const int rc = b200_spmv_time_pair(w->A, w->At, reps, ms);
+  b200_ctx_leave(prev);
+  if (rc != 0) return -1.0;
   if (alg_bytes) *alg_bytes = b200_spmv_alg_bytes(op == 0 ? w->A : w->At, 0);
   return ms[op == 0 ? 0 : 1];
 }
@@ -636,8 +691,8 @@ double scs_b200_time_spmv(ScsLinSysWork *w, scs_int op, scs_int reps, double *al
  * a genuine start on the right-hand side b, which the caller provides: length n + m, host). out_ms[0..4] = ms
  * per launch of K1, K2, K3, K4 and of the whole iteration; out_bytes[0..4] = the algorithmic bytes of each
  * (b200_cg_iter_alg_bytes, DESIGN.md section 3). */
-scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms,
-                                 double *out_bytes) {
+static scs_int time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms,
+                               double *out_bytes) {
   const size_t nm = (size_t)w->n + w->m;
   int k;
   if (w->P) return -1;
@@ -652,8 +707,15 @@ scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int r
   if (out_bytes) out_bytes[4] = b200_cg_iter_alg_bytes(&w->cg, out_bytes);
   return 0;
 }
+scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms,
+                                 double *out_bytes) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const scs_int rc = time_cg_kernels(w, b, reps, out_ms, out_bytes);
+  b200_ctx_leave(prev);
+  return rc;
+}
 
-double scs_b200_time_cg_iter(ScsLinSysWork *w, scs_int reps, double *alg_bytes) {
+static double time_cg_iter(ScsLinSysWork *w, scs_int reps, double *alg_bytes) {
   /* run `reps` genuine CG iterations on a synthetic rhs with the stop test
    * disabled (tol = 0 never satisfies ||r|| < tol) and time them on the stream */
   const size_t nm = (size_t)w->n + w->m;
@@ -678,5 +740,11 @@ double scs_b200_time_cg_iter(ScsLinSysWork *w, scs_int reps, double *alg_bytes) 
   if (alg_bytes) *alg_bytes = b200_cg_iter_alg_bytes(&w->cg, NULL);
 out:
   free(hb);
+  return ms;
+}
+double scs_b200_time_cg_iter(ScsLinSysWork *w, scs_int reps, double *alg_bytes) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const double ms = time_cg_iter(w, reps, alg_bytes);
+  b200_ctx_leave(prev);
   return ms;
 }

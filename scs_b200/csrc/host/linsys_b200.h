@@ -34,6 +34,9 @@ struct SCS_LIN_SYS_WORK {
   int last_admm_its, last_g_its;
   long long tot_cg_its;
   long long n_solves;
+  /* the execution context: the parent ScsWork's when created inside scs_init (own_ctx = 0), else its own */
+  B200Ctx *ctx;
+  int own_ctx;
 };
 
 /* device-pointer variants used by the ADMM driver */

@@ -2,7 +2,8 @@
  * the parity tests and bench.py to compare one operator at a time against the
  * reference: the cone projection (reference src/cones.c:1498-1596) and Anderson
  * acceleration (reference src/aa.c:657-979). Each call stages the host arrays
- * through device memory and runs the same kernels the ADMM driver uses. */
+ * through device memory and runs the same kernels the ADMM driver uses. Each
+ * workspace has an execution context of its own (dev_api.h), bound by every call. */
 #include "driver.h"
 #include <math.h>
 #include <stdio.h>
@@ -13,9 +14,17 @@ struct SCS_B200_CONE_WORK {
   int m;
   B200Cones *cones;
   double *d_x, *d_ry;
+  B200Ctx *ctx;
 };
 
-ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float *D) {
+static void cone_free(ScsB200ConeWork *c) {
+  b200_cones_destroy(c->cones);
+  b200_free(c->d_x);
+  b200_free(c->d_ry);
+  free(c);
+}
+
+static ScsB200ConeWork *init_cone(const ScsCone *k, scs_int m, const scs_float *D) {
   ScsB200ConeWork *c;
   double *bl = SCS_NULL, *bu = SCS_NULL;
   scs_int j;
@@ -51,6 +60,7 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float
   }
   c = (ScsB200ConeWork *)calloc(1, sizeof(*c));
   if (!c) return SCS_NULL;
+  c->ctx = b200_ctx_bound();
   c->m = (int)m;
   if (k->bsize > 1) {
     /* box bounds follow the row scaling (reference normalize_box_cone, cones.c:1160-1177);
@@ -94,11 +104,19 @@ fail_ints:
 fail:
   free(bl);
   free(bu);
-  scs_b200_finish_cone(c);
+  cone_free(c);
   return SCS_NULL;
 }
 
-scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x, const scs_float *r_y) {
+ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m, const scs_float *D) {
+  B200Ctx *ctx = b200_ctx_create(), *prev = b200_ctx_enter(ctx);
+  ScsB200ConeWork *c = init_cone(k, m, D); /* a failed init has freed its blocks under ctx */
+  b200_ctx_leave(prev);
+  if (!c) b200_ctx_release(ctx);
+  return c;
+}
+
+static scs_int proj_dual_cone(ScsB200ConeWork *c, scs_float *x, const scs_float *r_y) {
   const size_t bytes = (size_t)c->m * 8;
   if (b200_h2d(c->d_x, x, bytes) != 0) return -1;
   if (r_y && b200_h2d(c->d_ry, r_y, bytes) != 0) return -1;
@@ -107,22 +125,35 @@ scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x, const scs_floa
   if (b200_sync() != 0) return -1;
   return b200_cones_check(c->cones); /* a failed eigen-decomposition is an error, like cones.c:1048-1052 */
 }
+scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x, const scs_float *r_y) {
+  B200Ctx *prev = b200_ctx_enter(c->ctx);
+  const scs_int rc = proj_dual_cone(c, x, r_y);
+  b200_ctx_leave(prev);
+  return rc;
+}
 
 scs_int scs_b200_cone_logdet_stats(ScsB200ConeWork *c, scs_int *iter, scs_int *newton_success,
                                    scs_float *residuals) {
-  int it = 0, success = 0;
-  if (!c || b200_cones_logdet_stats(c->cones, &it, &success, residuals) != 0) return -1;
+  int it = 0, success = 0, rc;
+  B200Ctx *prev;
+  if (!c) return -1;
+  prev = b200_ctx_enter(c->ctx);
+  rc = b200_cones_logdet_stats(c->cones, &it, &success, residuals);
+  b200_ctx_leave(prev);
+  if (rc != 0) return -1;
   *iter = it;
   *newton_success = success;
   return 0;
 }
 
 void scs_b200_finish_cone(ScsB200ConeWork *c) {
+  B200Ctx *ctx, *prev;
   if (!c) return;
-  b200_cones_destroy(c->cones);
-  b200_free(c->d_x);
-  b200_free(c->d_ry);
-  free(c);
+  ctx = c->ctx;
+  prev = b200_ctx_enter(ctx);
+  cone_free(c);
+  b200_ctx_leave(prev);
+  b200_ctx_release(ctx);
 }
 
 /* ------------------------------------------------------------------ AA */
@@ -130,15 +161,24 @@ struct SCS_B200_AA_WORK {
   int dim;
   B200Aa *a;
   double *d_f, *d_x;
+  B200Ctx *ctx;
 };
 
 static int over_int(long long v) { return v > 2147483647LL; }
+
+static void aa_free(ScsB200AaWork *w) {
+  b200_aa_destroy(w->a);
+  b200_free(w->d_f);
+  b200_free(w->d_x);
+  free(w);
+}
 
 ScsB200AaWork *scs_b200_aa_init(scs_int dim, scs_int mem, scs_int min_len, scs_int type1,
                                 scs_float regularization, scs_float relaxation,
                                 scs_float safeguard_factor, scs_float max_weight_norm,
                                 scs_int ir_max_steps, scs_int verbosity) {
   ScsB200AaWork *w;
+  B200Ctx *prev;
   /* the vector length and the memory are int inside; larger 64-bit values are refused, not truncated */
   if (over_int(dim) || b200_over_dim("mem", -1, mem) || b200_over_dim("min_len", -1, min_len) ||
       b200_over_dim("ir_max_steps", -1, ir_max_steps))
@@ -146,17 +186,27 @@ ScsB200AaWork *scs_b200_aa_init(scs_int dim, scs_int mem, scs_int min_len, scs_i
   w = (ScsB200AaWork *)calloc(1, sizeof(*w));
   if (!w) return SCS_NULL;
   w->dim = (int)dim;
+  w->ctx = b200_ctx_create();
+  prev = b200_ctx_enter(w->ctx);
   w->a = b200_aa_create((int)dim, (int)mem, (int)min_len, type1 != 0, regularization, relaxation, safeguard_factor,
                         max_weight_norm, (int)ir_max_steps,
                         verbosity > 2 ? 2 : verbosity < 0 ? 0 : (int)verbosity); /* levels 0, 1, 2 */
-  if (!w->a) { free(w); return SCS_NULL; }
-  w->d_f = (double *)b200_malloc((size_t)dim * 8);
-  w->d_x = (double *)b200_malloc((size_t)dim * 8);
-  if (!w->d_f || !w->d_x) { scs_b200_aa_finish(w); return SCS_NULL; }
+  if (w->a) {
+    w->d_f = (double *)b200_malloc((size_t)dim * 8);
+    w->d_x = (double *)b200_malloc((size_t)dim * 8);
+  }
+  if (!w->a || !w->d_f || !w->d_x) {
+    B200Ctx *ctx = w->ctx;
+    aa_free(w);
+    b200_ctx_leave(prev);
+    b200_ctx_release(ctx);
+    return SCS_NULL;
+  }
+  b200_ctx_leave(prev);
   return w;
 }
 
-scs_float scs_b200_aa_apply(ScsB200AaWork *w, scs_float *f, const scs_float *x) {
+static scs_float aa_apply(ScsB200AaWork *w, scs_float *f, const scs_float *x) {
   const size_t bytes = (size_t)w->dim * 8;
   double nrm;
   if (b200_h2d(w->d_f, f, bytes) != 0 || b200_h2d(w->d_x, x, bytes) != 0) return NAN;
@@ -164,8 +214,14 @@ scs_float scs_b200_aa_apply(ScsB200AaWork *w, scs_float *f, const scs_float *x) 
   if (b200_d2h(f, w->d_f, bytes) != 0 || b200_sync() != 0) return NAN;
   return nrm;
 }
+scs_float scs_b200_aa_apply(ScsB200AaWork *w, scs_float *f, const scs_float *x) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const scs_float nrm = aa_apply(w, f, x);
+  b200_ctx_leave(prev);
+  return nrm;
+}
 
-scs_int scs_b200_aa_safeguard(ScsB200AaWork *w, scs_float *f_new, scs_float *x_new) {
+static scs_int aa_safeguard(ScsB200AaWork *w, scs_float *f_new, scs_float *x_new) {
   const size_t bytes = (size_t)w->dim * 8;
   int rc;
   if (b200_h2d(w->d_f, f_new, bytes) != 0 || b200_h2d(w->d_x, x_new, bytes) != 0) return 0;
@@ -177,15 +233,27 @@ scs_int scs_b200_aa_safeguard(ScsB200AaWork *w, scs_float *f_new, scs_float *x_n
   }
   return rc;
 }
+scs_int scs_b200_aa_safeguard(ScsB200AaWork *w, scs_float *f_new, scs_float *x_new) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const scs_int rc = aa_safeguard(w, f_new, x_new);
+  b200_ctx_leave(prev);
+  return rc;
+}
 
-void scs_b200_aa_reset(ScsB200AaWork *w) { b200_aa_reset_dev(w->a); }
+void scs_b200_aa_reset(ScsB200AaWork *w) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  b200_aa_reset_dev(w->a);
+  b200_ctx_leave(prev);
+}
 
 void scs_b200_aa_finish(ScsB200AaWork *w) {
+  B200Ctx *ctx, *prev;
   if (!w) return;
-  b200_aa_destroy(w->a);
-  b200_free(w->d_f);
-  b200_free(w->d_x);
-  free(w);
+  ctx = w->ctx;
+  prev = b200_ctx_enter(ctx);
+  aa_free(w);
+  b200_ctx_leave(prev);
+  b200_ctx_release(ctx);
 }
 
 AaStats scs_b200_aa_get_stats(const ScsB200AaWork *w) {

@@ -391,9 +391,8 @@ static void init_mark(const char *what, double *t_last) {
   }
 }
 
-void scs_finish(ScsWork *w) {
+static void finish_work(ScsWork *w) {
   double t_mark = now_ms();
-  if (!w) return;
   b200_sync();
   init_mark("finish: stream drained", &t_mark);
   if (w->log_csv_fout) fclose(w->log_csv_fout);
@@ -431,6 +430,15 @@ void scs_finish(ScsWork *w) {
   free(w->stgs);
   free(w);
   init_mark("finish: host copies", &t_mark);
+}
+void scs_finish(ScsWork *w) {
+  B200Ctx *ctx, *prev;
+  if (!w) return;
+  ctx = w->ctx;
+  prev = b200_ctx_enter(ctx);
+  finish_work(w);
+  b200_ctx_leave(prev);
+  b200_ctx_release(ctx); /* its stream has drained: the blocks freed under it join the shared pool */
 }
 
 static void set_diag_r_host(ScsWork *w) {
@@ -477,7 +485,7 @@ static void normalize_box_cone(ScsCone *k, const double *D, int bsize) {
   }
 }
 
-scs_int scs_update(ScsWork *w, scs_float *b, scs_float *c) {
+static scs_int update_work_bc(ScsWork *w, scs_float *b, scs_float *c) {
   const double t0 = now_ms();
   const int n = w->n, m = w->m;
   int i;
@@ -510,6 +518,12 @@ scs_int scs_update(ScsWork *w, scs_float *b, scs_float *c) {
   w->setup_time = now_ms() - t0;
   return 0;
 }
+scs_int scs_update(ScsWork *w, scs_float *b, scs_float *c) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const scs_int rc = update_work_bc(w, b, c);
+  b200_ctx_leave(prev);
+  return rc;
+}
 
 static void print_header(const ScsWork *w) {
   const ScsCone *k = w->k;
@@ -540,7 +554,8 @@ static void write_data_dev(const char *filename, const ScsData *d, const ScsCone
  * the data in host memory, validated there. On one GPU (dm != NULL) the operators are built on the device from dm's
  * blocks (build_ops_dev), which scs_init fills from the host A and P. Several GPUs (dm == NULL, scs_init only) cut A
  * into row blocks on the host (scs_init_lin_sys_work). */
-static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm, int dev_data) {
+static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm, int dev_data,
+                          B200Ctx *ctx) {
   ScsWork *w;
   const double t0 = now_ms();
   double t_mark = t0;
@@ -559,6 +574,10 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
     printf("ERROR: scs_b200 needs an sm_90 (H100) CUDA device: %s\n", b200_last_error());
     return SCS_NULL;
   }
+  if (!ctx) {
+    printf("ERROR: could not create the workspace's stream: %s\n", b200_last_error());
+    return SCS_NULL;
+  }
   if (stgs->write_data_filename) { /* reference scs.c:1270-1273 */
     printf("Writing raw problem data to %s\n", stgs->write_data_filename);
     if (dev_data) write_data_dev(stgs->write_data_filename, d, k, stgs);
@@ -566,6 +585,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   }
   w = (ScsWork *)calloc(1, sizeof(ScsWork));
   if (!w) return SCS_NULL;
+  w->ctx = ctx;
   n = w->n = d->n;
   m = w->m = d->m;
   l = (size_t)n + m + 1;
@@ -737,7 +757,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   } else {
     memcpy(w->b_orig, d->b, (size_t)m * 8);
     memcpy(w->c_orig, d->c, (size_t)n * 8);
-    if (scs_update(w, w->b_orig, w->c_orig) != 0) goto fail;
+    if (update_work_bc(w, w->b_orig, w->c_orig) != 0) goto fail;
   }
 
   /* the kernel layer takes int copies of the cone arrays (validated below 2^30) */
@@ -775,19 +795,24 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   return w;
 fail:
   printf("ERROR: scs_init failed (%s)\n", b200_last_error());
-  scs_finish(w);
+  finish_work(w); /* the caller releases ctx */
   return SCS_NULL;
 }
 
+/* Every workspace gets an execution context of its own (a parked one when a finished workspace left one): its stream,
+ * events, timers and free lists, so that workspaces of different threads solve concurrently. */
 ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   DevMats dm;
   ScsWork *w;
+  B200Ctx *ctx = d && k && stgs ? b200_ctx_create() : SCS_NULL, *prev = b200_ctx_enter(ctx);
   memset(&dm, 0, sizeof(dm));
-  w = init_work(d, k, stgs, b200_comm_nranks() > 1 ? SCS_NULL : &dm, 0);
+  w = init_work(d, k, stgs, b200_comm_nranks() > 1 ? SCS_NULL : &dm, 0, ctx);
   if (dm.Ap) { /* uploaded (a refused input never reaches the GPU): free only once the builder's kernels have run */
     b200_sync();
     dev_mats_free(&dm);
   }
+  b200_ctx_leave(prev);
+  if (!w) b200_ctx_release(ctx);
   return w;
 }
 
@@ -1310,11 +1335,11 @@ static int log_data_to_csv(ScsWork *w, int iter, double t_solve) {
 }
 
 /* ----------------------------------------------------------------- the solve */
-scs_int scs_solve(ScsWork *w, ScsSolution *sol, ScsInfo *info, scs_int warm_start) {
+static scs_int solve(ScsWork *w, ScsSolution *sol, ScsInfo *info, scs_int warm_start) {
   int i, l;
   double t_solve, total_accel = 0.0, total_cone = 0.0, total_lin = 0.0;
-  const long long launches0 = b200_launches();
-  long long cg0, solves0;
+  const long long launches0 = b200_ctx_launches();
+  long long cg0, solves0, k34_0[2];
   ScsSettings *stgs;
   if (!sol || !w || !info) {
     printf("ERROR: missing ScsWork, ScsSolution or ScsInfo input\n");
@@ -1334,6 +1359,8 @@ scs_int scs_solve(ScsWork *w, ScsSolution *sol, ScsInfo *info, scs_int warm_star
   info->status_val = SCS_UNFINISHED;
   cg0 = w->p->tot_cg_its;
   solves0 = w->p->n_solves;
+  k34_0[0] = w->p->cg.k34_solves[0];
+  k34_0[1] = w->p->cg.k34_solves[1];
   if (update_work(w, sol) != 0)
     return failure(w, w->m, w->n, sol, info, SCS_FAILED, "error in update_work", "failure");
   if (stgs->verbose) {
@@ -1439,7 +1466,9 @@ scs_int scs_solve(ScsWork *w, ScsSolution *sol, ScsInfo *info, scs_int warm_star
   info->accel_time = total_accel;
   w->stat_cg_iters = w->p->tot_cg_its - cg0;
   w->stat_solves = w->p->n_solves - solves0;
-  w->stat_launches = b200_launches() - launches0;
+  w->stat_launches = b200_ctx_launches() - launches0;
+  w->stat_k34[0] = w->p->cg.k34_solves[0] - k34_0[0];
+  w->stat_k34[1] = w->p->cg.k34_solves[1] - k34_0[1];
   if (w->log_csv_fout) { /* scs.c:1481 */
     fclose(w->log_csv_fout);
     w->log_csv_fout = SCS_NULL;
@@ -1460,6 +1489,12 @@ scs_int scs_solve(ScsWork *w, ScsSolution *sol, ScsInfo *info, scs_int warm_star
     printf("\n");
   }
   return info->status_val;
+}
+scs_int scs_solve(ScsWork *w, ScsSolution *sol, ScsInfo *info, scs_int warm_start) {
+  B200Ctx *prev = b200_ctx_enter(w ? w->ctx : SCS_NULL);
+  const scs_int status = solve(w, sol, info, warm_start);
+  b200_ctx_leave(prev);
+  return status;
 }
 
 scs_int scs(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, ScsSolution *sol,
@@ -1611,7 +1646,7 @@ static int single_gpu(void) {
   return 0;
 }
 
-ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, void *stream) {
+static ScsWork *init_device(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, void *stream, B200Ctx *ctx) {
   DevMats dm;
   ScsWork *w;
   memset(&dm, 0, sizeof(dm));
@@ -1632,15 +1667,22 @@ ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSetti
     printf("ERROR: Validation returned failure\n");
     return SCS_NULL;
   }
-  if (b200_wait_for_caller(stream) != 0) return SCS_NULL;
-  w = init_work(d, k, stgs, &dm, 1);
+  if (!ctx || b200_wait_for_caller(stream) != 0) return SCS_NULL;
+  w = init_work(d, k, stgs, &dm, 1, ctx);
   b200_sync(); /* the builder's blocks are free only once its kernels have run */
   dev_mats_free(&dm);
   b200_caller_waits(stream);
   return w;
 }
+ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, void *stream) {
+  B200Ctx *ctx = d && k && stgs ? b200_ctx_create() : SCS_NULL, *prev = b200_ctx_enter(ctx);
+  ScsWork *w = init_device(d, k, stgs, stream, ctx);
+  b200_ctx_leave(prev);
+  if (!w) b200_ctx_release(ctx);
+  return w;
+}
 
-scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream) {
+static scs_int update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream) {
   const int n = w ? w->n : 0, m = w ? w->m : 0;
   int rc = -1;
   if (!w || !single_gpu() || (d_b && !dev_ptr_ok(d_b, "b")) || (d_c && !dev_ptr_ok(d_c, "c"))) return -1;
@@ -1662,6 +1704,12 @@ scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float
   b200_caller_waits(stream);
   return rc;
 }
+scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream) {
+  B200Ctx *prev = b200_ctx_enter(w ? w->ctx : SCS_NULL);
+  const scs_int rc = update_device(w, d_b, d_c, stream);
+  b200_ctx_leave(prev);
+  return rc;
+}
 
 /* New values of A (and P) on the pattern the workspace was built with (DESIGN.md section 1, "Matrix update"): the
  * validating copy of init, the builder's transpose, a pattern check of every entry against the resident streams (one
@@ -1670,7 +1718,7 @@ scs_int scs_b200_update_device(ScsWork *w, const scs_float *d_b, const scs_float
 static void pattern_differs(const char *which) {
   printf("ERROR: the pattern of %s differs from the one the workspace was built with\n", which);
 }
-scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMatrix *P, void *stream) {
+static scs_int update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMatrix *P, void *stream) {
   const double t0 = now_ms();
   double t_mark = t0;
   const int n = w ? w->n : 0, m = w ? w->m : 0;
@@ -1800,8 +1848,14 @@ scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsM
   b200_caller_waits(stream);
   return rc;
 }
+scs_int scs_b200_update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMatrix *P, void *stream) {
+  B200Ctx *prev = b200_ctx_enter(w ? w->ctx : SCS_NULL);
+  const scs_int rc = update_matrix_device(w, A, P, stream);
+  b200_ctx_leave(prev);
+  return rc;
+}
 
-scs_int scs_b200_solve_device(ScsWork *w, ScsSolution *d_sol, ScsInfo *info, scs_int warm_start, void *stream) {
+static scs_int solve_device(ScsWork *w, ScsSolution *d_sol, ScsInfo *info, scs_int warm_start, void *stream) {
   scs_int status;
   if (!w || !d_sol || !info) {
     printf("ERROR: missing ScsWork, ScsSolution or ScsInfo input\n");
@@ -1812,8 +1866,14 @@ scs_int scs_b200_solve_device(ScsWork *w, ScsSolution *d_sol, ScsInfo *info, scs
     return -1;
   if (b200_wait_for_caller(stream) != 0) return -1;
   w->sol_on_dev = 1;
-  status = scs_solve(w, d_sol, info, warm_start);
+  status = solve(w, d_sol, info, warm_start);
   w->sol_on_dev = 0;
   b200_caller_waits(stream);
+  return status;
+}
+scs_int scs_b200_solve_device(ScsWork *w, ScsSolution *d_sol, ScsInfo *info, scs_int warm_start, void *stream) {
+  B200Ctx *prev = b200_ctx_enter(w ? w->ctx : SCS_NULL);
+  const scs_int status = solve_device(w, d_sol, info, warm_start, stream);
+  b200_ctx_leave(prev);
   return status;
 }

@@ -22,6 +22,7 @@
 // Algorithmic bytes: 24 nnz + 4 (m+n+2) + 24 m + 120 n; 96 n instead of 120 n fused   (DESIGN.md).
 #include "../common.cuh"
 #include "../dev_api.h"
+#include <atomic>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -971,7 +972,7 @@ extern "C" int b200_cg_set_preconditioner(const B200Cg *cg, const double *d_Pdia
 }
 
 // peer-memory reduction: 0 = automatic (one pass for 2 ranks, two-phase for more), 1 = one pass, 2 = two-phase
-static int g_p2p_mode = -1;
+static std::atomic<int> g_p2p_mode{-1};  // read by every solving thread: atomic
 extern "C" void scs_b200_set_p2p_mode(int mode) { g_p2p_mode = mode; }
 
 // y = (R_x + P + A' R_y^-1 A) x   (private.c:106-119); dot/hook optional
@@ -1083,7 +1084,7 @@ static int mat_vec(B200Cg *cg, const double *d_x, double *d_y, int with_dot, con
 
 // sharded-x push mode (see k_cgx_iteration): -1 = read SCS_B200_SHARD_X once (default ON; =0 selects the replicated
 // modes), 0 = off, 1 = on
-static int g_shard_x = -1;
+static std::atomic<int> g_shard_x{-1};
 extern "C" void scs_b200_set_shard_x(int on) { g_shard_x = on ? 1 : 0; }
 static int shard_x_active(const B200Cg *cg) {
   if (g_shard_x < 0) {
@@ -1159,13 +1160,14 @@ extern "C" int b200_cg_plan_k34(B200Cg *cg) {
   return 0;
 }
 
-static int cg_iteration(B200Cg *cg, double *d_x) {
+// fused: K3 and K4 as k_cg_update_p (the caller holds the token when its grid has more than one block)
+static int cg_iteration(B200Cg *cg, double *d_x, bool fused) {
   if (shard_x_active(cg)) return cg_iteration_shard_x(cg, d_x);
   cudaStream_t st = (cudaStream_t)b200_stream();
   const int n = cg->n;
   const int g = k34_grid(n);
   if (mat_vec(cg, cg->d_p, cg->d_Gp, 1, &cg->d_ctl->done) != 0) return -1;
-  if (cg->k34_fused) {
+  if (fused) {
     CUDA_OK(b200_launch(k_cg_update_p, dim3(g), dim3(VEC_THREADS), 0, st, true, n, d_x, cg->d_r, cg->d_p,
                         (const double *)cg->d_Gp, (const double *)cg->d_M, cg->d_ctl, cg->d_partials, cg->d_counter,
                         (unsigned long long *)nullptr));
@@ -1181,7 +1183,41 @@ static int cg_iteration(B200Cg *cg, double *d_x) {
   return 0;
 }
 
-extern "C" int b200_cg_one_iteration(B200Cg *cg, double *d_x) { return cg_iteration(cg, d_x); }
+// timing only (bench.py): runs the path planned at setup without taking the token, so it must not overlap a solve of
+// another thread
+extern "C" int b200_cg_one_iteration(B200Cg *cg, double *d_x) { return cg_iteration(cg, d_x, cg->k34_fused != 0); }
+
+// The fused kernel's grid barrier under concurrency. k_cg_update_p needs all of its blocks resident at once; setup
+// checks that against the whole GPU. Two such grids on two streams could each get part of the SMs and wait for each
+// other until the spin gives up. So a KKT solve whose fused grid has more than one block runs it only while it holds
+// this process-wide token, taken with a try-lock (never a wait) at the start of b200_cg_solve and given back once the
+// host has seen the solve's stream drain -- also when the solve fails, so no fused launch it enqueued can still be
+// waiting to run; without it the solve runs the pair k_cg_update + k_cg_pupdate,
+// which computes the same bits (tests/test_cg_fused_gpu.py). A single-block grid has no barrier to wait at.
+// The token lives in libscs_b200_token.so, which every library flavour links, so a process that loads several flavours
+// (the int, DLONG and spectral builds) still has one token.
+// Why this cannot deadlock: with the token, at most one spinning grid of this process is on the device (nranks > 1
+// keeps one solve at a time per process; grids of other processes are outside the token). Every other resident block belongs to a kernel that does not wait for another grid, so it
+// finishes and frees its slot. A PDL dependent -- in particular the next K1 behind the fused kernel on its own
+// stream -- becomes resident only after every block of its predecessor has been scheduled, so it cannot take the slot
+// a block of the spinning grid still needs. Hence every block of the fused grid is eventually resident and the
+// barrier releases.
+namespace {
+struct K34Token {
+  bool held = false;
+  bool take() { return held = b200_k34_token_take() != 0; }
+  // after the host has seen the stream drain
+  void give_back() {
+    if (held) b200_k34_token_give_back();
+    held = false;
+  }
+  // an error return: the fused launches already enqueued must have run (or the stream have failed) first
+  ~K34Token() {
+    if (held) cudaStreamSynchronize((cudaStream_t)b200_stream());
+    give_back();
+  }
+};
+}  // namespace
 
 // Per-kernel device times of the CG loop AS IT RUNS IN A SOLVE (bench.py roofline): `reps` genuine iterations on
 // the solver's own p / tmp / r, every kernel bracketed by CUDA events on the library stream. out_ms[0..3] = average
@@ -1372,9 +1408,12 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
   const int follow = its_hint / 8 > 8 ? (its_hint / 8 < 256 ? its_hint / 8 : 256) : 8;
   long long enq = 0;
   int polls = 0;
+  K34Token token;
+  const bool fused = cg->k34_fused && (k34_grid(n) == 1 || token.take());
+  ++cg->k34_solves[fused ? 0 : 1];
   for (;;) {
     for (int i = 0; i < batch; ++i)
-      if (cg_iteration(cg, d_b) != 0) return -1;
+      if (cg_iteration(cg, d_b, fused) != 0) return -1;
     enq += batch;
     CUDA_OK(cudaMemcpyAsync(cg->h_ctl, cg->d_ctl, sizeof(B200CgCtl), cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaStreamSynchronize(st));
@@ -1392,6 +1431,7 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
     if (its_hint > 0 && polls == 1) batch = follow;
     else batch = batch < 128 ? batch * 2 : 256;
   }
+  token.give_back();  // the last fused launch has finished: the host has seen the stream drain
   if (shard_x_active(cg) && !cg->h_ctl->skip) {
     // sharded-x mode: every rank owns a slice of x; all ranks need all of it for the back-substitution
     std::vector<int> xoff((size_t)cg->nranks + 1);

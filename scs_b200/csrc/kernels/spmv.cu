@@ -19,6 +19,7 @@
 // per extra row vector read by the epilogue).
 #include "../common.cuh"
 #include "../dev_api.h"
+#include <mutex>
 #include <stdlib.h>
 #include <string.h>
 #include <vector>
@@ -653,9 +654,8 @@ extern "C" const int *b200_spmv3_plan_vptr(const B200Spmv3PlanHost *h) {
 }
 
 // ------------------------------------------------------------------ device side
-static void spmv_set_attrs() {
-  static bool attr_done = false;
-  if (attr_done) return;
+// once per process, whichever thread launches first (std::call_once: concurrent solves may race to it)
+static void spmv_set_attrs_once() {
   const int bytes = (int)spmv3_smem_bytes();
   const cudaFuncAttribute at = cudaFuncAttributeMaxDynamicSharedMemorySize;
   cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_NONE, false>, at, bytes);
@@ -667,7 +667,10 @@ static void spmv_set_attrs() {
   cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_MUL, true>, at, bytes);
   cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA_DOT, true>, at, bytes);
   cudaFuncSetAttribute(spmv_flag_kernel<B200_POST_FMA, true>, at, bytes);
-  attr_done = true;
+}
+static void spmv_set_attrs() {
+  static std::once_flag once;
+  std::call_once(once, spmv_set_attrs_once);
 }
 
 // Last step of every builder, once M's stream (d_rowptr / d_colidx / d_vals, `stored`) is in place: the warp-tiles and

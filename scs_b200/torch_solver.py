@@ -11,6 +11,9 @@ package::
 values, ``b`` (m) and ``c`` (n) CUDA float64 tensors, all on the library's device (``SCS_B200_DEVICE`` /
 ``LOCAL_RANK``). int32 indices go to libscs_b200.so and int64 indices to the DLONG library, without a conversion; a
 cone with spectral keys selects the spectral flavour. Work is ordered with ``torch.cuda.current_stream()``.
+
+One ``SCS`` object per thread is supported: threads solve their own problems at the same time, each on its own
+stream inside the library, ordered with that thread's current stream (PyTorch's current stream is per thread).
 """
 import ctypes as C
 import os
