@@ -28,10 +28,13 @@
  *      libraries leave them out.
  *
  *  (3) OPERATOR-LEVEL entry points (scs_b200_*): the cone projection, Anderson
- *      acceleration and SpMV operators of the hot path callable one at a time
- *      with host buffers.  The reference keeps these internal
- *      (include/cones.h:80-90, include/aa.h:66-143, linsys/scs_matrix.h); they are
- *      exported here so the parity tests can compare operator by operator.
+ *      acceleration and SpMV operators of the hot path callable one at a time,
+ *      with host buffers or, through the *_device twins, with device buffers
+ *      (the KKT solve of group (2) has device twins here too).  The reference
+ *      keeps these internal (include/cones.h:80-90, include/aa.h:66-143,
+ *      linsys/scs_matrix.h); they are exported here so the parity tests can
+ *      compare operator by operator, and so that a caller's own first-order
+ *      method can use them on GPU memory.
  *
  * All compute happens in hand-written sm_90a CUDA kernels; there is no CPU
  * fallback: every entry point fails (NULL / nonzero / SCS_FAILED) when no CUDA
@@ -199,7 +202,30 @@ scs_int scs_update_lin_sys_diag_r(ScsLinSysWork *w,
 const char *scs_get_lin_sys_method(void);
 
 /* ------------------------------------------------------------------ (3) --
- * Operator-level entry points (host buffers; used by tests/ and bench.py). */
+ * Operator-level entry points: the cone projection, the SpMV pair, the KKT solve (through the plugin workspace of
+ * group (2)) and Anderson acceleration, each with host buffers and, as a twin named *_device, with device buffers.
+ *
+ * The device twins. `stream` is the caller's cudaStream_t; NULL means the legacy default stream.
+ *  - Semantics: each has its host twin's semantics, lengths and return values, and computes the same bits from the
+ *    same inputs. The projection works in place on d_x; d_b (n+m) is overwritten with [x; y] and d_s (n, or NULL) is
+ *    the warm start; accumulate != 0 adds into the incoming d_y; aa_apply returns aa_norm and writes d_f; safeguard
+ *    restores d_f_new and d_x_new when it rejects.
+ *  - Workspaces are interchangeable: one made by a host init serves the device calls, and one made by
+ *    scs_b200_init_lin_sys_work_device serves the host calls. State such as the box cone's Newton warm start, the
+ *    log-det warm starts and the AA history is the workspace's, whichever door advanced it.
+ *  - Vectors: device or managed memory of the library's device, used directly, with no staging copy. d_b of the KKT
+ *    solve must be 16-byte aligned (cudaMalloc and PyTorch's allocator give 256 bytes). Refused with a message, and
+ *    with -1, NaN (aa_apply) or NULL (init), before any buffer is written: a host pointer or memory of another device;
+ *    overlapping input and output ranges (d_x / d_r_y, d_x / d_y, d_b / d_s, d_f / d_x, d_f_new / d_x_new); a NULL
+ *    workspace; a process that is one of several ranks (the operator level is single-GPU). A refused safeguard
+ *    returns -1 like a rejection, but leaves the workspace and both vectors untouched.
+ *  - Stream ordering: the library's work starts after the work enqueued on `stream` at the call, and work enqueued on
+ *    `stream` after the call runs after the library's, with no host synchronisation needed for that.
+ *  - A call that reports a result returns once the result is known: the projection after the eigensolver's sticky
+ *    error flag is read (when the cone has eigen-decomposition cones), the KKT solve after the CG count, aa_apply and
+ *    safeguard after their scalars. The SpMV pair reports nothing and returns once its work is enqueued.
+ *  - Each call binds its workspace's execution context, as the host twins do: one workspace per thread keeps working.
+ * Every library flavour that exports a host twin exports its device twin, the plugin-only libraries included. */
 
 /* CG iterations used by the most recent scs_solve_lin_sys, and the running
  * total (reference private.h:29 tot_cg_its). */
@@ -213,6 +239,22 @@ scs_int scs_b200_accum_by_a(ScsLinSysWork *w, const scs_float *x, scs_float *y,
                             scs_int accumulate);
 scs_int scs_b200_accum_by_atrans(ScsLinSysWork *w, const scs_float *x,
                                  scs_float *y, scs_int accumulate);
+scs_int scs_b200_accum_by_a_device(ScsLinSysWork *w, const scs_float *d_x, scs_float *d_y, scs_int accumulate,
+                                   void *stream);
+scs_int scs_b200_accum_by_atrans_device(ScsLinSysWork *w, const scs_float *d_x, scs_float *d_y, scs_int accumulate,
+                                        void *stream);
+
+/* The device twins of scs_init_lin_sys_work / scs_solve_lin_sys / scs_update_lin_sys_diag_r (group (2)); the
+ * workspace is released with scs_free_lin_sys_work. A (and P, its upper triangle) as for scs_b200_init_device: the
+ * structs in host memory, p, i and x device pointers; d_diag_r holds n+m entries. The matrices go through the same
+ * validating copy as scs_b200_init_device, with its messages (64-bit indices narrowed in the DLONG flavours), then
+ * through the builder of scs_init_lin_sys_work; P entries below the diagonal are refused. The caller's arrays are only
+ * read. */
+ScsLinSysWork *scs_b200_init_lin_sys_work_device(const ScsMatrix *A, const ScsMatrix *P, const scs_float *d_diag_r,
+                                                 void *stream);
+scs_int scs_b200_solve_lin_sys_device(ScsLinSysWork *w, scs_float *d_b, const scs_float *d_s, scs_float tol,
+                                      void *stream);
+scs_int scs_b200_update_lin_sys_diag_r_device(ScsLinSysWork *w, const scs_float *d_diag_r, void *stream);
 
 /* Time one device SpMV (op 0: A x via the row-major copy, op 1: A' x via the
  * CSC arrays) with per-launch CUDA events over `reps` launches; A x and A'x are
@@ -244,6 +286,7 @@ ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m,
                                     const scs_float *D);
 scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x,
                                 const scs_float *r_y);
+scs_int scs_b200_proj_dual_cone_device(ScsB200ConeWork *c, scs_float *d_x, const scs_float *d_r_y, void *stream);
 void scs_b200_finish_cone(ScsB200ConeWork *c);
 /* The Newton_stats record (reference ScsConeWork.newton_stats) after the last scs_b200_proj_dual_cone: iter,
  * newton_success and the three residuals of the last log-det cone projected. Returns 0, or -1 when the workspace
@@ -263,6 +306,8 @@ ScsB200AaWork *scs_b200_aa_init(scs_int dim, scs_int mem, scs_int min_len,
 scs_float scs_b200_aa_apply(ScsB200AaWork *a, scs_float *f, const scs_float *x);
 scs_int scs_b200_aa_safeguard(ScsB200AaWork *a, scs_float *f_new,
                               scs_float *x_new);
+scs_float scs_b200_aa_apply_device(ScsB200AaWork *a, scs_float *d_f, const scs_float *d_x, void *stream);
+scs_int scs_b200_aa_safeguard_device(ScsB200AaWork *a, scs_float *d_f_new, scs_float *d_x_new, void *stream);
 void scs_b200_aa_reset(ScsB200AaWork *a);
 void scs_b200_aa_finish(ScsB200AaWork *a);
 AaStats scs_b200_aa_get_stats(const ScsB200AaWork *a);

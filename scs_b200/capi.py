@@ -375,6 +375,23 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_aa_finish.argtypes = [C.c_void_p]
     lib.scs_b200_aa_get_stats.restype = AaStats
     lib.scs_b200_aa_get_stats.argtypes = [C.c_void_p]
+    # the device twins of the operator-level entry points (vectors in device memory, the caller's cudaStream_t last)
+    for f in (lib.scs_b200_accum_by_a_device, lib.scs_b200_accum_by_atrans_device):
+        f.restype = I
+        f.argtypes = [C.c_void_p, c_double_p, c_double_p, I, C.c_void_p]
+    lib.scs_b200_init_lin_sys_work_device.restype = C.c_void_p
+    lib.scs_b200_init_lin_sys_work_device.argtypes = [C.POINTER(ScsMatrix), C.POINTER(ScsMatrix), c_double_p,
+                                                      C.c_void_p]
+    lib.scs_b200_solve_lin_sys_device.restype = I
+    lib.scs_b200_solve_lin_sys_device.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_double, C.c_void_p]
+    lib.scs_b200_update_lin_sys_diag_r_device.restype = I
+    lib.scs_b200_update_lin_sys_diag_r_device.argtypes = [C.c_void_p, c_double_p, C.c_void_p]
+    lib.scs_b200_proj_dual_cone_device.restype = I
+    lib.scs_b200_proj_dual_cone_device.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_void_p]
+    lib.scs_b200_aa_apply_device.restype = C.c_double
+    lib.scs_b200_aa_apply_device.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_void_p]
+    lib.scs_b200_aa_safeguard_device.restype = I
+    lib.scs_b200_aa_safeguard_device.argtypes = [C.c_void_p, c_double_p, c_double_p, C.c_void_p]
     lib.scs_b200_get_stats.restype = I
     lib.scs_b200_get_stats.argtypes = [C.c_void_p, C.POINTER(ScsB200Stats)]
     lib.scs_b200_set_max_iters.restype = I

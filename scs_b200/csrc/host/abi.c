@@ -5,9 +5,11 @@
  * checked here in scs_int width against the limits of the operators (dev_api.h B200_MAX_DIM, B200_MAX_STORED) and only
  * then narrowed; a value that does not fit is refused with a message that names the limit, never truncated. The
  * matrix indices of A and P are checked and narrowed on the device, by the validating copy (kernels/setup.cu) that
- * b200_csc_upload (host/linsys_b200.c) runs them through. */
+ * b200_csc_upload (host/linsys_b200.c) runs them through. The argument checks of the device-pointer entry points
+ * (device pointers, a single GPU, disjoint vectors) are here too. */
 #include "driver.h"
 #include <stddef.h>
+#include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -108,6 +110,27 @@ int b200_matrix_over_limits(const ScsMatrix *A, const ScsMatrix *P) {
     if (b200_over_stored("nnz(P)", P->p[P->n])) return 1;
   }
   return 0;
+}
+
+/* The argument checks of the device-pointer entry points (scs_b200_*_device: host/scs_driver.c, host/operators.c,
+ * host/linsys_b200.c), here because every library flavour links this file. */
+int b200_dev_ptr_ok(const void *p, const char *what) {
+  if (b200_is_device_ptr(p)) return 1;
+  printf("ERROR: %s must point to device memory of the library's CUDA device\n", what);
+  return 0;
+}
+int b200_single_gpu(void) {
+  if (b200_comm_nranks() <= 1) return 1;
+  printf("ERROR: the device-data entry points drive a single GPU; this process is one of %d ranks\n",
+         b200_comm_nranks());
+  return 0;
+}
+int b200_overlap(const char *a_name, const void *a, size_t a_bytes, const char *b_name, const void *b,
+                 size_t b_bytes) {
+  const uintptr_t pa = (uintptr_t)a, pb = (uintptr_t)b;
+  if (!a || !b || pa >= pb + b_bytes || pb >= pa + a_bytes) return 0;
+  printf("ERROR: %s and %s must not overlap\n", a_name, b_name);
+  return 1;
 }
 
 /* an int copy of v[0..n) (values already checked); NULL when n <= 0. 0, or -1 when out of memory */

@@ -10,11 +10,14 @@
  *   scs_get_lin_sys_method    <- :221-223
  *
  * plus device-pointer variants (b200_linsys_*_dev) used by the device-resident
- * ADMM driver (host/scs_driver.c) so that the hot loop never crosses PCIe.
+ * ADMM driver (host/scs_driver.c) so that the hot loop never crosses PCIe, and
+ * the operator level's device twins of the plugin calls and of the SpMV pair
+ * (scs_b200_*_device, include/scs_b200.h group (3)) on the caller's buffers.
  */
 #include "driver.h" /* ScsWork, for scs_b200_cg_k34_paths */
 #include "linsys_b200.h"
 #include <pthread.h>
+#include <stdint.h>
 #include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
@@ -249,6 +252,85 @@ int b200_csc_upload(const char *what, int rows, int n, const void *p, const void
   return 0;
 }
 
+void b200_dev_mats_free(B200DevMats *dm) {
+  b200_free(dm->Ap); b200_free(dm->Ai); b200_free(dm->Ax);
+  b200_free(dm->Pp); b200_free(dm->Pi); b200_free(dm->Px);
+  memset(dm, 0, sizeof(*dm));
+}
+
+scs_int b200_read_dev_int(const scs_int *d_v) {
+  scs_int v = -1;
+  if (b200_d2h(&v, d_v, sizeof(scs_int)) != 0 || b200_sync() != 0) return -1;
+  return v;
+}
+/* scs_init's validate_matrix (host/scs_driver.c) on device arrays, shared by scs_b200_init_device,
+ * scs_b200_update_matrix_device and scs_b200_init_lin_sys_work_device: the same checks, in the same order, with the same messages. The host reads p[n],
+ * then the pointer flags, then the first failing entry: no kernel reads an index before the check that guards it. */
+int b200_validate_matrix_dev(const ScsMatrix *A, const ScsMatrix *P, B200DevMats *dm) {
+  const int idx64 = sizeof(scs_int) == 8;
+  unsigned flags = 0;
+  unsigned long long first = 0;
+  long long ndiag = 0;
+  scs_int Anz;
+  if (!A) { printf("A matrix missing\n"); return -1; }
+  if (A->m <= 0 || A->n <= 0) { printf("A matrix dimensions must be positive\n"); return -1; }
+  if (!A->x || !A->i || !A->p) { printf("data incompletely specified\n"); return -1; }
+  Anz = b200_read_dev_int(A->p + A->n);
+  dm->Ap = (int *)b200_malloc(((size_t)A->n + 1) * 4);
+  if (!dm->Ap || b200_csc_check_ptrs((int)A->n, (long long)Anz, A->p, idx64, dm->Ap, &flags) != 0) return -1;
+  if (flags & B200_CSC_BAD_P0) { printf("A->p[0] must equal 0\n"); return -1; }
+  if (b200_over_stored("nnz(A) = A->p[n]", Anz)) return -1;
+  if (flags & B200_CSC_BAD_PTR) { printf("A->p (column pointers) must be nonnegative and nondecreasing\n"); return -1; }
+  if (((double)Anz / A->m > A->n) || Anz < 0) {
+    printf("Anz (nonzeros in A) = %li, outside of valid range\n", (long)Anz);
+    return -1;
+  }
+  dm->nnzA = Anz;
+  dm->Ai = (int *)b200_malloc((size_t)Anz * 4);
+  dm->Ax = (double *)b200_malloc((size_t)Anz * 8);
+  if (!dm->Ai || !dm->Ax ||
+      b200_csc_copy_entries((int)A->m, (int)A->n, Anz, A->i, A->x, idx64, dm->Ap, 0, dm->Ai, dm->Ax, &first, &ndiag) != 0)
+    return -1;
+  if (first != ~0ULL) {
+    const long long kk = (long long)(first >> 2);
+    if ((first & 3) == B200_CSC_BAD_ROW) {
+      printf("A row index %li outside valid range [0, %li]\n", (long)b200_read_dev_int(A->i + kk), (long)A->m - 1);
+    } else {
+      printf("A contains a non-finite entry\n");
+    }
+    return -1;
+  }
+  if (P) {
+    scs_int Pnz;
+    if (!P->x || !P->i || !P->p) { printf("P matrix incompletely specified\n"); return -1; }
+    if (P->n != A->n) { printf("P dimension inconsistent with n\n"); return -1; }
+    if (P->m != P->n) { printf("P is not square\n"); return -1; }
+    Pnz = b200_read_dev_int(P->p + P->n);
+    dm->Pp = (int *)b200_malloc(((size_t)P->n + 1) * 4);
+    if (!dm->Pp || b200_csc_check_ptrs((int)P->n, (long long)Pnz, P->p, idx64, dm->Pp, &flags) != 0) return -1;
+    if (flags & B200_CSC_BAD_P0) { printf("P->p[0] must equal 0\n"); return -1; }
+    if (b200_over_stored("nnz(P) = P->p[n]", Pnz)) return -1;
+    if (flags & B200_CSC_BAD_PTR) { printf("P->p (column pointers) must be nonnegative and nondecreasing\n"); return -1; }
+    if (((double)Pnz / P->m > P->n) || Pnz < 0) { printf("Pnz outside of valid range\n"); return -1; }
+    dm->nnzP = Pnz;
+    dm->Pi = (int *)b200_malloc((size_t)Pnz * 4);
+    dm->Px = (double *)b200_malloc((size_t)Pnz * 8);
+    if (!dm->Pi || !dm->Px ||
+        b200_csc_copy_entries((int)P->n, (int)P->n, Pnz, P->i, P->x, idx64, dm->Pp, 1, dm->Pi, dm->Px, &first,
+                              &ndiag) != 0)
+      return -1;
+    if (first != ~0ULL) {
+      const int code = (int)(first & 3);
+      printf(code == B200_CSC_BAD_ROW ? "P row index outside valid range\n"
+             : code == B200_CSC_BAD_UPPER ? "P is not upper triangular\n" : "P contains a non-finite entry\n");
+      return -1;
+    }
+    dm->fullP = 2 * (long long)Pnz - ndiag;
+    if (b200_over_stored("stored entries of the full symmetric P", dm->fullP)) return -1;
+  }
+  return 0;
+}
+
 /* Both resident orientations of an m x n host CSC (*A_out = the m x n operator, *At_out = the n x m one): one upload,
  * then the device builder */
 static int ops_from_host(int m, int n, const void *p, const void *i, const double *x, int idx64, B200Spmv **A_out,
@@ -308,7 +390,25 @@ static int cg_ops_refresh(ScsLinSysWork *w) {
   return b200_cg_classify_diag(&w->cg, w->d_perm);
 }
 
-static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_mark_p);
+static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, int diag_on_dev, double *t_mark_p);
+
+/* P's operator and diagonal (w->P, w->d_Pdiag) from its upper CSC in the builder's validated device arrays (nnzP
+ * entries; `full` stored entries once expanded to the full symmetric P). The structure's blocks are freed here,
+ * stream-ordered. */
+static int p_from_dev_csc(ScsLinSysWork *w, long long nnzP, long long full, const int *Pp, const int *Pi,
+                          const double *Px) {
+  const int n = w->n;
+  int *Fp = (int *)b200_malloc(((size_t)n + 1) * 4);
+  int *Fi = (int *)b200_malloc((size_t)full * 4);
+  int *Fsrc = (int *)b200_malloc((size_t)full * 4);
+  int rc = -1;
+  w->d_Pdiag = (double *)b200_malloc((size_t)n * 8);
+  if (Fp && Fi && Fsrc && w->d_Pdiag && b200_sym_expand_structure(n, nnzP, full, Pp, Pi, Fp, Fi, Fsrc) == 0 &&
+      b200_sym_build(n, full, Fp, Fi, Fsrc, Px, w->d_Pdiag, &w->P) == 0)
+    rc = 0;
+  b200_free(Fp); b200_free(Fi); b200_free(Fsrc);
+  return rc;
+}
 
 static ScsLinSysWork *init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P, const scs_float *diag_r) {
   ScsLinSysWork *w;
@@ -355,29 +455,22 @@ static ScsLinSysWork *init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P, 
   }
   setup_mark("linsys: both operators built on the device", &t_mark);
   if (P) { /* replicated on every rank: the upper CSC uploaded, then expanded to the full symmetric P on the device */
-    int *Pp = NULL, *Pi = NULL, *Fp = NULL, *Fi = NULL, *Fsrc = NULL;
+    int *Pp = NULL, *Pi = NULL;
     double *Px = NULL;
     long long nnzP = 0, ndiag = 0, full;
     int rc = -1;
     if (b200_csc_upload("P", n, n, P->p, P->i, P->x, idx64, 1, &Pp, &Pi, &Px, &nnzP, &ndiag) != 0) goto fail;
     full = 2 * nnzP - ndiag;
-    if (full > B200_MAX_STORED) {
+    if (full > B200_MAX_STORED)
       fprintf(stderr, "scs_b200: the full symmetric P has %lld stored entries, above the limit 2^31 - 129 of one "
               "operator\n", full);
-    } else {
-      Fp = (int *)b200_malloc(((size_t)n + 1) * 4);
-      Fi = (int *)b200_malloc((size_t)full * 4);
-      Fsrc = (int *)b200_malloc((size_t)full * 4);
-      w->d_Pdiag = (double *)b200_malloc((size_t)n * 8);
-      if (Fp && Fi && Fsrc && w->d_Pdiag && b200_sym_expand_structure(n, nnzP, full, Pp, Pi, Fp, Fi, Fsrc) == 0 &&
-          b200_sym_build(n, full, Fp, Fi, Fsrc, Px, w->d_Pdiag, &w->P) == 0)
-        rc = 0;
-    }
-    b200_free(Pp); b200_free(Pi); b200_free(Px); b200_free(Fp); b200_free(Fi); b200_free(Fsrc); /* stream-ordered */
+    else
+      rc = p_from_dev_csc(w, nnzP, full, Pp, Pi, Px);
+    b200_free(Pp); b200_free(Pi); b200_free(Px); /* stream-ordered */
     if (rc != 0) goto fail;
     setup_mark("linsys: operator P (device expansion)", &t_mark);
   }
-  if (linsys_vectors(w, diag_r, &t_mark) != 0) goto fail;
+  if (linsys_vectors(w, diag_r, 0, &t_mark) != 0) goto fail;
   return w;
 fail:
   fprintf(stderr, "scs_b200: init_lin_sys_work failed: %s\n", b200_last_error());
@@ -404,6 +497,65 @@ ScsLinSysWork *scs_init_lin_sys_work(const ScsMatrix *A, const ScsMatrix *P,
   return w;
 }
 
+/* scs_init_lin_sys_work with A, P and diag_r in device memory (single GPU): scs_b200_init_device's validating copy
+ * of the caller's CSC arrays, then the builder the host init runs on the blocks it uploads */
+static ScsLinSysWork *init_lin_sys_work_device(const ScsMatrix *A, const ScsMatrix *P, const scs_float *d_diag_r,
+                                               void *stream) {
+  double t_mark = wall_ms();
+  B200DevMats dm;
+  ScsLinSysWork *w = SCS_NULL;
+  memset(&dm, 0, sizeof(dm));
+  if (!A) { printf("A matrix missing\n"); return SCS_NULL; }
+  if (b200_runtime_init() != 0) {
+    fprintf(stderr, "scs_b200: no usable sm_90 device: %s\n", b200_last_error());
+    return SCS_NULL;
+  }
+  if (!b200_single_gpu() || b200_over_dim("A->m", -1, A->m) || b200_over_dim("A->n", -1, A->n)) return SCS_NULL;
+  if ((A->p && !b200_dev_ptr_ok(A->p, "A->p")) || (A->i && !b200_dev_ptr_ok(A->i, "A->i")) ||
+      (A->x && !b200_dev_ptr_ok(A->x, "A->x")) ||
+      (P && ((P->p && !b200_dev_ptr_ok(P->p, "P->p")) || (P->i && !b200_dev_ptr_ok(P->i, "P->i")) ||
+             (P->x && !b200_dev_ptr_ok(P->x, "P->x")))) ||
+      !b200_dev_ptr_ok(d_diag_r, "diag_r"))
+    return SCS_NULL;
+  if (b200_wait_for_caller(stream) != 0) return SCS_NULL;
+  if (b200_validate_matrix_dev(A, P, &dm) != 0) {
+    printf("invalid linear system input data\n");
+  } else if ((w = (ScsLinSysWork *)calloc(1, sizeof(ScsLinSysWork))) != SCS_NULL) {
+    w->ctx = b200_ctx_bound();
+    w->n = (int)A->n; w->m = (int)A->m;
+    w->nnz = dm.nnzA;
+    w->nranks = 1;
+    w->mloc = w->m;
+    if (b200_setup_ops_from_dev(w->m, w->n, dm.nnzA, dm.Ap, dm.Ai, dm.Ax, &w->A, &w->At) != 0 ||
+        (P && p_from_dev_csc(w, dm.nnzP, dm.fullP, dm.Pp, dm.Pi, dm.Px) != 0) ||
+        linsys_vectors(w, d_diag_r, 1, &t_mark) != 0) {
+      fprintf(stderr, "scs_b200: init_lin_sys_work failed: %s\n", b200_last_error());
+      scs_free_lin_sys_work(w);
+      w = SCS_NULL;
+    }
+  }
+  b200_sync(); /* the builder's blocks are free only once its kernels have run */
+  b200_dev_mats_free(&dm);
+  b200_caller_waits(stream);
+  return w;
+}
+ScsLinSysWork *scs_b200_init_lin_sys_work_device(const ScsMatrix *A, const ScsMatrix *P, const scs_float *d_diag_r,
+                                                 void *stream) {
+  B200Ctx *own = SCS_NULL, *prev = SCS_NULL;
+  ScsLinSysWork *w;
+  if (!b200_ctx_bound()) {
+    own = b200_ctx_create();
+    prev = b200_ctx_enter(own);
+  }
+  w = init_lin_sys_work_device(A, P, d_diag_r, stream);
+  if (w) w->own_ctx = own != SCS_NULL;
+  if (own) {
+    b200_ctx_leave(prev);
+    if (!w) b200_ctx_release(own);
+  }
+  return w;
+}
+
 /* single GPU, from operators built on the device (the device-data entry points, host/scs_driver.c): the workspace takes
  * A, At, P and d_Pdiag over, also when it fails */
 ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B200Spmv *P, double *d_Pdiag,
@@ -420,7 +572,7 @@ ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B20
   w->nranks = 1;
   w->mloc = m;
   w->A = A; w->At = At; w->P = P; w->d_Pdiag = d_Pdiag;
-  if (linsys_vectors(w, diag_r, &t_mark) != 0) {
+  if (linsys_vectors(w, diag_r, 0, &t_mark) != 0) {
     fprintf(stderr, "scs_b200: init_lin_sys_work failed: %s\n", b200_last_error());
     scs_free_lin_sys_work(w);
     return SCS_NULL;
@@ -428,8 +580,9 @@ ScsLinSysWork *b200_linsys_from_ops(int m, int n, B200Spmv *A, B200Spmv *At, B20
   return w;
 }
 
-/* the work vectors, the preconditioner and the CG loop's reordered pair of a workspace whose operators are built */
-static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_mark_p) {
+/* the work vectors, the preconditioner and the CG loop's reordered pair of a workspace whose operators are built;
+ * diag_r (n + m) in host memory, or with diag_on_dev in device memory */
+static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, int diag_on_dev, double *t_mark_p) {
   const int n = w->n, m = w->m;
   double t_mark = *t_mark_p;
   w->d_diag_r = (double *)b200_malloc(((size_t)n + m + 1) * 8);
@@ -492,7 +645,9 @@ static int linsys_vectors(ScsLinSysWork *w, const scs_float *diag_r, double *t_m
     w->cg.d_p = (double *)b200_malloc((size_t)n * 8);
     if (!w->cg.d_p) return -1;
   }
-  if (b200_h2d(w->d_diag_r, diag_r, ((size_t)n + m) * 8) != 0) return -1;
+  if ((diag_on_dev ? b200_d2d(w->d_diag_r, diag_r, ((size_t)n + m) * 8)
+                   : b200_h2d(w->d_diag_r, diag_r, ((size_t)n + m) * 8)) != 0)
+    return -1;
   if (b200_cg_set_preconditioner(&w->cg, w->d_Pdiag) != 0) return -1;
   if (b200_cg_plan_k34(&w->cg) != 0) return -1;
   if (b200_sync() != 0) return -1;
@@ -590,12 +745,15 @@ int b200_linsys_update_diag_r_dev(ScsLinSysWork *w, const double *d_diag_r) {
   return cg_ops_refresh(w); /* the operators may have been rescaled in place; R_y has changed */
 }
 
-static scs_int solve_lin_sys(ScsLinSysWork *w, scs_float *b, const scs_float *s, scs_float tol) {
-  const size_t nm = (size_t)w->n + w->m;
+static void warn_tol(scs_float tol) {
   if (tol <= 0.) {
     fprintf(stderr, "Warning: tol = %4f <= 0, likely compiled without setting INDIRECT flag.\n",
             tol);
   }
+}
+static scs_int solve_lin_sys(ScsLinSysWork *w, scs_float *b, const scs_float *s, scs_float tol) {
+  const size_t nm = (size_t)w->n + w->m;
+  warn_tol(tol);
   if (b200_h2d(w->d_b, b, nm * 8) != 0) return -1;
   if (s && b200_h2d(w->d_s, s, (size_t)w->n * 8) != 0) return -1;
   if (b200_linsys_solve_dev(w, w->d_b, s ? w->d_s : NULL, tol, NULL) != 0) return -1;
@@ -622,6 +780,58 @@ scs_int scs_update_lin_sys_diag_r(ScsLinSysWork *w, const scs_float *new_diag_r)
   return rc;
 }
 
+/* The device twins (include/scs_b200.h group (3)): the host twin's device function on the caller's buffers, after
+ * the argument checks, between b200_wait_for_caller and b200_caller_waits. */
+static int device_call_ok(const ScsLinSysWork *w) {
+  if (!w) { printf("ERROR: missing ScsLinSysWork input\n"); return 0; }
+  return b200_single_gpu();
+}
+
+static scs_int solve_lin_sys_device(ScsLinSysWork *w, scs_float *d_b, const scs_float *d_s, scs_float tol,
+                                    void *stream) {
+  int rc;
+  if (!b200_dev_ptr_ok(d_b, "b") || (d_s && !b200_dev_ptr_ok(d_s, "s")) ||
+      b200_overlap("b", d_b, ((size_t)w->n + w->m) * 8, "s", d_s, (size_t)w->n * 8))
+    return -1;
+  if ((uintptr_t)d_b % 16 != 0) { /* the CG loop's update kernels read and write x two entries at a time */
+    printf("ERROR: b must be 16-byte aligned\n");
+    return -1;
+  }
+  warn_tol(tol);
+  if (b200_wait_for_caller(stream) != 0) return -1;
+  rc = b200_linsys_solve_dev(w, d_b, d_s, tol, NULL); /* returns once the host has read the CG count */
+  b200_caller_waits(stream);
+  return rc == 0 ? 0 : -1;
+}
+scs_int scs_b200_solve_lin_sys_device(ScsLinSysWork *w, scs_float *d_b, const scs_float *d_s, scs_float tol,
+                                      void *stream) {
+  B200Ctx *prev;
+  scs_int rc;
+  if (!device_call_ok(w)) return -1;
+  prev = b200_ctx_enter(w->ctx);
+  rc = solve_lin_sys_device(w, d_b, d_s, tol, stream);
+  b200_ctx_leave(prev);
+  return rc;
+}
+
+static scs_int update_lin_sys_diag_r_device(ScsLinSysWork *w, const scs_float *d_diag_r, void *stream) {
+  int rc;
+  if (!b200_dev_ptr_ok(d_diag_r, "diag_r")) return -1;
+  if (b200_wait_for_caller(stream) != 0) return -1;
+  rc = b200_linsys_update_diag_r_dev(w, d_diag_r); /* its classification of R_y reads 4 bytes back */
+  b200_caller_waits(stream);
+  return rc == 0 ? 0 : -1;
+}
+scs_int scs_b200_update_lin_sys_diag_r_device(ScsLinSysWork *w, const scs_float *d_diag_r, void *stream) {
+  B200Ctx *prev;
+  scs_int rc;
+  if (!device_call_ok(w)) return -1;
+  prev = b200_ctx_enter(w->ctx);
+  rc = update_lin_sys_diag_r_device(w, d_diag_r, stream);
+  b200_ctx_leave(prev);
+  return rc;
+}
+
 scs_int scs_b200_linsys_last_cg_its(const ScsLinSysWork *w) { return w->last_cg_its; }
 long long scs_b200_linsys_total_cg_its(const ScsLinSysWork *w) { return w->tot_cg_its; }
 
@@ -642,9 +852,17 @@ scs_int scs_b200_cg_k34_paths(const ScsWork *w, long long out[2]) {
   return 0;
 }
 
+/* y (+)= M x on device vectors: accumulating, the chain of each row starts at y's own entry */
+static int accum_dev(const B200Spmv *M, const double *d_x, double *d_y, scs_int accumulate) {
+  B200SpmvArgs a;
+  memset(&a, 0, sizeof(a));
+  a.d_x = d_x; a.d_y = d_y; a.d_init = accumulate ? d_y : NULL; a.init_sign = 1.0;
+  a.post = B200_POST_NONE; a.hook = B200_HOOK_NONE;
+  return b200_spmv(M, &a);
+}
+
 static scs_int accum_generic(ScsLinSysWork *w, const B200Spmv *M, int ncols, int nrows,
                              const scs_float *x, scs_float *y, scs_int accumulate) {
-  B200SpmvArgs a;
   B200Ctx *prev = b200_ctx_enter(w->ctx);
   double *d_x = (double *)b200_malloc((size_t)ncols * 8);
   double *d_y = (double *)b200_malloc((size_t)nrows * 8);
@@ -653,10 +871,7 @@ static scs_int accum_generic(ScsLinSysWork *w, const B200Spmv *M, int ncols, int
   if (!d_x || !d_y) goto out;
   if (b200_h2d(d_x, x, (size_t)ncols * 8) != 0) goto out;
   if (accumulate && b200_h2d(d_y, y, (size_t)nrows * 8) != 0) goto out;
-  memset(&a, 0, sizeof(a));
-  a.d_x = d_x; a.d_y = d_y; a.d_init = accumulate ? d_y : NULL; a.init_sign = 1.0;
-  a.post = B200_POST_NONE; a.hook = B200_HOOK_NONE;
-  if (b200_spmv(M, &a) != 0) goto out;
+  if (accum_dev(M, d_x, d_y, accumulate) != 0) goto out;
   if (b200_d2h(y, d_y, (size_t)nrows * 8) != 0) goto out;
   if (b200_sync() != 0) goto out;
   rc = 0;
@@ -674,6 +889,33 @@ scs_int scs_b200_accum_by_a(ScsLinSysWork *w, const scs_float *x, scs_float *y,
 scs_int scs_b200_accum_by_atrans(ScsLinSysWork *w, const scs_float *x, scs_float *y,
                                  scs_int accumulate) {
   return accum_generic(w, w->At, w->m, w->n, x, y, accumulate);
+}
+
+/* enqueued only: the SpMV reports nothing, and the caller's stream waits for it */
+static scs_int accum_device(ScsLinSysWork *w, int trans, const scs_float *d_x, scs_float *d_y, scs_int accumulate,
+                            void *stream) {
+  size_t ncols, nrows;
+  B200Ctx *prev;
+  int rc = -1;
+  if (!device_call_ok(w)) return -1;
+  ncols = (size_t)(trans ? w->m : w->n);
+  nrows = (size_t)(trans ? w->n : w->m);
+  prev = b200_ctx_enter(w->ctx);
+  if (b200_dev_ptr_ok(d_x, "x") && b200_dev_ptr_ok(d_y, "y") && !b200_overlap("x", d_x, ncols * 8, "y", d_y, nrows * 8) &&
+      b200_wait_for_caller(stream) == 0) {
+    rc = accum_dev(trans ? w->At : w->A, d_x, d_y, accumulate) == 0 ? 0 : -1;
+    b200_caller_waits(stream);
+  }
+  b200_ctx_leave(prev);
+  return rc;
+}
+scs_int scs_b200_accum_by_a_device(ScsLinSysWork *w, const scs_float *d_x, scs_float *d_y, scs_int accumulate,
+                                   void *stream) {
+  return accum_device(w, 0, d_x, d_y, accumulate, stream);
+}
+scs_int scs_b200_accum_by_atrans_device(ScsLinSysWork *w, const scs_float *d_x, scs_float *d_y, scs_int accumulate,
+                                        void *stream) {
+  return accum_device(w, 1, d_x, d_y, accumulate, stream);
 }
 
 /* --- device timing helpers for bench.py (inputs resident in HBM) --------- */

@@ -58,5 +58,26 @@ void b200_row_partition(int m, int n, const scs_int *Ap, const scs_int *Ai, int 
 int b200_over_dim(const char *what, long long index, scs_int v);
 int b200_over_stored(const char *what, scs_int v);
 int b200_matrix_over_limits(const ScsMatrix *A, const ScsMatrix *P);
+/* the argument checks of the device-pointer entry points (host/abi.c), each printing a message when it fails:
+ * b200_dev_ptr_ok: 1 when p is device or managed memory of the library's device; b200_single_gpu: 1 unless the
+ * process is one of several ranks; b200_overlap: 1 when the byte ranges [a, a + a_bytes) and [b, b + b_bytes)
+ * intersect (a NULL pointer overlaps nothing) */
+int b200_dev_ptr_ok(const void *p, const char *what);
+int b200_single_gpu(void);
+int b200_overlap(const char *a_name, const void *a, size_t a_bytes, const char *b_name, const void *b,
+                 size_t b_bytes);
+
+/* The caller's device CSC arrays, validated and copied into the library's own int32 / fp64 blocks */
+typedef struct {
+  int *Ap, *Ai, *Pp, *Pi;
+  double *Ax, *Px;
+  long long nnzA, nnzP, fullP;
+} B200DevMats;
+void b200_dev_mats_free(B200DevMats *dm);
+/* one scs_int of device memory, read back (syncs); -1 on failure */
+scs_int b200_read_dev_int(const scs_int *d_v);
+/* scs_init's validate_matrix on device arrays (the CSC index arrays in scs_int width): the same checks, in the same
+ * order, with the same messages, run by the validating copy (kernels/setup.cu) into dm's blocks. 0, or -1 */
+int b200_validate_matrix_dev(const ScsMatrix *A, const ScsMatrix *P, B200DevMats *dm);
 
 #endif

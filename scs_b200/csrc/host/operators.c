@@ -1,9 +1,9 @@
-/* operators.c -- operator-level C-ABI entry points with HOST buffers, used by
- * the parity tests and bench.py to compare one operator at a time against the
- * reference: the cone projection (reference src/cones.c:1498-1596) and Anderson
- * acceleration (reference src/aa.c:657-979). Each call stages the host arrays
- * through device memory and runs the same kernels the ADMM driver uses. Each
- * workspace has an execution context of its own (dev_api.h), bound by every call. */
+/* operators.c -- operator-level C-ABI entry points: the cone projection (reference src/cones.c:1498-1596) and
+ * Anderson acceleration (reference src/aa.c:657-979), each through two doors. The host door stages host arrays
+ * through the workspace's device buffers (the parity tests and bench.py compare one operator at a time against the
+ * reference with it); the device door (scs_b200_*_device) runs on the caller's device buffers, ordered with the
+ * caller's stream. Both run the same kernels the ADMM driver uses. Each workspace has an execution context of its own
+ * (dev_api.h), bound by every call. */
 #include "driver.h"
 #include <math.h>
 #include <stdio.h>
@@ -132,6 +132,31 @@ scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x, const scs_floa
   return rc;
 }
 
+/* The device twins (include/scs_b200.h group (3)): the host twin's device function on the caller's buffers, after
+ * the argument checks, between b200_wait_for_caller and b200_caller_waits. */
+static scs_int proj_dual_cone_device(ScsB200ConeWork *c, scs_float *d_x, const scs_float *d_r_y, void *stream) {
+  const size_t bytes = (size_t)c->m * 8;
+  int rc;
+  if (!b200_dev_ptr_ok(d_x, "x") || (d_r_y && !b200_dev_ptr_ok(d_r_y, "r_y")) ||
+      b200_overlap("x", d_x, bytes, "r_y", d_r_y, bytes))
+    return -1;
+  if (b200_wait_for_caller(stream) != 0) return -1;
+  rc = b200_cones_proj_dual(c->cones, d_x, d_r_y);
+  b200_caller_waits(stream);
+  if (rc != 0) return -1;
+  return b200_cones_check(c->cones); /* reads the sticky flag back when there are eigen-decomposition cones */
+}
+scs_int scs_b200_proj_dual_cone_device(ScsB200ConeWork *c, scs_float *d_x, const scs_float *d_r_y, void *stream) {
+  B200Ctx *prev;
+  scs_int rc;
+  if (!c) { printf("ERROR: missing ScsB200ConeWork input\n"); return -1; }
+  if (!b200_single_gpu()) return -1;
+  prev = b200_ctx_enter(c->ctx);
+  rc = proj_dual_cone_device(c, d_x, d_r_y, stream);
+  b200_ctx_leave(prev);
+  return rc;
+}
+
 scs_int scs_b200_cone_logdet_stats(ScsB200ConeWork *c, scs_int *iter, scs_int *newton_success,
                                    scs_float *residuals) {
   int it = 0, success = 0, rc;
@@ -236,6 +261,39 @@ static scs_int aa_safeguard(ScsB200AaWork *w, scs_float *f_new, scs_float *x_new
 scs_int scs_b200_aa_safeguard(ScsB200AaWork *w, scs_float *f_new, scs_float *x_new) {
   B200Ctx *prev = b200_ctx_enter(w->ctx);
   const scs_int rc = aa_safeguard(w, f_new, x_new);
+  b200_ctx_leave(prev);
+  return rc;
+}
+
+/* the AA twins: refused with NaN (apply) or -1 (safeguard), the workspace and both vectors untouched */
+static int aa_device_ok(const ScsB200AaWork *w, const char *f_name, const scs_float *d_f, const char *x_name,
+                        const scs_float *d_x) {
+  const size_t bytes = w ? (size_t)w->dim * 8 : 0;
+  if (!w) { printf("ERROR: missing ScsB200AaWork input\n"); return 0; }
+  return b200_single_gpu() && b200_dev_ptr_ok(d_f, f_name) && b200_dev_ptr_ok(d_x, x_name) &&
+         !b200_overlap(f_name, d_f, bytes, x_name, d_x, bytes);
+}
+scs_float scs_b200_aa_apply_device(ScsB200AaWork *w, scs_float *d_f, const scs_float *d_x, void *stream) {
+  B200Ctx *prev;
+  scs_float nrm = NAN;
+  if (!aa_device_ok(w, "f", d_f, "x", d_x)) return NAN;
+  prev = b200_ctx_enter(w->ctx);
+  if (b200_wait_for_caller(stream) == 0) {
+    nrm = b200_aa_apply_dev(w->a, d_f, d_x); /* the scalars it needs are read back before it returns */
+    b200_caller_waits(stream);
+  }
+  b200_ctx_leave(prev);
+  return nrm;
+}
+scs_int scs_b200_aa_safeguard_device(ScsB200AaWork *w, scs_float *d_f_new, scs_float *d_x_new, void *stream) {
+  B200Ctx *prev;
+  scs_int rc = -1;
+  if (!aa_device_ok(w, "f_new", d_f_new, "x_new", d_x_new)) return -1;
+  prev = b200_ctx_enter(w->ctx);
+  if (b200_wait_for_caller(stream) == 0) {
+    rc = b200_aa_safeguard_dev(w->a, d_f_new, d_x_new);
+    b200_caller_waits(stream);
+  }
   b200_ctx_leave(prev);
   return rc;
 }

@@ -111,19 +111,8 @@ static int validate_matrix(const ScsMatrix *A, const ScsMatrix *P) {
   return 0;
 }
 
-/* The caller's device CSC arrays, validated and copied into the library's own int32 / fp64 blocks */
-typedef struct {
-  int *Ap, *Ai, *Pp, *Pi;
-  double *Ax, *Px;
-  long long nnzA, nnzP, fullP;
-} DevMats;
-static void dev_mats_free(DevMats *dm) {
-  b200_free(dm->Ap); b200_free(dm->Ai); b200_free(dm->Ax);
-  b200_free(dm->Pp); b200_free(dm->Pi); b200_free(dm->Px);
-  memset(dm, 0, sizeof(*dm));
-}
 /* the same blocks from a host A and P that validate_matrix has accepted (scs_init on one GPU) */
-static int dev_mats_from_host(const ScsMatrix *A, const ScsMatrix *P, DevMats *dm) {
+static int dev_mats_from_host(const ScsMatrix *A, const ScsMatrix *P, B200DevMats *dm) {
   const int idx64 = sizeof(scs_int) == 8;
   long long ndiag = 0;
   if (b200_csc_upload("A", (int)A->m, (int)A->n, A->p, A->i, A->x, idx64, 0, &dm->Ap, &dm->Ai, &dm->Ax, &dm->nnzA,
@@ -137,78 +126,6 @@ static int dev_mats_from_host(const ScsMatrix *A, const ScsMatrix *P, DevMats *d
   }
   return 0;
 }
-static scs_int read_dev_int(const scs_int *d_v) {
-  scs_int v = -1;
-  if (b200_d2h(&v, d_v, sizeof(scs_int)) != 0 || b200_sync() != 0) return -1;
-  return v;
-}
-/* validate_matrix on device arrays: the same checks, in the same order, with the same messages. The host reads p[n],
- * then the pointer flags, then the first failing entry: no kernel reads an index before the check that guards it. */
-static int validate_matrix_dev(const ScsMatrix *A, const ScsMatrix *P, DevMats *dm) {
-  const int idx64 = sizeof(scs_int) == 8;
-  unsigned flags = 0;
-  unsigned long long first = 0;
-  long long ndiag = 0;
-  scs_int Anz;
-  if (!A) { printf("A matrix missing\n"); return -1; }
-  if (A->m <= 0 || A->n <= 0) { printf("A matrix dimensions must be positive\n"); return -1; }
-  if (!A->x || !A->i || !A->p) { printf("data incompletely specified\n"); return -1; }
-  Anz = read_dev_int(A->p + A->n);
-  dm->Ap = (int *)b200_malloc(((size_t)A->n + 1) * 4);
-  if (!dm->Ap || b200_csc_check_ptrs((int)A->n, (long long)Anz, A->p, idx64, dm->Ap, &flags) != 0) return -1;
-  if (flags & B200_CSC_BAD_P0) { printf("A->p[0] must equal 0\n"); return -1; }
-  if (b200_over_stored("nnz(A) = A->p[n]", Anz)) return -1;
-  if (flags & B200_CSC_BAD_PTR) { printf("A->p (column pointers) must be nonnegative and nondecreasing\n"); return -1; }
-  if (((double)Anz / A->m > A->n) || Anz < 0) {
-    printf("Anz (nonzeros in A) = %li, outside of valid range\n", (long)Anz);
-    return -1;
-  }
-  dm->nnzA = Anz;
-  dm->Ai = (int *)b200_malloc((size_t)Anz * 4);
-  dm->Ax = (double *)b200_malloc((size_t)Anz * 8);
-  if (!dm->Ai || !dm->Ax ||
-      b200_csc_copy_entries((int)A->m, (int)A->n, Anz, A->i, A->x, idx64, dm->Ap, 0, dm->Ai, dm->Ax, &first, &ndiag) != 0)
-    return -1;
-  if (first != ~0ULL) {
-    const long long kk = (long long)(first >> 2);
-    if ((first & 3) == B200_CSC_BAD_ROW) {
-      printf("A row index %li outside valid range [0, %li]\n", (long)read_dev_int(A->i + kk), (long)A->m - 1);
-    } else {
-      printf("A contains a non-finite entry\n");
-    }
-    return -1;
-  }
-  if (P) {
-    scs_int Pnz;
-    if (!P->x || !P->i || !P->p) { printf("P matrix incompletely specified\n"); return -1; }
-    if (P->n != A->n) { printf("P dimension inconsistent with n\n"); return -1; }
-    if (P->m != P->n) { printf("P is not square\n"); return -1; }
-    Pnz = read_dev_int(P->p + P->n);
-    dm->Pp = (int *)b200_malloc(((size_t)P->n + 1) * 4);
-    if (!dm->Pp || b200_csc_check_ptrs((int)P->n, (long long)Pnz, P->p, idx64, dm->Pp, &flags) != 0) return -1;
-    if (flags & B200_CSC_BAD_P0) { printf("P->p[0] must equal 0\n"); return -1; }
-    if (b200_over_stored("nnz(P) = P->p[n]", Pnz)) return -1;
-    if (flags & B200_CSC_BAD_PTR) { printf("P->p (column pointers) must be nonnegative and nondecreasing\n"); return -1; }
-    if (((double)Pnz / P->m > P->n) || Pnz < 0) { printf("Pnz outside of valid range\n"); return -1; }
-    dm->nnzP = Pnz;
-    dm->Pi = (int *)b200_malloc((size_t)Pnz * 4);
-    dm->Px = (double *)b200_malloc((size_t)Pnz * 8);
-    if (!dm->Pi || !dm->Px ||
-        b200_csc_copy_entries((int)P->n, (int)P->n, Pnz, P->i, P->x, idx64, dm->Pp, 1, dm->Pi, dm->Px, &first,
-                              &ndiag) != 0)
-      return -1;
-    if (first != ~0ULL) {
-      const int code = (int)(first & 3);
-      printf(code == B200_CSC_BAD_ROW ? "P row index outside valid range\n"
-             : code == B200_CSC_BAD_UPPER ? "P is not upper triangular\n" : "P contains a non-finite entry\n");
-      return -1;
-    }
-    dm->fullP = 2 * (long long)Pnz - ndiag;
-    if (b200_over_stored("stored entries of the full symmetric P", dm->fullP)) return -1;
-  }
-  return 0;
-}
-
 static int validate_cones(const ScsData *d, const ScsCone *k) {
   scs_int i;
   long long dims;
@@ -311,7 +228,7 @@ static int validate_cones(const ScsData *d, const ScsCone *k) {
   return 0;
 }
 
-static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm) {
+static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, B200DevMats *dm) {
   if (d->m <= 0 || d->n <= 0) {
     printf("m and n must both be greater than 0; m = %li, n = %li\n", (long)d->m, (long)d->n);
     return -1;
@@ -322,7 +239,7 @@ static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs,
     return -1;
   }
   if (!d->b || !d->c) { printf("b or c missing\n"); return -1; }
-  if ((dm ? validate_matrix_dev(d->A, d->P, dm) : validate_matrix(d->A, d->P)) < 0) {
+  if ((dm ? b200_validate_matrix_dev(d->A, d->P, dm) : validate_matrix(d->A, d->P)) < 0) {
     printf("invalid linear system input data\n");
     return -1;
   }
@@ -547,14 +464,14 @@ static void print_header(const ScsWork *w) {
 }
 
 static int update_bc_dev(ScsWork *w);
-static int build_ops_dev(ScsWork *w, DevMats *dm);
+static int build_ops_dev(ScsWork *w, B200DevMats *dm);
 static void write_data_dev(const char *filename, const ScsData *d, const ScsCone *k, const ScsSettings *stgs);
 
 /* dev_data: the device-data entry point, d's arrays are device pointers, validated into dm's blocks; else scs_init,
  * the data in host memory, validated there. On one GPU (dm != NULL) the operators are built on the device from dm's
  * blocks (build_ops_dev), which scs_init fills from the host A and P. Several GPUs (dm == NULL, scs_init only) cut A
  * into row blocks on the host (scs_init_lin_sys_work). */
-static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, DevMats *dm, int dev_data,
+static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, B200DevMats *dm, int dev_data,
                           B200Ctx *ctx) {
   ScsWork *w;
   const double t0 = now_ms();
@@ -802,14 +719,14 @@ fail:
 /* Every workspace gets an execution context of its own (a parked one when a finished workspace left one): its stream,
  * events, timers and free lists, so that workspaces of different threads solve concurrently. */
 ScsWork *scs_init(const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
-  DevMats dm;
+  B200DevMats dm;
   ScsWork *w;
   B200Ctx *ctx = d && k && stgs ? b200_ctx_create() : SCS_NULL, *prev = b200_ctx_enter(ctx);
   memset(&dm, 0, sizeof(dm));
   w = init_work(d, k, stgs, b200_comm_nranks() > 1 ? SCS_NULL : &dm, 0, ctx);
   if (dm.Ap) { /* uploaded (a refused input never reaches the GPU): free only once the builder's kernels have run */
     b200_sync();
-    dev_mats_free(&dm);
+    b200_dev_mats_free(&dm);
   }
   b200_ctx_leave(prev);
   if (!w) b200_ctx_release(ctx);
@@ -1559,7 +1476,7 @@ static int update_bc_dev(ScsWork *w) {
 /* the linear-system workspace from dm's blocks: both operators of A; with P, the structure of the full P, the
  * P-aware equilibration on the device and then P's operator and diagonal; with P = 0, b200_equilibrate_dev on the
  * built pair */
-static int build_ops_dev(ScsWork *w, DevMats *dm) {
+static int build_ops_dev(ScsWork *w, B200DevMats *dm) {
   const int n = w->n, m = w->m;
   B200Spmv *A = SCS_NULL, *At = SCS_NULL, *P = SCS_NULL;
   int *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL;
@@ -1611,7 +1528,7 @@ static int dev_to_host(void **dst, const void *d_src, size_t bytes) {
 static void write_data_dev(const char *filename, const ScsData *d, const ScsCone *k, const ScsSettings *stgs) {
   ScsData hd = *d;
   ScsMatrix hA = *d->A, hP;
-  const long long nnzA = read_dev_int(d->A->p + d->A->n), nnzP = d->P ? read_dev_int(d->P->p + d->P->n) : 0;
+  const long long nnzA = b200_read_dev_int(d->A->p + d->A->n), nnzP = d->P ? b200_read_dev_int(d->P->p + d->P->n) : 0;
   int ok = dev_to_host((void **)&hA.p, d->A->p, ((size_t)d->n + 1) * sizeof(scs_int)) == 0 &&
            dev_to_host((void **)&hA.i, d->A->i, (size_t)nnzA * sizeof(scs_int)) == 0 &&
            dev_to_host((void **)&hA.x, d->A->x, (size_t)nnzA * 8) == 0 &&
@@ -1633,21 +1550,8 @@ static void write_data_dev(const char *filename, const ScsData *d, const ScsCone
   free(hA.p); free(hA.i); free(hA.x); free(hP.p); free(hP.i); free(hP.x); free(hd.b); free(hd.c);
 }
 
-/* a device pointer of the library's device, else a message and 0 */
-static int dev_ptr_ok(const void *p, const char *what) {
-  if (b200_is_device_ptr(p)) return 1;
-  printf("ERROR: %s must point to device memory of the library's CUDA device\n", what);
-  return 0;
-}
-static int single_gpu(void) {
-  if (b200_comm_nranks() <= 1) return 1;
-  printf("ERROR: the device-data entry points drive a single GPU; this process is one of %d ranks\n",
-         b200_comm_nranks());
-  return 0;
-}
-
 static ScsWork *init_device(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, void *stream, B200Ctx *ctx) {
-  DevMats dm;
+  B200DevMats dm;
   ScsWork *w;
   memset(&dm, 0, sizeof(dm));
   if (!d || !k || !stgs) {
@@ -1658,19 +1562,19 @@ static ScsWork *init_device(const ScsData *d, const ScsCone *k, const ScsSetting
     printf("ERROR: scs_b200 needs an sm_90 (H100) CUDA device: %s\n", b200_last_error());
     return SCS_NULL;
   }
-  if (!single_gpu()) return SCS_NULL;
-  if ((d->A && ((d->A->p && !dev_ptr_ok(d->A->p, "A->p")) || (d->A->i && !dev_ptr_ok(d->A->i, "A->i")) ||
-                (d->A->x && !dev_ptr_ok(d->A->x, "A->x")))) ||
-      (d->P && ((d->P->p && !dev_ptr_ok(d->P->p, "P->p")) || (d->P->i && !dev_ptr_ok(d->P->i, "P->i")) ||
-                (d->P->x && !dev_ptr_ok(d->P->x, "P->x")))) ||
-      (d->b && !dev_ptr_ok(d->b, "b")) || (d->c && !dev_ptr_ok(d->c, "c"))) {
+  if (!b200_single_gpu()) return SCS_NULL;
+  if ((d->A && ((d->A->p && !b200_dev_ptr_ok(d->A->p, "A->p")) || (d->A->i && !b200_dev_ptr_ok(d->A->i, "A->i")) ||
+                (d->A->x && !b200_dev_ptr_ok(d->A->x, "A->x")))) ||
+      (d->P && ((d->P->p && !b200_dev_ptr_ok(d->P->p, "P->p")) || (d->P->i && !b200_dev_ptr_ok(d->P->i, "P->i")) ||
+                (d->P->x && !b200_dev_ptr_ok(d->P->x, "P->x")))) ||
+      (d->b && !b200_dev_ptr_ok(d->b, "b")) || (d->c && !b200_dev_ptr_ok(d->c, "c"))) {
     printf("ERROR: Validation returned failure\n");
     return SCS_NULL;
   }
   if (!ctx || b200_wait_for_caller(stream) != 0) return SCS_NULL;
   w = init_work(d, k, stgs, &dm, 1, ctx);
   b200_sync(); /* the builder's blocks are free only once its kernels have run */
-  dev_mats_free(&dm);
+  b200_dev_mats_free(&dm);
   b200_caller_waits(stream);
   return w;
 }
@@ -1685,7 +1589,7 @@ ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSetti
 static scs_int update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream) {
   const int n = w ? w->n : 0, m = w ? w->m : 0;
   int rc = -1;
-  if (!w || !single_gpu() || (d_b && !dev_ptr_ok(d_b, "b")) || (d_c && !dev_ptr_ok(d_c, "c"))) return -1;
+  if (!w || !b200_single_gpu() || (d_b && !b200_dev_ptr_ok(d_b, "b")) || (d_c && !b200_dev_ptr_ok(d_c, "c"))) return -1;
   if (b200_wait_for_caller(stream) != 0) return -1;
   do {
     if (!w->d_b_orig) w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
@@ -1722,14 +1626,14 @@ static scs_int update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMat
   const double t0 = now_ms();
   double t_mark = t0;
   const int n = w ? w->n : 0, m = w ? w->m : 0;
-  DevMats dm;
+  B200DevMats dm;
   int *Tp = SCS_NULL, *Ti = SCS_NULL, *Fp = SCS_NULL, *Fi = SCS_NULL, *Fsrc = SCS_NULL;
   double *Tx = SCS_NULL, *Fx = SCS_NULL;
   unsigned *d_bad = SCS_NULL, bad = ~0u;
   int rc = -1;
   memset(&dm, 0, sizeof(dm));
   if (!w) { printf("ERROR: missing ScsWork input\n"); return -1; }
-  if (!single_gpu()) return -1;
+  if (!b200_single_gpu()) return -1;
   if (!A) { printf("ERROR: A matrix missing\n"); return -1; }
   if (P && !w->p->P) { printf("ERROR: P is given, but the workspace was built without P\n"); return -1; }
   if (!P && w->p->P) { printf("ERROR: the workspace was built with P, and no P is given\n"); return -1; }
@@ -1741,15 +1645,15 @@ static scs_int update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMat
     printf("ERROR: P is %li x %li; the workspace was built for %i x %i\n", (long)P->m, (long)P->n, n, n);
     return -1;
   }
-  if ((A->p && !dev_ptr_ok(A->p, "A->p")) || (A->i && !dev_ptr_ok(A->i, "A->i")) ||
-      (A->x && !dev_ptr_ok(A->x, "A->x")) ||
-      (P && ((P->p && !dev_ptr_ok(P->p, "P->p")) || (P->i && !dev_ptr_ok(P->i, "P->i")) ||
-             (P->x && !dev_ptr_ok(P->x, "P->x")))))
+  if ((A->p && !b200_dev_ptr_ok(A->p, "A->p")) || (A->i && !b200_dev_ptr_ok(A->i, "A->i")) ||
+      (A->x && !b200_dev_ptr_ok(A->x, "A->x")) ||
+      (P && ((P->p && !b200_dev_ptr_ok(P->p, "P->p")) || (P->i && !b200_dev_ptr_ok(P->i, "P->i")) ||
+             (P->x && !b200_dev_ptr_ok(P->x, "P->x")))))
     return -1;
   if (b200_wait_for_caller(stream) != 0) return -1;
   do {
     /* 1. everything is checked before the first write to a resident array */
-    if (validate_matrix_dev(A, P, &dm) != 0) { printf("invalid linear system input data\n"); break; }
+    if (b200_validate_matrix_dev(A, P, &dm) != 0) { printf("invalid linear system input data\n"); break; }
     if (dm.nnzA != w->nnzA) { pattern_differs("A"); break; }
     if (P && (dm.nnzP != w->nnzP || dm.fullP != b200_spmv_nnz(w->p->P))) { pattern_differs("P"); break; }
     init_mark("update: validating copy", &t_mark);
@@ -1843,7 +1747,7 @@ static scs_int update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMat
   b200_sync();
   b200_free(Tp); b200_free(Ti); b200_free(Tx); b200_free(d_bad);
   b200_free(Fp); b200_free(Fi); b200_free(Fsrc); b200_free(Fx);
-  dev_mats_free(&dm);
+  b200_dev_mats_free(&dm);
   if (rc == 0) w->setup_time = now_ms() - t0;
   b200_caller_waits(stream);
   return rc;
@@ -1861,8 +1765,8 @@ static scs_int solve_device(ScsWork *w, ScsSolution *d_sol, ScsInfo *info, scs_i
     printf("ERROR: missing ScsWork, ScsSolution or ScsInfo input\n");
     return -1;
   }
-  if (!single_gpu() || !dev_ptr_ok(d_sol->x, "sol->x") || !dev_ptr_ok(d_sol->y, "sol->y") ||
-      !dev_ptr_ok(d_sol->s, "sol->s"))
+  if (!b200_single_gpu() || !b200_dev_ptr_ok(d_sol->x, "sol->x") || !b200_dev_ptr_ok(d_sol->y, "sol->y") ||
+      !b200_dev_ptr_ok(d_sol->s, "sol->s"))
     return -1;
   if (b200_wait_for_caller(stream) != 0) return -1;
   w->sol_on_dev = 1;

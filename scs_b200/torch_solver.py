@@ -93,6 +93,14 @@ def _iptr(t, T):
     return C.cast(C.c_void_p(t.data_ptr()), T.int_p)
 
 
+def _matrix(M, T, keep):
+    """the ScsMatrix (struct classes T) of a CUDA sparse-CSC tensor, pointing into its arrays; the contiguous arrays
+    are appended to `keep`, which must outlive the call that reads them"""
+    p, i, x = M.ccol_indices().contiguous(), M.row_indices().contiguous(), M.values().contiguous()
+    keep.extend((p, i, x))
+    return T.ScsMatrix(_dptr(x), _iptr(i, T), _iptr(p, T), M.shape[0], M.shape[1])
+
+
 class SCS:
     """A problem resident on the GPU (scs_b200_init_device), solved and updated in place there."""
 
@@ -106,14 +114,8 @@ class SCS:
         T = capi.abi(self._long)
         self._T = T
         self._keep = []  # the tensors the structs point into, alive as long as the call needs them
-
-        def mat(M):
-            p, i, x = M.ccol_indices().contiguous(), M.row_indices().contiguous(), M.values().contiguous()
-            self._keep += [p, i, x]
-            return T.ScsMatrix(_dptr(x), _iptr(i, T), _iptr(p, T), M.shape[0], M.shape[1])
-
-        A = mat(data["A"])
-        P = mat(data["P"]) if data.get("P") is not None else None
+        A = _matrix(data["A"], T, self._keep)
+        P = _matrix(data["P"], T, self._keep) if data.get("P") is not None else None
         b, c = data["b"].contiguous(), data["c"].contiguous()
         self._keep += [b, c]
         d = T.ScsData(self.m, self.n, C.pointer(A), C.pointer(P) if P is not None else C.POINTER(T.ScsMatrix)(),
@@ -159,13 +161,8 @@ class SCS:
                                      f"got {M.ccol_indices().dtype}")
                 _check_device(name, M, self.device.index)
             keep = []
-
-            def mat(M):
-                p, i, x = M.ccol_indices().contiguous(), M.row_indices().contiguous(), M.values().contiguous()
-                keep.extend((p, i, x))
-                return self._T.ScsMatrix(_dptr(x), _iptr(i, self._T), _iptr(p, self._T), M.shape[0], M.shape[1])
-            Am = mat(A)
-            Pm = mat(P) if P is not None else None
+            Am = _matrix(A, self._T, keep)
+            Pm = _matrix(P, self._T, keep) if P is not None else None
             rc = self._lib.scs_b200_update_matrix_device(self._work, C.byref(Am),
                                                          C.byref(Pm) if Pm is not None else None, self._stream())
             if rc != 0:
