@@ -281,7 +281,8 @@ scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int r
  * D is the row scaling of the equilibrated problem (length m) or NULL
  * (reference normalize_box_cone, cones.c:1160-1177).  x (length m) and r_y
  * (length m or NULL) are HOST arrays; x is projected in place onto the dual
- * cone under the R-metric. Returns 0, or <0 on failure. */
+ * cone under the R-metric. Returns 0, or <0 on failure. scs_b200_init_cone checks the cone as
+ * scs_init does, for m rows, and refuses it (NULL) with scs_init's message before any device work. */
 ScsB200ConeWork *scs_b200_init_cone(const ScsCone *k, scs_int m,
                                     const scs_float *D);
 scs_int scs_b200_proj_dual_cone(ScsB200ConeWork *c, scs_float *x,

@@ -81,8 +81,8 @@ int b200_equilibrate_qp_dev(B200Spmv *A_rows, B200Spmv *A_cols, const int *d_Pp,
                             const int *d_Fp, const int *d_Fi, const int *d_Fsrc, const int *bnd, int nbnd,
                             double *d_D, double *d_E);
 /* b = b_orig * D, c = c_orig * E (D, E NULL: plain copies); h_max (host, 4) receives max |b_orig|, max |b|,
- * max |c_orig|, max |c| (synchronises). b200_scale_b_c then multiplies both by sigma: together the device form of
- * host/equilibrate.c b200_normalize_b_c, bit for bit */
+ * max |c_orig|, max |c| (synchronises; NaN entries are skipped). b200_scale_b_c then multiplies both by sigma:
+ * together the reference's normalize_b_c (src/normalize.c:33-61), the only normaliser of b and c */
 int b200_normalize_b_c_dev(int m, int n, const double *d_b_orig, const double *d_c_orig, const double *d_D,
                            const double *d_E, double *d_b, double *d_c, double *h_max);
 int b200_scale_b_c(int m, int n, double *d_b, double *d_c, double sigma);
@@ -90,7 +90,7 @@ int b200_rescale_dev(B200Spmv *M, const double *d_rowscale, const double *d_cols
 
 /* ---------------------------------------------------------------- cones (kernels/cones.cu) */
 typedef struct B200Cones B200Cones;
-/* k_* arrays are HOST arrays; box bounds already scaled (normalize_box_cone). */
+/* k_* arrays are HOST arrays; box bounds already scaled (b200_normalize_box). */
 B200Cones *b200_cones_create(int m, int nz, int nl, int bsize, const double *h_bl,
                              const double *h_bu, int qsize, const int *h_q, int ssize,
                              const int *h_s);

@@ -29,18 +29,6 @@
 #define DIV_EPS_TOL (1E-18)
 #define SAFEDIV_POS(X, Y) ((Y) < DIV_EPS_TOL ? ((X) / DIV_EPS_TOL) : (X) / (Y))
 
-#ifdef USE_SPECTRAL_CONES
-/* rows of the spectral cones (reference cones.c:435-443); a log-det cone of order d has d(d+1)/2 + 2 */
-static inline long long b200_spectral_rows(const ScsCone *k) {
-  long long rows = 0;
-  scs_int i;
-  for (i = 0; i < k->dsize; ++i) rows += (long long)k->d[i] * (k->d[i] + 1) / 2 + 2;
-  for (i = 0; i < k->nucsize; ++i) rows += (long long)k->nuc_m[i] * k->nuc_n[i] + 1;
-  for (i = 0; i < k->ell1_size; ++i) rows += (long long)k->ell1[i] + 1;
-  for (i = 0; i < k->sl_size; ++i) rows += (long long)k->sl_n[i] * (k->sl_n[i] + 1) / 2 + 1;
-  return rows;
-}
-#endif
 #ifndef MAX
 #define MAX(a, b) (((a) > (b)) ? (a) : (b))
 #endif
@@ -62,12 +50,11 @@ struct SCS_WORK {
   double setup_time;
   int time_limit_reached;
   /* host copies */
-  ScsData *d;       /* deep copy, A/P/b/c NORMALISED */
+  ScsData *d;       /* m, n; A/P deep copies, NORMALISED, only where several GPUs equilibrate on the host */
   ScsCone *k;       /* deep copy, box bounds normalised */
   ScsSettings *stgs;
   double *D, *E;    /* equilibration (NULL when normalize == 0) */
   double primal_scale, dual_scale;
-  double *b_orig, *c_orig;
   double nm_b_orig, nm_c_orig;
   double *h_diag_r; /* l */
   int *cone_boundaries;
@@ -96,14 +83,12 @@ struct SCS_WORK {
    * iterates are copied to the host every iteration and every column is recomputed there */
   char *log_csv_name; /* deep copy of ScsSettings.log_csv_filename */
   FILE *log_csv_fout; /* opened ("w") at the start of every scs_solve, closed at its end (rw.c:686-705) */
-  double *log_host; /* scratch: u, u_t, v, v_prev, rsk (l each), ax (m), aty (n), px (n) */
-  /* device-data entry points (scs_b200_*_device): b_orig, c_orig on the device (NULL until a device call needs them);
-   * *_on_dev = the device copy is the current one and the host copy stale; bc_host_stale = d->b, d->c (host) are
-   * stale; sol_on_dev = the ScsSolution of the running solve holds device pointers */
+  double *log_host; /* scratch: u, u_t, v, v_prev, rsk (l each), ax (m), aty (n), px (n), b (m), c (n) */
+  /* b and c as given, through either door: the only copy of them; d_b, d_c are normalised from these (update_bc_dev) */
   double *d_b_orig, *d_c_orig;
-  int b_on_dev, c_on_dev, bc_host_stale, sol_on_dev;
+  int sol_on_dev; /* the ScsSolution of the running solve holds device pointers */
   /* what init decided and the solves overwrite, kept for scs_b200_update_matrix_device: the equilibration it used
-   * (B200_EQUIL_*), the initial scale, and the box bounds as given (normalize_box_cone scales k->bl / k->bu) */
+   * (B200_EQUIL_*), the initial scale, and the box bounds as given (b200_normalize_box scales k->bl / k->bu) */
   int equil;
   double scale0;
   double *bl_orig, *bu_orig;
@@ -123,6 +108,13 @@ int b200_cone_ints(const ScsCone *k, B200ConeInts *c); /* 0, or -1 (out of memor
 void b200_cone_ints_free(B200ConeInts *c);
 
 int b200_equilibrate(ScsMatrix *P, ScsMatrix *A, const int *bnd, int nbnd, double *D, double *E);
-double b200_normalize_b_c(int m, int n, const double *D, const double *E, double *b, double *c);
+
+/* the cone setup of scs_init and scs_b200_init_cone (host/cone_setup.c). b200_validate_cones: 0, or -1 after printing
+ * the reference's message, before any device work. b200_normalize_box: bl, bu (k's box bounds or copies of them)
+ * scaled in place by the row scaling D (m entries; NULL: left as they are). b200_cones_build: the device cone
+ * workspace of a validated k with box bounds bl, bu, or NULL. */
+int b200_validate_cones(const ScsCone *k, scs_int m);
+void b200_normalize_box(const ScsCone *k, const double *D, double *bl, double *bu);
+B200Cones *b200_cones_build(const ScsCone *k, scs_int m, const double *bl, const double *bu);
 
 #endif

@@ -1,13 +1,12 @@
-/* equilibrate.c -- Ruiz + L2 equilibration of A and P on the host at setup,
- * and the b/c scaling.  Setup path (runs once per scs_init), not part of the
- * per-iteration hot loop. The matrix equilibration serves the multi-GPU path
- * with P != 0 only; one GPU runs its device form, b200_equilibrate_qp_dev
- * (kernels/equil.cu), with the same bits.
+/* equilibrate.c -- Ruiz + L2 equilibration of A and P on the host at setup.
+ * Setup path (runs once per scs_init), not part of the per-iteration hot
+ * loop. It serves the multi-GPU path with P != 0 only; one GPU runs its
+ * device form, b200_equilibrate_qp_dev (kernels/equil.cu), with the same bits.
  *
  * Same algorithm and constants as reference linsys/scs_matrix.c:229-496
  * (compute_ruiz_mats / compute_l2_mats / rescale / normalize_a_p: 25 Ruiz
  * passes + 1 L2 pass, limits 1e-4 / 1e4, D constant inside every cone of
- * size > 1) and src/normalize.c:33-61 (normalize_b_c).
+ * size > 1).
  */
 #include "driver.h"
 #include <math.h>
@@ -153,25 +152,4 @@ int b200_equilibrate(ScsMatrix *P, ScsMatrix *A, const int *bnd, int nbnd, doubl
   free(Dt);
   free(Et);
   return 0;
-}
-
-/* b *= D, c *= E, sigma = 1/clip(max(|b|_inf, |c|_inf)); returns sigma (normalize.c:33-61) */
-double b200_normalize_b_c(int m, int n, const double *D, const double *E, double *b, double *c) {
-  int i;
-  double nm_c = 0.0, nm_b = 0.0, sigma;
-  for (i = 0; i < n; ++i) {
-    c[i] *= E[i];
-    if (fabs(c[i]) > nm_c) nm_c = fabs(c[i]);
-  }
-  for (i = 0; i < m; ++i) {
-    b[i] *= D[i];
-    if (fabs(b[i]) > nm_b) nm_b = fabs(b[i]);
-  }
-  sigma = nm_c > nm_b ? nm_c : nm_b;
-  sigma = sigma < MIN_NORMALIZATION_FACTOR ? 1.0 : sigma;
-  sigma = sigma > MAX_NORMALIZATION_FACTOR ? MAX_NORMALIZATION_FACTOR : sigma;
-  sigma = SAFEDIV_POS(1.0, sigma);
-  for (i = 0; i < n; ++i) c[i] *= sigma;
-  for (i = 0; i < m; ++i) b[i] *= sigma;
-  return sigma;
 }

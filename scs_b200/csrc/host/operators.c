@@ -27,80 +27,28 @@ static void cone_free(ScsB200ConeWork *c) {
 static ScsB200ConeWork *init_cone(const ScsCone *k, scs_int m, const scs_float *D) {
   ScsB200ConeWork *c;
   double *bl = SCS_NULL, *bu = SCS_NULL;
-  scs_int j;
-  long long dims;
-  B200ConeInts ci;
   if (!k || m <= 0) return SCS_NULL;
-  if (b200_over_dim("m", -1, m) || b200_cone_over_limits(k)) return SCS_NULL; /* in scs_int width, before narrowing */
-  if (k->cssize < 0 || (k->cssize > 0 && !k->cs)) return SCS_NULL;
-  if (k->ep < 0 || k->ed < 0 || k->psize < 0 || (k->psize > 0 && !k->p)) return SCS_NULL;
-  dims = (long long)k->z + k->l + k->bsize;
-  for (j = 0; j < k->qsize; ++j) dims += k->q[j];
-  for (j = 0; j < k->ssize; ++j) dims += ((long long)k->s[j] * (k->s[j] + 1)) / 2;
-  for (j = 0; j < k->cssize; ++j) dims += (long long)k->cs[j] * k->cs[j];
-  dims += 3LL * ((long long)k->ep + k->ed + k->psize);
-#ifdef USE_SPECTRAL_CONES
-  if (k->dsize < 0 || k->nucsize < 0 || k->ell1_size < 0 || k->sl_size < 0) return SCS_NULL;
-  if ((k->dsize > 0 && !k->d) || (k->nucsize > 0 && (!k->nuc_m || !k->nuc_n)) || (k->ell1_size > 0 && !k->ell1) ||
-      (k->sl_size > 0 && (!k->sl_n || !k->sl_k)))
-    return SCS_NULL;
-  for (j = 0; j < k->dsize; ++j)
-    if (k->d[j] < 1) return SCS_NULL;
-  for (j = 0; j < k->nucsize; ++j)
-    if (k->nuc_m[j] < 1 || k->nuc_n[j] < 1 || k->nuc_n[j] > k->nuc_m[j]) return SCS_NULL;
-  for (j = 0; j < k->ell1_size; ++j)
-    if (k->ell1[j] < 1) return SCS_NULL;
-  for (j = 0; j < k->sl_size; ++j)
-    if (k->sl_k[j] <= 0 || k->sl_k[j] >= k->sl_n[j]) return SCS_NULL;
-  dims += b200_spectral_rows(k);
-#endif
-  if (dims != m) {
-    fprintf(stderr, "scs_b200: cone dims %lld != m %lld\n", dims, (long long)m);
-    return SCS_NULL;
-  }
+  if (b200_over_dim("m", -1, m) || b200_validate_cones(k, m) != 0) return SCS_NULL; /* before any device work */
   c = (ScsB200ConeWork *)calloc(1, sizeof(*c));
   if (!c) return SCS_NULL;
   c->ctx = b200_ctx_bound();
   c->m = (int)m;
-  if (k->bsize > 1) {
-    /* box bounds follow the row scaling (reference normalize_box_cone, cones.c:1160-1177);
-     * as in the reference, the +-1e15 -> inf mapping only happens when a scaling is given */
-    const double *Db = D ? D + k->z + k->l : SCS_NULL;
+  if (k->bsize > 1) { /* the caller's bounds stay as given */
     bl = (double *)malloc((size_t)(k->bsize - 1) * 8);
     bu = (double *)malloc((size_t)(k->bsize - 1) * 8);
     if (!bl || !bu) goto fail;
-    for (j = 0; j < k->bsize - 1; ++j) {
-      bl[j] = k->bl[j];
-      bu[j] = k->bu[j];
-      if (Db) {
-        const double factor = Db[j + 1] / Db[0];
-        if (bu[j] >= MAX_BOX_VAL) bu[j] = INFINITY; else bu[j] *= factor;
-        if (bl[j] <= -MAX_BOX_VAL) bl[j] = -INFINITY; else bl[j] *= factor;
-      }
-    }
+    memcpy(bl, k->bl, (size_t)(k->bsize - 1) * 8);
+    memcpy(bu, k->bu, (size_t)(k->bsize - 1) * 8);
+    b200_normalize_box(k, D, bl, bu);
   }
-  if (b200_cone_ints(k, &ci) != 0) goto fail; /* int copies for the kernel layer */
-  c->cones = b200_cones_create(c->m, (int)k->z, (int)k->l, (int)k->bsize, bl, bu, (int)k->qsize, ci.q, (int)k->ssize,
-                               ci.s);
-  free(bl);
-  free(bu);
-  bl = bu = SCS_NULL;
-  if (!c->cones) goto fail_ints;
-#ifdef USE_SPECTRAL_CONES
-  if (b200_cones_set_spectral(c->cones, (int)k->dsize, ci.d, (int)k->nucsize, ci.nuc_m, ci.nuc_n, (int)k->ell1_size, ci.ell1,
-                              (int)k->sl_size, ci.sl_n, ci.sl_k) != 0)
-    goto fail_ints;
-#endif
-  if (b200_cones_set_triples(c->cones, (int)k->ep, (int)k->ed, (int)k->psize, k->p) != 0) goto fail_ints;
-  if (b200_cones_set_complex_psd(c->cones, (int)k->cssize, ci.cs, (int)(k->ep + k->ed + k->psize)) != 0)
-    goto fail_ints;
-  b200_cone_ints_free(&ci);
+  c->cones = b200_cones_build(k, m, bl, bu);
+  if (!c->cones) goto fail;
   c->d_x = (double *)b200_malloc((size_t)m * 8);
   c->d_ry = (double *)b200_malloc((size_t)m * 8);
   if (!c->d_x || !c->d_ry) goto fail;
+  free(bl);
+  free(bu);
   return c;
-fail_ints:
-  b200_cone_ints_free(&ci);
 fail:
   free(bl);
   free(bu);

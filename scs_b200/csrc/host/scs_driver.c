@@ -55,8 +55,6 @@ void scs_set_default_settings(ScsSettings *stgs) {
   stgs->time_limit_secs = 0.;
 }
 
-static scs_int sd_size(scs_int s) { return (s * (s + 1)) / 2; }
-
 /* ----------------------------------------------------------------- validation */
 /* Every count is read in scs_int width: nnz(A) is checked against the operator limit before i[] or x[] is read, and a
  * 64-bit index that would truncate to a valid int (2^32 + 3 -> 3) fails the range checks. */
@@ -126,108 +124,6 @@ static int dev_mats_from_host(const ScsMatrix *A, const ScsMatrix *P, B200DevMat
   }
   return 0;
 }
-static int validate_cones(const ScsData *d, const ScsCone *k) {
-  scs_int i;
-  long long dims;
-  if (b200_cone_over_limits(k)) return -1; /* every count and size below 2^30, before any sum of them */
-  if (k->z < 0) { printf("free cone dimension error\n"); return -1; }
-  if (k->l < 0) { printf("lp cone dimension error\n"); return -1; }
-  if (k->bsize < 0) { printf("box cone dimension error\n"); return -1; }
-  if (k->bsize > 1) {
-    if (!k->bl || !k->bu) { printf("box cone bounds missing\n"); return -1; }
-    for (i = 0; i < k->bsize - 1; ++i) {
-      if (isnan(k->bl[i]) || isnan(k->bu[i])) { printf("box cone bounds cannot be NaN\n"); return -1; }
-      if (k->bl[i] == INFINITY || k->bu[i] == -INFINITY) {
-        printf("box cone bounds use invalid infinity direction\n");
-        return -1;
-      }
-      if (k->bl[i] > k->bu[i]) {
-        printf("infeasible: box lower bound larger than upper bound\n");
-        return -1;
-      }
-    }
-  }
-  if (k->qsize < 0 || (k->qsize > 0 && !k->q)) { printf("soc cone dimension error\n"); return -1; }
-  for (i = 0; i < k->qsize; ++i)
-    if (k->q[i] < 0) { printf("soc cone dimension error\n"); return -1; }
-  if (k->ssize < 0 || (k->ssize > 0 && !k->s)) { printf("sd cone dimension error\n"); return -1; }
-  for (i = 0; i < k->ssize; ++i)
-    if (k->s[i] < 0) { printf("sd cone dimension error\n"); return -1; }
-  if (k->cssize < 0 || k->ed < 0 || k->ep < 0 || k->psize < 0) {
-    printf("cone dimension error\n");
-    return -1;
-  }
-  if (k->cssize > 0) {
-    if (!k->cs) { printf("complex sd cone array missing\n"); return -1; }
-    for (i = 0; i < k->cssize; ++i)
-      if (k->cs[i] < 0) { printf("complex sd cone dimension error\n"); return -1; }
-  }
-  if (k->psize > 0) { /* reference cones.c:678-690 */
-    if (!k->p) { printf("power cone array missing\n"); return -1; }
-    for (i = 0; i < k->psize; ++i)
-      if (!isfinite(k->p[i]) || k->p[i] < -1 || k->p[i] > 1) { printf("power cone error, values must be in [-1,1]\n"); return -1; }
-  }
-#ifdef USE_SPECTRAL_CONES /* reference cones.c:690-754 */
-  if (k->dsize < 0 || (k->dsize > 0 && !k->d)) { printf("logdet cone dimension error\n"); return -1; }
-  for (i = 0; i < k->dsize; ++i)
-    if (k->d[i] < 1) { printf("logdet cone dimension error\n"); return -1; }
-  if (k->nucsize < 0) { printf("nuclear cone dimension error\n"); return -1; }
-  if (k->nucsize > 0 && (!k->nuc_m || !k->nuc_n)) { printf("nuclear cone arrays missing\n"); return -1; }
-  for (i = 0; i < k->nucsize; ++i)
-    if (k->nuc_m[i] < 1 || k->nuc_n[i] < 1 || k->nuc_n[i] > k->nuc_m[i]) {
-      printf("nuclear norm cone dimension error\n");
-      return -1;
-    }
-  if (k->ell1_size < 0) { printf("ell1 cone dimension error\n"); return -1; }
-  if (k->ell1_size > 0 && !k->ell1) { printf("ell1 cone array missing\n"); return -1; }
-  for (i = 0; i < k->ell1_size; ++i)
-    if (k->ell1[i] < 1) { printf("ell1 cone dimension error\n"); return -1; }
-  if (k->sl_size < 0) { printf("sum-of-largest-eigenvalues cone dimension error\n"); return -1; }
-  if (k->sl_size > 0 && (!k->sl_n || !k->sl_k)) { printf("sum-of-largest-eigenvalues cone arrays missing\n"); return -1; }
-  for (i = 0; i < k->sl_size; ++i)
-    if (k->sl_k[i] >= k->sl_n[i] || k->sl_k[i] <= 0) {
-      printf("sum-of-largest-eigenvalues cone dimension error\n");
-      return -1;
-    }
-#endif
-  dims = (long long)k->z + k->l + k->bsize;
-  for (i = 0; i < k->qsize; ++i) dims += k->q[i];
-  for (i = 0; i < k->ssize; ++i) dims += sd_size(k->s[i]);
-  for (i = 0; i < k->cssize; ++i) dims += (long long)k->cs[i] * k->cs[i];
-  dims += 3LL * ((long long)k->ep + k->ed + k->psize);
-#ifdef USE_SPECTRAL_CONES
-  dims += b200_spectral_rows(k);
-#endif
-  if (dims != d->m) {
-#ifdef USE_SPECTRAL_CONES
-    /* name the spectral families: a wrong cone array usually comes from one of them */
-    {
-      static const char *names[4] = {"log-det", "nuclear-norm", "l1-norm", "sum-of-largest-eigenvalues"};
-      long long rows[4] = {0, 0, 0, 0};
-      scs_int counts[4];
-      int f, first = 1;
-      for (i = 0; i < k->dsize; ++i) rows[0] += (long long)k->d[i] * (k->d[i] + 1) / 2 + 2;
-      for (i = 0; i < k->nucsize; ++i) rows[1] += (long long)k->nuc_m[i] * k->nuc_n[i] + 1;
-      for (i = 0; i < k->ell1_size; ++i) rows[2] += (long long)k->ell1[i] + 1;
-      for (i = 0; i < k->sl_size; ++i) rows[3] += (long long)k->sl_n[i] * (k->sl_n[i] + 1) / 2 + 1;
-      counts[0] = k->dsize; counts[1] = k->nucsize; counts[2] = k->ell1_size; counts[3] = k->sl_size;
-      printf("Error: Cone dims %li != rows in A %li", (long)dims, (long)d->m);
-      for (f = 0; f < 4; ++f) {
-        if (counts[f] == 0) continue;
-        printf("%s%lli rows in %lli %s cone%s", first ? " (spectral: " : ", ", rows[f], (long long)counts[f],
-               names[f], counts[f] == 1 ? "" : "s");
-        first = 0;
-      }
-      printf("%s\n", first ? "" : ")");
-    }
-#else
-    printf("Error: Cone dims %li != rows in A %li\n", (long)dims, (long)d->m);
-#endif
-    return -1;
-  }
-  return 0;
-}
-
 static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs, B200DevMats *dm) {
   if (d->m <= 0 || d->n <= 0) {
     printf("m and n must both be greater than 0; m = %li, n = %li\n", (long)d->m, (long)d->n);
@@ -243,7 +139,7 @@ static int validate(const ScsData *d, const ScsCone *k, const ScsSettings *stgs,
     printf("invalid linear system input data\n");
     return -1;
   }
-  if (validate_cones(d, k) < 0) { printf("cone validation error\n"); return -1; }
+  if (b200_validate_cones(k, d->m) < 0) { printf("cone validation error\n"); return -1; }
   if (stgs->max_iters <= 0) { printf("max_iters must be positive\n"); return -1; }
   if (!isfinite(stgs->eps_abs) || stgs->eps_abs < 0) { printf("eps_abs tolerance must be a nonnegative finite number\n"); return -1; }
   if (!isfinite(stgs->eps_rel) || stgs->eps_rel < 0) { printf("eps_rel tolerance must be a nonnegative finite number\n"); return -1; }
@@ -331,11 +227,11 @@ static void finish_work(ScsWork *w) {
   init_mark("finish: device vectors", &t_mark);
   b200_host_free(w->h_sc);
   init_mark("finish: pinned scalars", &t_mark);
-  free(w->D); free(w->E); free(w->b_orig); free(w->c_orig); free(w->h_diag_r);
+  free(w->D); free(w->E); free(w->h_diag_r);
   free(w->cone_boundaries);
   free(w->bl_orig); free(w->bu_orig);
   if (w->d) {
-    free_matrix(w->d->A); free_matrix(w->d->P); free(w->d->b); free(w->d->c); free(w->d);
+    free_matrix(w->d->A); free_matrix(w->d->P); free(w->d);
   }
   if (w->k) {
     free(w->k->bu); free(w->k->bl); free(w->k->q); free(w->k->s); free(w->k->p); free(w->k->cs);
@@ -378,66 +274,28 @@ static int set_cone_boundaries(ScsWork *w) {
   if (!b) return -1;
   b[count++] = k->z + k->l + k->bsize;
   for (i = 0; i < k->qsize; ++i) b[count++] = k->q[i];
-  for (i = 0; i < k->ssize; ++i) b[count++] = sd_size(k->s[i]);
+  for (i = 0; i < k->ssize; ++i) b[count++] = k->s[i] * (k->s[i] + 1) / 2;
   for (i = 0; i < k->cssize; ++i) b[count++] = k->cs[i] * k->cs[i];
   for (i = 0; i < k->ep + k->ed + k->psize; ++i) b[count++] = 3; /* every triple shares one D (cones.c:405-408) */
 #ifdef USE_SPECTRAL_CONES /* one D value per spectral cone (cones.c:411-419) */
-  for (i = 0; i < k->dsize; ++i) b[count++] = sd_size(k->d[i]) + 2;
+  for (i = 0; i < k->dsize; ++i) b[count++] = k->d[i] * (k->d[i] + 1) / 2 + 2;
   for (i = 0; i < k->nucsize; ++i) b[count++] = k->nuc_m[i] * k->nuc_n[i] + 1;
   for (i = 0; i < k->ell1_size; ++i) b[count++] = k->ell1[i] + 1;
-  for (i = 0; i < k->sl_size; ++i) b[count++] = sd_size(k->sl_n[i]) + 1;
+  for (i = 0; i < k->sl_size; ++i) b[count++] = k->sl_n[i] * (k->sl_n[i] + 1) / 2 + 1;
 #endif
   w->cone_boundaries = b;
   w->cone_boundaries_len = total + 1;
   return 0;
 }
 
-/* box bounds follow the row scaling (reference cones.c:1160-1177) */
-static void normalize_box_cone(ScsCone *k, const double *D, int bsize) {
-  int j;
-  for (j = 0; j < bsize - 1; j++) {
-    const double factor = D ? D[j + 1] / D[0] : 1.0;
-    if (k->bu[j] >= MAX_BOX_VAL) k->bu[j] = INFINITY; else k->bu[j] *= factor;
-    if (k->bl[j] <= -MAX_BOX_VAL) k->bl[j] = -INFINITY; else k->bl[j] *= factor;
-  }
-}
-
-static scs_int update_work_bc(ScsWork *w, scs_float *b, scs_float *c) {
-  const double t0 = now_ms();
-  const int n = w->n, m = w->m;
-  int i;
-  w->g_valid = 0; /* new normalised b and c */
-  /* originals last set through scs_b200_update_device and kept here: their host copies are brought up to date */
-  if ((!b && w->b_on_dev && b200_d2h(w->b_orig, w->d_b_orig, (size_t)m * 8) != 0) ||
-      (!c && w->c_on_dev && b200_d2h(w->c_orig, w->d_c_orig, (size_t)n * 8) != 0) || b200_sync() != 0)
-    return -1;
-  w->b_on_dev = w->c_on_dev = w->bc_host_stale = 0;
-  if (b) {
-    if (w->b_orig != b) memcpy(w->b_orig, b, (size_t)m * sizeof(double));
-    w->nm_b_orig = 0.0;
-    for (i = 0; i < m; ++i) w->nm_b_orig = MAX(w->nm_b_orig, fabs(w->b_orig[i]));
-  }
-  memcpy(w->d->b, w->b_orig, (size_t)m * sizeof(double));
-  if (c) {
-    if (w->c_orig != c) memcpy(w->c_orig, c, (size_t)n * sizeof(double));
-    w->nm_c_orig = 0.0;
-    for (i = 0; i < n; ++i) w->nm_c_orig = MAX(w->nm_c_orig, fabs(w->c_orig[i]));
-  }
-  memcpy(w->d->c, w->c_orig, (size_t)n * sizeof(double));
-  if (w->D) {
-    const double sigma = b200_normalize_b_c(m, n, w->D, w->E, w->d->b, w->d->c);
-    w->primal_scale = sigma;
-    w->dual_scale = sigma;
-  }
-  if (b200_h2d(w->d_b, w->d->b, (size_t)m * 8) != 0) return -1;
-  if (b200_h2d(w->d_c, w->d->c, (size_t)n * 8) != 0) return -1;
-  if (b200_sync() != 0) return -1;
-  w->setup_time = now_ms() - t0;
-  return 0;
-}
+static int update_bc_dev(ScsWork *w);
+/* the originals given (NULL: the resident one is kept) uploaded, then normalised on the device like every door's */
 scs_int scs_update(ScsWork *w, scs_float *b, scs_float *c) {
   B200Ctx *prev = b200_ctx_enter(w->ctx);
-  const scs_int rc = update_work_bc(w, b, c);
+  scs_int rc = -1;
+  if ((!b || b200_h2d(w->d_b_orig, b, (size_t)w->m * 8) == 0) &&
+      (!c || b200_h2d(w->d_c_orig, c, (size_t)w->n * 8) == 0))
+    rc = update_bc_dev(w);
   b200_ctx_leave(prev);
   return rc;
 }
@@ -463,7 +321,6 @@ static void print_header(const ScsWork *w) {
          (long)w->nnzA, (long)w->nnzP);
 }
 
-static int update_bc_dev(ScsWork *w);
 static int build_ops_dev(ScsWork *w, B200DevMats *dm);
 static void write_data_dev(const char *filename, const ScsData *d, const ScsCone *k, const ScsSettings *stgs);
 
@@ -477,7 +334,6 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   const double t0 = now_ms();
   double t_mark = t0;
   int n, m, i, host_copy;
-  B200ConeInts ci;
   size_t l;
   if (!d || !k || !stgs) {
     printf("ERROR: Missing ScsData, ScsCone, or ScsSettings input\n");
@@ -521,16 +377,10 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   w->equil = !stgs->normalize ? B200_EQUIL_NONE : d->P ? B200_EQUIL_QP : B200_EQUIL_PAIR;
   host_copy = !dm && w->equil != B200_EQUIL_PAIR;
   w->scale0 = stgs->scale;
-  if (dev_data) { /* the host copies of b and c are filled when a host call needs them */
-    w->d->b = (double *)malloc((size_t)m * 8);
-    w->d->c = (double *)malloc((size_t)n * 8);
-    if (!w->d->b || !w->d->c) goto fail;
-  } else {
-    w->d->A = host_copy ? copy_matrix(d->A) : SCS_NULL;
-    w->d->P = host_copy && d->P ? copy_matrix(d->P) : SCS_NULL;
-    w->d->b = (double *)dup_mem(d->b, (size_t)m * 8);
-    w->d->c = (double *)dup_mem(d->c, (size_t)n * 8);
-    if ((host_copy && !w->d->A) || (host_copy && d->P && !w->d->P) || !w->d->b || !w->d->c) goto fail;
+  if (host_copy) {
+    w->d->A = copy_matrix(d->A);
+    w->d->P = d->P ? copy_matrix(d->P) : SCS_NULL;
+    if (!w->d->A || (d->P && !w->d->P)) goto fail;
   }
   *w->k = *k;
   w->k->bu = w->k->bl = SCS_NULL; w->k->q = SCS_NULL; w->k->s = SCS_NULL;
@@ -573,10 +423,8 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
   }
   if (w->stgs->verbose) print_header(w);
 
-  w->b_orig = (double *)malloc((size_t)m * 8);
-  w->c_orig = (double *)malloc((size_t)n * 8);
   w->h_diag_r = (double *)malloc(l * 8);
-  if (!w->b_orig || !w->c_orig || !w->h_diag_r) goto fail;
+  if (!w->h_diag_r) goto fail;
   if (set_cone_boundaries(w) != 0) goto fail;
   set_diag_r_host(w);
 
@@ -589,7 +437,7 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
     if (host_copy) {
       if (b200_equilibrate(w->d->P, w->d->A, w->cone_boundaries, w->cone_boundaries_len, w->D, w->E) != 0)
         goto fail;
-      if (w->k->bsize > 1) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
+      b200_normalize_box(w->k, w->D, w->k->bl, w->k->bu);
     }
   }
 
@@ -659,43 +507,14 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
     if (b200_d2h(w->D, w->d_D, (size_t)m * 8) != 0 || b200_d2h(w->E, w->d_E, (size_t)n * 8) != 0 ||
         b200_sync() != 0)
       goto fail;
-    if (w->k->bsize > 1) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
+    b200_normalize_box(w->k, w->D, w->k->bl, w->k->bu);
     init_mark("init: device equilibration + preconditioner", &t_mark);
   }
-  /* b, c: stores *_orig, normalises, uploads */
-  if (dev_data) {
-    w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
-    w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
-    if (!w->d_b_orig || !w->d_c_orig || b200_d2d(w->d_b_orig, d->b, (size_t)m * 8) != 0 ||
-        b200_d2d(w->d_c_orig, d->c, (size_t)n * 8) != 0)
-      goto fail;
-    w->b_on_dev = w->c_on_dev = 1;
-    if (update_bc_dev(w) != 0) goto fail;
-  } else {
-    memcpy(w->b_orig, d->b, (size_t)m * 8);
-    memcpy(w->c_orig, d->c, (size_t)n * 8);
-    if (update_work_bc(w, w->b_orig, w->c_orig) != 0) goto fail;
-  }
-
-  /* the kernel layer takes int copies of the cone arrays (validated below 2^30) */
-  if (b200_cone_ints(w->k, &ci) != 0) goto fail;
-  w->cones = b200_cones_create(m, (int)w->k->z, (int)w->k->l, (int)w->k->bsize, w->k->bl, w->k->bu,
-                               (int)w->k->qsize, ci.q, (int)w->k->ssize, ci.s);
-#ifdef USE_SPECTRAL_CONES
-  if (w->cones && b200_cones_set_spectral(w->cones, (int)w->k->dsize, ci.d, (int)w->k->nucsize, ci.nuc_m, ci.nuc_n, (int)w->k->ell1_size,
-                                          ci.ell1, (int)w->k->sl_size, ci.sl_n, ci.sl_k) != 0) {
-    printf("ERROR: init_cone failure (spectral cones)\n");
-    b200_cone_ints_free(&ci);
-    goto fail;
-  }
-#endif
-  if (!w->cones || b200_cones_set_triples(w->cones, (int)w->k->ep, (int)w->k->ed, (int)w->k->psize, w->k->p) != 0 ||
-      b200_cones_set_complex_psd(w->cones, (int)w->k->cssize, ci.cs, (int)(w->k->ep + w->k->ed + w->k->psize)) != 0) {
+  w->cones = b200_cones_build(w->k, m, w->k->bl, w->k->bu);
+  if (!w->cones) {
     printf("ERROR: init_cone failure\n");
-    b200_cone_ints_free(&ci);
     goto fail;
   }
-  b200_cone_ints_free(&ci);
   if (!w->p) w->p = scs_init_lin_sys_work(w->d->A, w->d->P, w->h_diag_r);
   if (!w->p) { printf("ERROR: init_lin_sys_work failure\n"); goto fail; }
   if (w->stgs->acceleration_lookback) {
@@ -705,8 +524,18 @@ static ScsWork *init_work(const ScsData *d, const ScsCone *k, const ScsSettings 
                               AA_MAX_WEIGHT_NORM, AA_IR_MAX_STEPS, 0);
     if (!w->accel && w->stgs->verbose) printf("WARN: aa_init returned NULL, no acceleration applied.\n");
   }
+  /* b, c: the originals onto the device, normalised there. Allocated last: placed before the blocks the ADMM loop
+   * streams, their 32 MB at C2 moved those and bench.py ran 0.7 % fewer iterations/s (H100 80GB HBM3, 700 W). */
+  w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
+  w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
+  if (!w->d_b_orig || !w->d_c_orig) goto fail;
+  if (dev_data)
+    i = b200_d2d(w->d_b_orig, d->b, (size_t)m * 8) | b200_d2d(w->d_c_orig, d->c, (size_t)n * 8);
+  else
+    i = b200_h2d(w->d_b_orig, d->b, (size_t)m * 8) | b200_h2d(w->d_c_orig, d->c, (size_t)n * 8);
+  if (i != 0 || update_bc_dev(w) != 0) goto fail;
   if (b200_sync() != 0) goto fail;
-  init_mark("init: b, c, cones, AA workspace", &t_mark);
+  init_mark("init: cones, AA workspace, b, c", &t_mark);
   w->r_orig.last_iter = w->r_norm.last_iter = -1;
   w->setup_time = now_ms() - t0;
   return w;
@@ -1125,27 +954,23 @@ static int log_data_to_csv(ScsWork *w, int iter, double t_solve) {
   const B200Residuals *r = &w->r_orig;
   B200Residuals rn_local, *rn = &rn_local;
   FILE *f = w->log_csv_fout;
-  double *u, *ut, *v, *vp, *rsk, *ax, *aty, *px;
+  double *u, *ut, *v, *vp, *rsk, *ax, *aty, *px, *bv, *cv;
   double acc[16];
   double tau, inv_ds, inv_ps;
   long long i;
   if (!f) return 0;
   if (populate_residual_struct(w, iter) != 0) return -1;
-  if (w->bc_host_stale) { /* set on the device (scs_b200_update_device): a debugging mode may copy them here */
-    if (b200_d2h(w->d->b, w->d_b, (size_t)m * 8) != 0 || b200_d2h(w->d->c, w->d_c, (size_t)n * 8) != 0 ||
-        b200_sync() != 0)
-      return -1;
-    w->bc_host_stale = 0;
-  }
   if (!w->log_host) {
-    w->log_host = (double *)malloc((size_t)(5 * l + m + 2 * (long long)n) * sizeof(double));
+    w->log_host = (double *)malloc((size_t)(5 * l + 2 * (long long)m + 3 * (long long)n) * sizeof(double));
     if (!w->log_host) return -1;
   }
   u = w->log_host; ut = u + l; v = ut + l; vp = v + l; rsk = vp + l; ax = rsk + l; aty = ax + m; px = aty + n;
+  bv = px + n; cv = bv + m;
   if (b200_d2h(u, w->adm.d_u, (size_t)l * 8) != 0 || b200_d2h(ut, w->adm.d_u_t, (size_t)l * 8) != 0 ||
       b200_d2h(v, w->adm.d_v, (size_t)l * 8) != 0 || b200_d2h(vp, w->adm.d_v_prev, (size_t)l * 8) != 0 ||
       b200_d2h(rsk, w->adm.d_rsk, (size_t)l * 8) != 0 || b200_d2h(ax, w->d_ax, (size_t)m * 8) != 0 ||
-      b200_d2h(aty, w->d_aty, (size_t)n * 8) != 0 || b200_sync() != 0)
+      b200_d2h(aty, w->d_aty, (size_t)n * 8) != 0 || b200_d2h(bv, w->d_b, (size_t)m * 8) != 0 ||
+      b200_d2h(cv, w->d_c, (size_t)n * 8) != 0 || b200_sync() != 0)
     return -1;
   if (w->p->P) {
     if (b200_d2h(px, w->d_px, (size_t)n * 8) != 0 || b200_sync() != 0) return -1;
@@ -1187,7 +1012,7 @@ static int log_data_to_csv(ScsWork *w, int iter, double t_solve) {
     for (i = 0; i < n; ++i) {
       const double e = w->E ? w->E[i] : 1.0;
       const double xo = w->E ? u[i] * (e / w->dual_scale) : u[i];
-      const double rr = px[i] + aty[i] + tau * w->d->c[i];
+      const double rr = px[i] + aty[i] + tau * cv[i];
       const double ro = rr * (inv_ps / e);
       if (fabs(xo) > xi) xi = fabs(xo);
       x2 += xo * xo;
@@ -1198,7 +1023,7 @@ static int log_data_to_csv(ScsWork *w, int iter, double t_solve) {
       const double d = w->D ? w->D[i] : 1.0;
       const double yo = w->D ? u[n + i] * (d / w->primal_scale) : u[n + i];
       const double so = w->D ? rsk[n + i] / (d * w->dual_scale) : rsk[n + i];
-      const double rr = ax[i] + rsk[n + i] - tau * w->d->b[i];
+      const double rr = ax[i] + rsk[n + i] - tau * bv[i];
       const double ro = rr * (inv_ds / d);
       if (fabs(yo) > yi) yi = fabs(yo);
       if (fabs(so) > si) si = fabs(so);
@@ -1447,8 +1272,9 @@ long long scs_b200_launch_count(void) { return b200_launches(); }
 scs_int scs_b200_device_ok(void) { return b200_device_ok(); }
 
 /* ----------------------------------------------------------------- device-data entry points */
-/* scs_update's normalisation on the device originals: b200_normalize_b_c's products and maxima, bit for bit; the
- * four maxima are the only values that reach the host */
+/* b and c normalised from the device originals, for every door (reference scs_update and normalize_b_c, scs.c:1287-1325
+ * and normalize.c:33-61; the maxima skip NaN like its norm_inf): the four maxima are the only values that reach the
+ * host */
 static int update_bc_dev(ScsWork *w) {
   const double t0 = now_ms();
   double mx[4], sigma;
@@ -1468,7 +1294,6 @@ static int update_bc_dev(ScsWork *w) {
     w->dual_scale = sigma;
   }
   if (b200_sync() != 0) return -1;
-  w->bc_host_stale = 1;
   w->setup_time = now_ms() - t0;
   return 0;
 }
@@ -1510,7 +1335,7 @@ static int build_ops_dev(ScsWork *w, B200DevMats *dm) {
       if (b200_d2h(w->D, w->d_D, (size_t)m * 8) != 0 || b200_d2h(w->E, w->d_E, (size_t)n * 8) != 0 ||
           b200_sync() != 0)
         break;
-      if (w->k->bsize > 1) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
+      b200_normalize_box(w->k, w->D, w->k->bl, w->k->bu);
     }
     rc = 0;
   } while (0);
@@ -1587,24 +1412,12 @@ ScsWork *scs_b200_init_device(const ScsData *d, const ScsCone *k, const ScsSetti
 }
 
 static scs_int update_device(ScsWork *w, const scs_float *d_b, const scs_float *d_c, void *stream) {
-  const int n = w ? w->n : 0, m = w ? w->m : 0;
   int rc = -1;
   if (!w || !b200_single_gpu() || (d_b && !b200_dev_ptr_ok(d_b, "b")) || (d_c && !b200_dev_ptr_ok(d_c, "c"))) return -1;
   if (b200_wait_for_caller(stream) != 0) return -1;
-  do {
-    if (!w->d_b_orig) w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
-    if (!w->d_c_orig) w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
-    if (!w->d_b_orig || !w->d_c_orig) break;
-    /* an original kept from a host call is uploaded once (a workspace of scs_init, or after scs_update) */
-    if (d_b ? b200_d2d(w->d_b_orig, d_b, (size_t)m * 8) != 0
-            : !w->b_on_dev && b200_h2d(w->d_b_orig, w->b_orig, (size_t)m * 8) != 0)
-      break;
-    if (d_c ? b200_d2d(w->d_c_orig, d_c, (size_t)n * 8) != 0
-            : !w->c_on_dev && b200_h2d(w->d_c_orig, w->c_orig, (size_t)n * 8) != 0)
-      break;
-    w->b_on_dev = w->c_on_dev = 1;
+  if ((!d_b || b200_d2d(w->d_b_orig, d_b, (size_t)w->m * 8) == 0) &&
+      (!d_c || b200_d2d(w->d_c_orig, d_c, (size_t)w->n * 8) == 0))
     rc = update_bc_dev(w);
-  } while (0);
   b200_caller_waits(stream);
   return rc;
 }
@@ -1714,7 +1527,7 @@ static scs_int update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMat
     if (w->k->bsize > 1) {
       memcpy(w->k->bl, w->bl_orig, (size_t)(w->k->bsize - 1) * 8);
       memcpy(w->k->bu, w->bu_orig, (size_t)(w->k->bsize - 1) * 8);
-      if (w->D) normalize_box_cone(w->k, w->D + w->k->z + w->k->l, w->k->bsize);
+      b200_normalize_box(w->k, w->D, w->k->bl, w->k->bu);
     }
     if (b200_cones_set_box(w->cones, w->k->bl, w->k->bu) != 0) goto dev_fail;
     /* the log-det cones' warm starts and saved projections, as init leaves them */
@@ -1730,13 +1543,7 @@ static scs_int update_matrix_device(ScsWork *w, const ScsMatrix *A, const ScsMat
       goto dev_fail;
     if (w->accel) b200_aa_restart_dev(w->accel);
     w->r_orig.last_iter = w->r_norm.last_iter = -1;
-    /* 7. b and c renormalised from the originals with the new D, E (a host original is uploaded once) */
-    if (!w->d_b_orig) w->d_b_orig = (double *)b200_malloc((size_t)m * 8);
-    if (!w->d_c_orig) w->d_c_orig = (double *)b200_malloc((size_t)n * 8);
-    if (!w->d_b_orig || !w->d_c_orig || (!w->b_on_dev && b200_h2d(w->d_b_orig, w->b_orig, (size_t)m * 8) != 0) ||
-        (!w->c_on_dev && b200_h2d(w->d_c_orig, w->c_orig, (size_t)n * 8) != 0))
-      goto dev_fail;
-    w->b_on_dev = w->c_on_dev = 1;
+    /* 7. b and c renormalised from the originals with the new D, E */
     if (update_bc_dev(w) != 0) goto dev_fail;
     init_mark("update: box bounds, resets, b and c", &t_mark);
     rc = 0;

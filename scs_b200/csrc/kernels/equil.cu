@@ -261,13 +261,11 @@ out:
 }
 
 // ---------------------------------------------------------------------------------------------
-// b and c from device originals (the device-data entry points): out = orig * scale (scale NULL: a copy), with max |orig|
-// and max |out| into d_max[0], d_max[1]. A maximum does not depend on the order it is taken in, and the products are
-// elementwise, so this is bit for bit the host's b200_normalize_b_c. Non-negative doubles order like their bit
-// patterns, so the maxima are taken with an integer atomicMax, and a NaN entry is skipped. For max |b| and max |c|
-// that is what the host's `>` does. For max |b_orig| and max |c_orig| it is not: scs_update's MAX(nm, |x|) takes a
-// NaN and then the largest |x| after the last NaN, so with a NaN in b or c (neither API validates them) nm_b_orig /
-// nm_c_orig, and the convergence tests that read them, can differ between the two doors.
+// b and c from their device originals (every door): out = orig * scale (scale NULL: a copy), with max |orig| and
+// max |out| into d_max[0], d_max[1]. A maximum does not depend on the order it is taken in, and the products are
+// elementwise, so the result is the reference's normalize_b_c bit for bit. Non-negative doubles order like their bit
+// patterns, so the maxima are taken with an integer atomicMax, and a NaN entry is skipped, as the reference's norm_inf
+// (src/linalg.c:71-79) skips it.
 __device__ __forceinline__ void bc_atomic_max(double *d_max, double v) {
   for (int o = 16; o > 0; o >>= 1) {
     const double w = __shfl_xor_sync(0xffffffffu, v, o);

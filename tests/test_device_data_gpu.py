@@ -293,6 +293,63 @@ def test_mixed_sequences_and_user_memory_unchanged():
             assert torch.equal(before[k], v)
 
 
+def _csv_bc_norms(path):
+    """(b_nrm_inf, c_nrm_inf) of every row of a CSV trace"""
+    import csv
+    with open(path) as f:
+        return [(float(r["b_nrm_inf"]), float(r["c_nrm_inf"])) for r in csv.DictReader(f)]
+
+
+def test_nan_in_b_and_c_is_skipped_by_both_doors_and_updates_keep_the_other_original(tmp_path):
+    """max |b| and max |c| of the data as given skip a NaN, as the reference's norm_inf does, whichever door the data
+    comes through; an update of b alone keeps c, and one of c alone keeps b"""
+    prob = problems.make_problem(30, 10, 3, {"z": 3, "l": 17, "q": [4, 6]}, seed=4)
+    A, cone = sp.csc_matrix(prob["A"][:3], shape=prob["A"][3]), prob["cone"]
+    b, c = prob["b"].copy(), prob["c"].copy()
+    j, mid = int(np.argmax(np.abs(b))), b.size // 2
+    b[[j, mid]] = b[[mid, j]]
+    b[mid + 1] = np.nan  # after the largest |b|: a maximum restarted at the NaN would miss it
+    c[-1] = np.nan
+    seq = [(2.0 * b, None), (None, 3.0 * c)]
+    want, bb, cc = [], b, c
+    for step in [(None, None)] + seq:
+        bb = bb if step[0] is None else step[0]
+        cc = cc if step[1] is None else step[1]
+        want.append((np.nanmax(np.abs(bb)), np.nanmax(np.abs(cc))))
+    lib = capi.load()
+    host_csv = str(tmp_path / "host.csv")
+    hp = capi.HostProblem((A.data, A.indices, A.indptr, A.shape), b, c, cone)
+    w = lib.scs_init(C.byref(hp.data), C.byref(hp.cone),
+                     C.byref(capi.default_settings(lib, verbose=0, max_iters=1, log_csv_filename=host_csv.encode())))
+    assert w
+    host = []
+    x, y, s = np.zeros(hp.n), np.zeros(hp.m), np.zeros(hp.m)
+    try:
+        for step in [None] + seq:
+            if step is not None:
+                assert lib.scs_update(w, *[capi.dptr(np.ascontiguousarray(v)) if v is not None else None
+                                           for v in step]) == 0
+            sol, info = capi.ScsSolution(capi.dptr(x), capi.dptr(y), capi.dptr(s)), capi.ScsInfo()
+            lib.scs_solve(w, C.byref(sol), C.byref(info), 0)
+            host.append(_csv_bc_norms(host_csv))
+    finally:
+        lib.scs_finish(w)
+    dev_csv = str(tmp_path / "device.csv")
+    solver = torch_solver.SCS(to_torch(A, None, b, c), cone, verbose=0, max_iters=1, log_csv_filename=dev_csv.encode())
+    device = []
+    try:
+        for step in [None] + seq:
+            if step is not None:
+                solver.update(*[None if v is None else torch.tensor(v, device=solver.device) for v in step])
+            solver.solve(warm_start=False)
+            device.append(_csv_bc_norms(dev_csv))
+    finally:
+        solver.close()
+    assert host == device
+    for rows, nm in zip(host, want):
+        assert len(rows) >= 2 and all(r == nm for r in rows), (rows, nm)
+
+
 def _bad(name):
     A, P, b, c, cone = read_fixture("mpc_bug1")
     A, P = A.copy(), P.copy()

@@ -66,6 +66,14 @@ def bad_cones(base):
     return out
 
 
+def struct_cones(base):
+    """(cone, mutate) pairs whose fault lies in the struct and not in the dict: a NULL array behind a positive size"""
+    def no_q(k): k.q = type(k.q)()
+    def no_bl(k): k.bl = capi.c_double_p()
+    bx = dict(base, l=base["l"] - 3, bl=[0.0, 0.0], bu=[1.0, 1.0])
+    return [(dict(base), no_q), (bx, no_bl)]
+
+
 def libs(lib):
     pairs = [("scs_b200", lib)]
     if os.path.exists(REF_LIB):
@@ -104,3 +112,21 @@ def test_bad_P_is_refused(lib):
     prob["P"] = (L.data.copy(), L.indices.astype(np.int32), L.indptr.astype(np.int32), (n, n))   # LOWER triangle
     for name, library in libs(lib):
         assert run(library, prob) == SCS_FAILED, name
+
+
+@pytest.mark.parametrize("i", range(14))
+def test_init_cone_refuses_what_scs_init_refuses_with_its_message(lib, capfd, i):
+    """scs_b200_init_cone validates like scs_init: the same cones refused, before any device work, with the line
+    scs_init prints for them, also where a positive size has no array behind it"""
+    prob = base_problem()
+    cases = [(c, None) for c in bad_cones(prob["cone"])] + struct_cones(prob["cone"])
+    cone, mutate = cases[i]
+    capfd.readouterr()
+    assert run(lib, prob, cone=cone, mutate=(lambda hp, st: mutate(hp.cone)) if mutate else None) == SCS_FAILED
+    init_out = capfd.readouterr().out
+    k, keep = capi.make_cone(cone)
+    if mutate:
+        mutate(k)
+    assert not lib.scs_b200_init_cone(C.byref(k), prob["m"], None)
+    cone_out = capfd.readouterr().out
+    assert cone_out.count("\n") == 1 and init_out.startswith(cone_out), (cone_out, init_out)
