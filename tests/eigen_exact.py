@@ -188,7 +188,9 @@ def gate(delta_in, N, x):
 # ---------------------------------------------------------------------------------------------- projections, exactly
 def ell1_threshold(t, a):
     """exact mu >= 0 of Pi onto {(t, a): ||a||_1 <= t} for a >= 0 (Fractions): (t + mu, max(a - mu, 0)); mu = None when
-    -t >= max a (Pi = 0)"""
+    -t >= max a (Pi = 0). a may also be a numpy integer array with an integer t (the path for long vectors)."""
+    if isinstance(a, np.ndarray):
+        return _ell1_threshold_int(t, a)
     if not a or -t >= max(a):
         return None
     if sum(a) <= t:
@@ -202,6 +204,25 @@ def ell1_threshold(t, a):
         if v > mu >= nxt:
             return mu
     raise AssertionError("no threshold")
+
+
+def _ell1_threshold_int(t, a):
+    """ell1_threshold for integer magnitudes (numpy, sum below 2^62) and an integer t: the same sorted scan on int64
+    prefix sums, the threshold (cs_j - t) / (j + 2) compared by cross-multiplication"""
+    T = int(t)
+    assert T == t and a.dtype.kind in "iu"
+    a = a.astype(np.int64)
+    if a.size == 0 or -T >= int(a.max()):
+        return None
+    if int(a.sum()) <= T:
+        return Fraction(0)
+    s = np.sort(a)[::-1]
+    cs = np.cumsum(s)
+    j2 = np.arange(2, s.size + 2, dtype=np.int64)
+    nxt = np.append(s[1:], 0)
+    ok = np.nonzero((s * j2 > cs - T) & (cs - T >= nxt * j2))[0]
+    assert ok.size, "no threshold"
+    return Fraction(int(cs[ok[0]]) - T, int(j2[ok[0]]))
 
 
 def proj_ell1_exact(t, a):
