@@ -231,6 +231,12 @@ const char *scs_get_lin_sys_method(void);
  * total (reference private.h:29 tot_cg_its). */
 scs_int scs_b200_linsys_last_cg_its(const ScsLinSysWork *w);
 long long scs_b200_linsys_total_cg_its(const ScsLinSysWork *w);
+/* KKT solves of this workspace whose CG iterations ran as batches of one cooperative kernel each (kernels/cg.cu
+ * k_cg_batch; SCS_B200_CG_BATCH_KERNEL=0 selects three kernels per iteration) */
+long long scs_b200_linsys_cg_batch_solves(const ScsLinSysWork *w);
+/* 0: every later KKT solve of the process runs three kernels per CG iteration, as SCS_B200_CG_BATCH_KERNEL=0 does;
+ * 1: the batch kernel where it can run (the default) */
+void scs_b200_set_cg_batch_kernel(int on);
 
 /* y (+)= A x  and  y (+)= A' x  through the device SpMV kernels
  * (reference linsys/scs_matrix.c:161-203 accum_by_atrans / accum_by_a).
@@ -274,6 +280,11 @@ double scs_b200_time_cg_iter(ScsLinSysWork *w, scs_int reps, double *alg_bytes);
  * pushes), the slice kernel; [3] = 0; [4] = iteration; [5..11] = the phases inside the slice kernel (rank-local). */
 scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms,
                                  double *out_bytes);
+/* The CG loop's batch kernel (k_cg_batch) over one launch of `reps` genuine iterations after the same start on b:
+ * out_ms[0..4] = ms per iteration of its K1 phase, K2 phase, update up to the beta wait and p update (block 0's
+ * globaltimer, each with the barrier or wait that ends it), and of the whole launch (CUDA events). Single GPU, P = NULL; -1 when
+ * the workspace cannot run the batch kernel. */
+scs_int scs_b200_time_cg_batch(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms);
 
 /* Cone operator: replaces reference src/cones.c:1498-1596 (init_cone /
  * proj_dual_cone / finish_cone) for zero, LP, box, SOC, PSD, exponential and power cones,

@@ -345,6 +345,10 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_linsys_last_cg_its.argtypes = [C.c_void_p]
     lib.scs_b200_linsys_total_cg_its.restype = C.c_longlong
     lib.scs_b200_linsys_total_cg_its.argtypes = [C.c_void_p]
+    lib.scs_b200_linsys_cg_batch_solves.restype = C.c_longlong
+    lib.scs_b200_linsys_cg_batch_solves.argtypes = [C.c_void_p]
+    lib.scs_b200_set_cg_batch_kernel.restype = None
+    lib.scs_b200_set_cg_batch_kernel.argtypes = [I]
     for f in (lib.scs_b200_accum_by_a, lib.scs_b200_accum_by_atrans):
         f.restype = I
         f.argtypes = [C.c_void_p, c_double_p, c_double_p, I]
@@ -354,6 +358,8 @@ def _declare(lib, ours, cone=ScsCone, T=None):
     lib.scs_b200_time_cg_iter.argtypes = [C.c_void_p, I, c_double_p]
     lib.scs_b200_time_cg_kernels.restype = I
     lib.scs_b200_time_cg_kernels.argtypes = [C.c_void_p, c_double_p, I, c_double_p, c_double_p]
+    lib.scs_b200_time_cg_batch.restype = I
+    lib.scs_b200_time_cg_batch.argtypes = [C.c_void_p, c_double_p, I, c_double_p]
     lib.scs_b200_init_cone.restype = C.c_void_p
     lib.scs_b200_init_cone.argtypes = [C.POINTER(cone), I, c_double_p]
     lib.scs_b200_proj_dual_cone.restype = I

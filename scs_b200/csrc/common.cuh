@@ -90,17 +90,18 @@ __device__ __forceinline__ void block_max(double (&v)[NV], double *smem) {
 // `mine`. `is_max[i]` selects max instead of sum for value i (bitmask).
 // The counter is reset by the last block, so the buffer is reusable by the
 // next kernel on the same stream.
+// grid_finish_of: the same over `nblocks` participating blocks, this one being block `bid` (a kernel that runs the
+// reduction of a smaller grid than its own).
 template <int NV>
-__device__ __forceinline__ bool grid_finish(double (&mine)[NV], double *partials,
-                                            unsigned int *counter, unsigned max_mask,
-                                            double *smem) {
+__device__ __forceinline__ bool grid_finish_of(double (&mine)[NV], double *partials, unsigned int *counter,
+                                               unsigned max_mask, double *smem, unsigned nblocks, unsigned bid) {
   __shared__ int s_last;
   if (threadIdx.x == 0) {
 #pragma unroll
-    for (int i = 0; i < NV; ++i) partials[i * gridDim.x + blockIdx.x] = mine[i];
+    for (int i = 0; i < NV; ++i) partials[i * nblocks + bid] = mine[i];
     __threadfence();
     unsigned t = atomicAdd(counter, 1u);
-    s_last = (t == gridDim.x - 1);
+    s_last = (t == nblocks - 1);
   }
   __syncthreads();
   if (!s_last) return false;
@@ -111,8 +112,8 @@ __device__ __forceinline__ bool grid_finish(double (&mine)[NV], double *partials
   for (int i = 0; i < NV; ++i) {
     const bool mx = (max_mask >> i) & 1u;
     double a = 0.0;
-    for (unsigned j = threadIdx.x; j < gridDim.x; j += blockDim.x) {
-      double p = __ldcg(&partials[i * gridDim.x + j]);
+    for (unsigned j = threadIdx.x; j < nblocks; j += blockDim.x) {
+      double p = __ldcg(&partials[i * nblocks + j]);
       a = mx ? fmax(a, p) : a + p;
     }
     acc[i] = a;
@@ -130,6 +131,11 @@ __device__ __forceinline__ bool grid_finish(double (&mine)[NV], double *partials
     __threadfence();
   }
   return true;
+}
+template <int NV>
+__device__ __forceinline__ bool grid_finish(double (&mine)[NV], double *partials, unsigned int *counter,
+                                            unsigned max_mask, double *smem) {
+  return grid_finish_of<NV>(mine, partials, counter, max_mask, smem, gridDim.x, blockIdx.x);
 }
 
 // ---------------------------------------------------------------- Moreau post-scaling (cones)

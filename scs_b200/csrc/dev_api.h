@@ -234,6 +234,8 @@ typedef struct {
                                 peer-mapped exchange allocation */
   int k34_fused;       /* 1: K3 and K4 run as one kernel (k_cg_update_p); set by b200_cg_plan_k34 */
   long long k34_solves[2]; /* KKT solves run with the fused kernel / with the pair k_cg_update + k_cg_pupdate */
+  int k34_batch;       /* 1: the batch kernel (k_cg_batch) fits the device; set by b200_cg_plan_k34 */
+  long long k34_batch_solves; /* KKT solves whose CG iterations ran as k_cg_batch launches (counted in k34_solves[0]) */
 } B200Cg;
 
 /* M_j = 1 / (R_x,j + P_jj + sum_k A_kj^2 / R_y,k)   (private.c:50-82) */
@@ -259,6 +261,9 @@ int b200_cg_one_iteration(B200Cg *cg, double *d_x);
 double b200_cg_iter_alg_bytes(const B200Cg *cg, double *per_kernel);
 /* per-kernel device times (ms per launch) of `reps` genuine CG iterations: K1, K2, K3, K4, whole iteration */
 int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *out_ms);
+/* the batch kernel's phases over one launch of `reps` genuine iterations (ms per iteration): K1, K2, update to its
+ * beta wait, p update, whole launch; -1 when the workspace cannot run it */
+int b200_cg_time_batch(B200Cg *cg, double *d_x, int reps, double *out_ms);
 
 /* ------------------------------------------------------------ comm (kernels/comm.cu) */
 int b200_comm_rank(void);

@@ -833,6 +833,7 @@ scs_int scs_b200_update_lin_sys_diag_r_device(ScsLinSysWork *w, const scs_float 
 }
 
 scs_int scs_b200_linsys_last_cg_its(const ScsLinSysWork *w) { return w->last_cg_its; }
+long long scs_b200_linsys_cg_batch_solves(const ScsLinSysWork *w) { return w->cg.k34_batch_solves; }
 long long scs_b200_linsys_total_cg_its(const ScsLinSysWork *w) { return w->tot_cg_its; }
 
 /* SCS_B200_G_REUSE=0 makes the ADMM driver's update_work re-solve g at every scs_solve, as the reference does, for A/B
@@ -948,6 +949,23 @@ static scs_int time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int rep
   if (b200_cg_time_kernels(&w->cg, w->d_b, (int)reps, out_ms) != 0) return -1;
   if (out_bytes) out_bytes[4] = b200_cg_iter_alg_bytes(&w->cg, out_bytes);
   return 0;
+}
+/* the batch kernel's phases (b200_cg_time_batch) on the solver's own vectors after a genuine start on b (n + m, host) */
+static scs_int time_cg_batch(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms) {
+  const size_t nm = (size_t)w->n + w->m;
+  if (b200_h2d(w->d_b, b, nm * 8) != 0) return -1;
+  if (b200_cg_solve(&w->cg, w->d_b, NULL, 0.0, 1, 0, NULL) < 0) return -1;
+  w->cg.h_ctl->done = 0;
+  w->cg.h_ctl->max_its = 2000000000;
+  if (b200_h2d(w->cg.d_ctl, w->cg.h_ctl, sizeof(B200CgCtl)) != 0) return -1;
+  if (b200_cg_time_batch(&w->cg, w->d_b, 3, out_ms) != 0) return -1; /* warm-up */
+  return b200_cg_time_batch(&w->cg, w->d_b, (int)reps, out_ms) == 0 ? 0 : -1;
+}
+scs_int scs_b200_time_cg_batch(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms) {
+  B200Ctx *prev = b200_ctx_enter(w->ctx);
+  const scs_int rc = time_cg_batch(w, b, reps, out_ms);
+  b200_ctx_leave(prev);
+  return rc;
 }
 scs_int scs_b200_time_cg_kernels(ScsLinSysWork *w, const scs_float *b, scs_int reps, double *out_ms,
                                  double *out_bytes) {

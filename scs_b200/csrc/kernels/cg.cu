@@ -18,11 +18,14 @@
 //   K3  x += alpha p; r -= alpha Gp; z = M r; z'r, ||r||_inf; stop test; beta
 //   K4  p = z + beta p
 // Up to n = 2 SMs * 4096 (single GPU), K3 and K4 run as one kernel, k_cg_update_p, that keeps z and p in registers
-// across a grid barrier: 3 kernels per iteration, z never stored.
+// across a grid barrier: 3 kernels per iteration, z never stored. There, with the reordered pair and P = 0, a whole
+// batch of iterations runs as one cooperative kernel, k_cg_batch, with the three as phases behind grid barriers.
 // Algorithmic bytes: 24 nnz + 4 (m+n+2) + 24 m + 120 n; 96 n instead of 120 n fused   (DESIGN.md).
 #include "../common.cuh"
 #include "../dev_api.h"
+#include "../spmv_flag.cuh"
 #include <atomic>
+#include <mutex>
 #include <math.h>
 #include <stdlib.h>
 #include <string.h>
@@ -361,6 +364,363 @@ k_cg_update_p(int n, double *__restrict__ x, double *__restrict__ r, double *__r
     __syncthreads();
     if (threadIdx.x == 0) atomicMax(stamps + 2, cg_globaltimer());
   }
+}
+
+
+// ---------------------------------------------------------------------------
+// A batch of CG iterations as ONE cooperative kernel (single GPU, the reordered pair, P = 0): k_cg_batch runs up to
+// `iters` iterations, each as three phases behind grid barriers instead of three launches:
+//   K1      tmp = R_y^-1 A_cg p    A_cg's partition, warp-tiles and lanes (spmv3_consume_stage): the same row sums
+//   K2      Gp = R_x p + At_cg' tmp, p'Gp over At_cg's CTAs with its slots and ticket, the last one writes alpha
+//   update  k_cg_update_p on k34_grid(n) VIRTUAL blocks of VEC_THREADS threads: CTA c runs virtual blocks c and c + G,
+//           virtual warp w of them (w < 32) on real warp w % 24, lane for lane. The same elements in the same order,
+//           cg_update_elem, the warp trees of block_sum / block_max, the slots and the finish of grid_finish over the
+//           virtual grid: z'r, ||r||_inf and beta are the same bits. z and p wait for beta in the ring's shared
+//           memory (CG_BATCH_ZP_BYTES; k34_fused bounds n so that they fit).
+// A grid barrier (cg_grid_sync) follows K1 and another the p update. After K2 and after the update's reductions the
+// CTAs wait instead for the release of the last one to finish the reduction (cg_flag_wait): it stores a new value into
+// a word every CTA read at the start of the iteration, after alpha, resp. the control block, so one round of atomics
+// (the tickets) serves both the reduction and the synchronisation. Every CTA reads `done` after the wait that follows
+// the update's finish and leaves the loop when it is set, so iterations past the stop cost nothing. Within one launch p and tmp are rewritten between phases: every read of them is a weak load after the
+// acquire that precedes the phase (spmv3_consume_stage<.., NC = false>), never the non-coherent path. The first ring stages of K2
+// and of the next iteration's K1 are issued before the barrier that precedes them (matrix streams are never written). The grid is co-resident (cooperative
+// launch, checked at setup) and runs only under the K34 token. stamps (timing runs only, else NULL): block 0's
+// %globaltimer at the start of every iteration and after each of its four barriers or waits, 5 per iteration.
+#define CG_BATCH_VW (2 * VEC_THREADS / 32)  // virtual warps per CTA
+#define CG_BATCH_ZP_BYTES (2 * CG_BATCH_VW * CG_FUSED_V2 * 32 * 16)
+struct B200CgBatchArgs {
+  double *x, *r, *p, *Gp, *tmp;
+  const double *M;
+  const double *d1;       // K1's 1 / R_y (vector or table), dmask1 its row mask for B200_D_TWO
+  const unsigned *dmask1;
+  int dform1;
+  const double *d2;       // K2's R_x (vector or table)
+  int dform2;
+  B200CgCtl *ctl;
+  double *partials;       // the update's slots and ticket
+  unsigned *counter;
+  unsigned *bar;          // the grid barrier's word
+  int *seq;               // released by K2's finish (a new value every iteration)
+  int g34;                // virtual blocks of the update
+  unsigned long long *stamps;
+};
+
+// grid barrier over the co-resident grid: block 0 adds 2^31 - (G - 1), every other block 1, so the top bit flips once
+// all have arrived and the low bits are 0 again (the word needs no reset between barriers or launches). The arrival is
+// a release at gpu scope (after __syncthreads, so it orders the whole CTA's stores), the spin an acquire (which also
+// invalidates the SM's L1; __syncthreads then orders the CTA's later loads after it). Gives up after ~1.5 s and raises
+// the sticky ctl->pad[0]; returns 0 then (uniform over the CTA). `between` runs in thread 0 after its arrival, before
+// it waits: work that must follow the CTA's __syncthreads but need not delay the other CTAs.
+struct CgNothing {
+  __device__ void operator()() const {}
+};
+template <typename F = CgNothing>
+__device__ __forceinline__ int cg_grid_sync(unsigned *bar, B200CgCtl *ctl, int *s_ok, F between = F()) {
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    const unsigned add = blockIdx.x == 0 ? 0x80000000u - (gridDim.x - 1) : 1u;
+    unsigned old;
+    asm volatile("atom.add.release.gpu.global.u32 %0, [%1], %2;" : "=r"(old) : "l"(bar), "r"(add) : "memory");
+    between();
+    const long long t0 = clock64();
+    int ok = 1;
+    for (;;) {
+      unsigned cur;
+      asm volatile("ld.acquire.gpu.global.u32 %0, [%1];" : "=r"(cur) : "l"(bar) : "memory");
+      if ((cur ^ old) & 0x80000000u) break;
+      if (*((volatile int *)&ctl->pad[0]) || clock64() - t0 > 3000000000LL) {
+        ctl->pad[0] = 1;
+        ok = 0;
+        break;
+      }
+    }
+    *s_ok = ok;
+  }
+  __syncthreads();
+  return *s_ok;
+}
+// the release side of cg_flag_wait: the finishing CTA's thread 0, after its stores of the results
+__device__ __forceinline__ void cg_flag_release(int *word, int v) {
+  asm volatile("st.release.gpu.global.s32 [%0], %1;" ::"l"(word), "r"(v) : "memory");
+}
+__device__ __forceinline__ int cg_flag_load(const int *word) {
+  int v;
+  asm volatile("ld.relaxed.gpu.global.s32 %0, [%1];" : "=r"(v) : "l"(word) : "memory");
+  return v;
+}
+// thread 0 spins (acquire) until *word is no longer `old`, the value it read before the grid barrier that precedes
+// the release (so it cannot see the new value too early, nor miss it: the next release needs this CTA at that barrier
+// again). Same timeout as cg_grid_sync.
+__device__ __forceinline__ int cg_flag_wait(const int *word, int old, B200CgCtl *ctl, int *s_ok) {
+  if (threadIdx.x == 0) {
+    const long long t0 = clock64();
+    int ok = 1;
+    for (;;) {
+      int cur;
+      asm volatile("ld.acquire.gpu.global.s32 %0, [%1];" : "=r"(cur) : "l"(word) : "memory");
+      if (cur != old) break;
+      if (*((volatile int *)&ctl->pad[0]) || clock64() - t0 > 3000000000LL) {
+        ctl->pad[0] = 1;
+        ok = 0;
+        break;
+      }
+    }
+    *s_ok = ok;
+  }
+  __syncthreads();
+  return *s_ok;
+}
+
+// producer: stages [from, to) of this CTA's share of op, stage i at ring position ring + i
+template <bool IDX24>
+__device__ __forceinline__ void cg_batch_produce(const B200FlagView &op, const Spmv3Ring &R, int ring, int from, int to,
+                                                 uint64_t pol) {
+  if (from >= to) return;
+  const int4 *g = op.wt + (size_t)op.cta_begin[blockIdx.x] * SPMV3_NCW;
+  for (int i = from; i < to; ++i) {
+    const int q = ring + i, st = q % SPMV3_STAGES, use = q / SPMV3_STAGES;
+    const int ka = __ldg(&g[(size_t)i * SPMV3_NCW].y) & ~3;
+    const int4 l = __ldg(&g[(size_t)(i + 1) * SPMV3_NCW - 1]);
+    const int cnt = (l.y + l.z - ka + 3) & ~3;
+    if (use > 0) mbar_wait(&R.empty[st], (unsigned)((use - 1) & 1));
+    spmv3_issue_stage<IDX24>(R, st, g, i, ka, cnt, op.idx, op.vals, pol);
+  }
+}
+// one product as a phase: this CTA's nt stages of op from ring position `ring` (the first `pre` of them were issued by
+// the previous phase), then the first ring round of the next phase (nt_next stages of next)
+template <int POST, bool IDX24, bool NEXT_IDX24>
+__device__ __forceinline__ void cg_batch_spmv(const B200FlagView &op, int nt, int pre, const B200FlagView &next,
+                                              int nt_next, int &ring, const Spmv3Ring &R, const Spmv3Epi &E,
+                                              double &dot_acc) {
+  const int wid = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  if (wid == 0) {
+    if (lane == 0) {
+      const uint64_t pol = l2_policy_evict_first();
+      cg_batch_produce<IDX24>(op, R, ring, pre, nt, pol);
+      cg_batch_produce<NEXT_IDX24>(next, R, ring + nt, 0, nt_next < SPMV3_STAGES ? nt_next : SPMV3_STAGES, pol);
+    }
+  } else {
+    for (int i = 0; i < nt; ++i) {
+      const int q = ring + i;
+      spmv3_consume_stage<POST, IDX24, false>(R, q % SPMV3_STAGES, (unsigned)((q / SPMV3_STAGES) & 1), wid - 1, lane,
+                                              E, dot_acc);
+    }
+  }
+  ring += nt;
+}
+
+template <bool PK1, bool PK2>
+__global__ void __launch_bounds__(SPMV3_THREADS, 1)
+k_cg_batch(int n, int iters, B200FlagView A, B200FlagView At, B200CgBatchArgs a) {
+  extern __shared__ __align__(128) unsigned char smem_raw[];
+  __shared__ __align__(8) uint64_t s_mbar[2 * SPMV3_STAGES];
+  __shared__ double s_red[64];
+  __shared__ double s_ws[CG_BATCH_VW], s_wm[CG_BATCH_VW];  // per virtual warp: warp_sum of z'r, warp_max of |r|
+  __shared__ double s_tail[2], s_beta;
+  __shared__ int s_ok, s_flag;
+  double *s_vals = reinterpret_cast<double *>(smem_raw);
+  int *s_idx = reinterpret_cast<int *>(s_vals + SPMV3_STAGES * SPMV3_CAP);
+  int4 *s_desc = reinterpret_cast<int4 *>(s_idx + SPMV3_STAGES * SPMV3_CAP);
+  double *s_out = reinterpret_cast<double *>(s_desc + SPMV3_STAGES * SPMV3_NCW);
+  const Spmv3Ring R = {s_vals, s_idx, s_desc, s_mbar, s_mbar + SPMV3_STAGES, s_out};
+  // the update's z and p, [virtual warp][k][lane], over the ring (every stage has been consumed by then)
+  double2 *s_z = reinterpret_cast<double2 *>(smem_raw);
+  double2 *s_p = s_z + CG_BATCH_VW * CG_FUSED_V2 * 32;
+  const int tid = threadIdx.x, lane = tid & 31, wid = tid >> 5, b = blockIdx.x, G = gridDim.x;
+  volatile B200CgCtl *c = a.ctl;
+  if (tid == 0) {
+    for (int s = 0; s < SPMV3_STAGES; ++s) {
+      mbar_init(&R.full[s], 1);
+      mbar_init(&R.empty[s], SPMV3_NCW);
+    }
+    mbar_fence_init();
+    s_flag = c->done;
+  }
+  __syncthreads();
+  if (s_flag) return;
+  const int nt1 = b < A.grid ? A.cta_begin[b + 1] - A.cta_begin[b] : 0;
+  const int nt2 = b < At.grid ? At.cta_begin[b + 1] - At.cta_begin[b] : 0;
+  Spmv3Epi E1 = {a.p, a.tmp, nullptr, 1.0, a.d1, a.dmask1, a.dform1, 0.0, 0.0, nullptr, false, nullptr, nullptr, 0ull};
+  Spmv3Epi E2 = {a.tmp, a.Gp, nullptr, 1.0, a.d2, nullptr, a.dform2, 0.0, 0.0, a.p, false, nullptr, nullptr, 0ull};
+  if (a.dform1 != B200_D_VEC) {
+    E1.dt0 = a.d1[0];
+    E1.dt1 = a.dform1 == B200_D_TWO ? a.d1[1] : E1.dt0;
+  }
+  if (a.dform2 != B200_D_VEC) E2.dt0 = E2.dt1 = a.d2[0];
+  const int g34 = a.g34, n2 = n >> 1, stride = g34 * VEC_THREADS;
+  double2 *x2 = reinterpret_cast<double2 *>(a.x), *r2 = reinterpret_cast<double2 *>(a.r),
+          *p2 = reinterpret_cast<double2 *>(a.p);
+  const double2 *g2 = reinterpret_cast<const double2 *>(a.Gp), *m2 = reinterpret_cast<const double2 *>(a.M);
+  unsigned long long *stamp = (a.stamps != nullptr && b == 0 && tid == 0) ? a.stamps : nullptr;
+  int ring = 0;
+  for (int it = 0; it < iters; ++it) {
+    if (stamp) stamp[5 * it] = cg_globaltimer();
+    // the words the two finishes release this iteration, as they are before the K1 -> K2 barrier (thread 0 only)
+    const int seq0 = tid == 0 ? cg_flag_load(a.seq) : 0;
+    const int its0 = tid == 0 ? cg_flag_load(&a.ctl->iters) : 0;
+    double dot = 0.0;
+    // ---- K1, then K2's first ring round
+    const int pre1 = it > 0 ? (nt1 < SPMV3_STAGES ? nt1 : SPMV3_STAGES) : 0;  // issued before the last barrier
+    cg_batch_spmv<B200_POST_MUL, PK1, PK2>(A, nt1, pre1, At, nt2, ring, R, E1, dot);
+    if (!cg_grid_sync(a.bar, a.ctl, &s_ok)) return;
+    if (stamp) stamp[5 * it + 1] = cg_globaltimer();
+    // ---- K2 and its dot product; the last of At's CTAs writes alpha (spmv_tail, B200_HOOK_CG_ALPHA)
+    cg_batch_spmv<B200_POST_FMA_DOT, PK2, PK2>(At, nt2, nt2 < SPMV3_STAGES ? nt2 : SPMV3_STAGES, At, 0, ring, R, E2,
+                                               dot);
+    if (b < At.grid) {
+      double acc[1] = {dot};
+      block_sum<1>(acc, s_red);
+      if (grid_finish_of<1>(acc, At.partials, At.counter, 0u, s_red, (unsigned)At.grid, (unsigned)b)) {
+        if (tid == 0) {
+          c->pGp = acc[0];
+          c->alpha = c->ztr / acc[0];
+          cg_flag_release(a.seq, seq0 + 1);
+        }
+      }
+    }
+    // At's CTAs stored Gp and took their tickets before the release; the update reads Gp and alpha after it
+    if (!cg_flag_wait(a.seq, seq0, a.ctl, &s_ok)) return;
+    if (stamp) stamp[5 * it + 2] = cg_globaltimer();
+    // ---- update, first half (k_cg_update_p up to its barrier) on the virtual blocks
+    const double alpha = c->alpha, nalpha = -alpha;
+    for (int vw = wid; vw < CG_BATCH_VW; vw += SPMV3_THREADS / 32) {
+      const int v = b + (vw >> 4) * G;
+      double acc0 = 0.0, acc1 = 0.0;
+      if (v < g34) {
+        const int i0 = v * VEC_THREADS + (vw & 15) * 32 + lane;
+#pragma unroll
+        for (int k = 0; k < CG_FUSED_V2; ++k) {
+          const int i = i0 + k * stride;
+          if (i < n2) {
+            double2 xa = x2[i], ra = r2[i], pa = p2[i], ga = g2[i], ma = m2[i], za;
+            cg_update_elem(alpha, nalpha, xa.x, ra.x, pa.x, ga.x, ma.x, za.x, acc0, acc1);
+            cg_update_elem(alpha, nalpha, xa.y, ra.y, pa.y, ga.y, ma.y, za.y, acc0, acc1);
+            x2[i] = xa; r2[i] = ra;
+            s_z[(vw * CG_FUSED_V2 + k) * 32 + lane] = za;
+            s_p[(vw * CG_FUSED_V2 + k) * 32 + lane] = pa;
+          }
+        }
+        if ((n & 1) && v == 0 && vw == 0 && lane == 0) {  // k_cg_update_p's tail: block 0, thread 0, last
+          const int k = n - 1;
+          double xv = a.x[k], rv = a.r[k], zt;
+          const double pt = a.p[k];
+          cg_update_elem(alpha, nalpha, xv, rv, pt, a.Gp[k], a.M[k], zt, acc0, acc1);
+          a.x[k] = xv; a.r[k] = rv;
+          s_tail[0] = zt;
+          s_tail[1] = pt;
+        }
+      }
+      acc0 = warp_sum(acc0);
+      acc1 = warp_max(acc1);
+      if (lane == 0) {
+        s_ws[vw] = acc0;
+        s_wm[vw] = acc1;
+      }
+    }
+    __syncthreads();
+    // block_sum / block_max's second stage for each virtual block (16 warps), into its slots of grid_finish<2>
+    if (wid < 2 && b + wid * G < g34) {
+      const double t = warp_sum(lane < 16 ? s_ws[wid * 16 + lane] : 0.0);
+      const double u = warp_max(lane < 16 ? s_wm[wid * 16 + lane] : 0.0);
+      if (lane == 0) {
+        a.partials[b + wid * G] = t;
+        a.partials[g34 + b + wid * G] = u;
+      }
+    }
+    __syncthreads();
+    if (tid == 0) {
+      const unsigned mine = (unsigned)(b < g34) + (unsigned)(b + G < g34);
+      int last = 0;
+      if (mine) {  // release of this CTA's slots, acquire of the others' for the finish
+        unsigned t;
+        asm volatile("atom.add.acq_rel.gpu.global.u32 %0, [%1], %2;" : "=r"(t) : "l"(a.counter), "r"(mine) : "memory");
+        last = t + mine == (unsigned)g34;
+      }
+      s_flag = last;
+    }
+    __syncthreads();
+    if (s_flag) {
+      // grid_finish<2> over the g34 virtual blocks: thread t < VEC_THREADS takes slot t; the threads beyond a virtual
+      // block's VEC_THREADS hold exact zeros, which leave block_sum's and block_max's trees as they are
+      double s[1] = {0.0}, m[1] = {0.0};
+      if (tid < g34) {
+        s[0] = s[0] + __ldcg(&a.partials[tid]);
+        m[0] = fmax(m[0], __ldcg(&a.partials[g34 + tid]));
+      }
+      block_sum<1>(s, s_red);
+      block_max<1>(m, s_red);
+      if (tid == 0) {
+        // k_cg_update_p's last block
+        const double ztr_prev = c->ztr;
+        const int its = its0 + 1;
+        int done = 0;
+        c->ztr_prev = ztr_prev;
+        c->ztr = s[0];
+        c->rnorm = m[0];
+        if (m[0] < c->tol) {
+          done = 1;
+        } else if (ztr_prev == 0.0) {
+          done = 1;
+        } else {
+          c->beta = s[0] / ztr_prev;
+          if (its >= c->max_its) done = 1;
+        }
+        if (done) c->done = 1;
+        *a.counter = 0u;
+        cg_flag_release(&a.ctl->iters, its);  // last: it releases the other CTAs (k_cg_update_p stores iters last too)
+      }
+    }
+    if (!cg_flag_wait(&a.ctl->iters, its0, a.ctl, &s_ok)) return;
+    if (stamp) stamp[5 * it + 3] = cg_globaltimer();
+    // ---- update, second half: p = z + beta p unless the stop test fired
+    if (tid == 0) {
+      s_flag = c->done;
+      s_beta = c->beta;
+    }
+    __syncthreads();
+    if (s_flag) return;
+    const double beta = s_beta;
+    for (int vw = wid; vw < CG_BATCH_VW; vw += SPMV3_THREADS / 32) {
+      const int v = b + (vw >> 4) * G;
+      if (v >= g34) continue;
+      const int i0 = v * VEC_THREADS + (vw & 15) * 32 + lane;
+#pragma unroll
+      for (int k = 0; k < CG_FUSED_V2; ++k) {
+        const int i = i0 + k * stride;
+        if (i < n2) {
+          double2 pa = s_p[(vw * CG_FUSED_V2 + k) * 32 + lane];
+          const double2 za = s_z[(vw * CG_FUSED_V2 + k) * 32 + lane];
+          pa.x = fma(beta, pa.x, za.x); pa.y = fma(beta, pa.y, za.y);
+          p2[i] = pa;
+        }
+      }
+      if ((n & 1) && v == 0 && vw == 0 && lane == 0) a.p[n - 1] = fma(beta, s_tail[1], s_tail[0]);
+    }
+    // the next K1's first ring round overwrites what z and p occupied in this CTA: after every thread's last read of
+    // them, a proxy fence and the barrier's __syncthreads, thread 0 issues it between its arrival and its wait (A_cg's
+    // stream is never written)
+    fence_proxy_async();
+    const int pre_next = it + 1 < iters ? (nt1 < SPMV3_STAGES ? nt1 : SPMV3_STAGES) : 0;
+    const int ring_now = ring;
+    auto prefetch = [&] {
+      if (pre_next > 0) cg_batch_produce<PK1>(A, R, ring_now, 0, pre_next, l2_policy_evict_first());
+    };
+    if (!cg_grid_sync(a.bar, a.ctl, &s_ok, prefetch)) {
+      if (tid == 0)  // the stages in flight land before the CTA exits
+        for (int i = 0; i < pre_next; ++i) mbar_wait(&R.full[(ring + i) % SPMV3_STAGES], ((ring + i) / SPMV3_STAGES) & 1);
+      return;
+    }
+    if (stamp) stamp[5 * it + 4] = cg_globaltimer();
+  }
+}
+// dynamic shared memory: the ring (stages, descriptors, warp scratch; its barriers are static) or z and p, the larger
+#define CG_BATCH_RING_BYTES \
+  ((size_t)SPMV3_STAGES * (SPMV3_CAP * 12 + SPMV3_NCW * 16) + (size_t)SPMV3_NCW * SPMV3_WT * 8)
+#define CG_BATCH_SMEM (CG_BATCH_RING_BYTES > CG_BATCH_ZP_BYTES ? CG_BATCH_RING_BYTES : CG_BATCH_ZP_BYTES)
+typedef void (*CgBatchFn)(int, int, B200FlagView, B200FlagView, B200CgBatchArgs);
+static CgBatchFn cg_batch_fn(bool packed1, bool packed2) {
+  return packed1 ? (packed2 ? k_cg_batch<true, true> : k_cg_batch<true, false>)
+                 : (packed2 ? k_cg_batch<false, true> : k_cg_batch<false, false>);
 }
 
 
@@ -1157,7 +1517,76 @@ extern "C" int b200_cg_plan_k34(B200Cg *cg) {
   int per_sm = 0;
   CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, k_cg_update_p, VEC_THREADS, 0));
   cg->k34_fused = (long long)per_sm * b200_num_sms() >= k34_grid(cg->n) ? 1 : 0;
+  // the batch kernel: one CTA per SM must fit, and the device must take cooperative launches
+  cg->k34_batch = 0;
+  if (!cg->k34_fused) return 0;
+  static std::once_flag once;
+  std::call_once(once, [] {
+    for (int k = 0; k < 4; ++k)
+      cudaFuncSetAttribute(cg_batch_fn(k & 1, k & 2), cudaFuncAttributeMaxDynamicSharedMemorySize,
+                           (int)CG_BATCH_SMEM);
+  });
+  int dev = 0, coop = 0;
+  CUDA_OK(cudaGetDevice(&dev));
+  CUDA_OK(cudaDeviceGetAttribute(&coop, cudaDevAttrCooperativeLaunch, dev));
+  int fit = coop;
+  for (int k = 0; k < 4 && fit; ++k) {
+    CUDA_OK(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, cg_batch_fn(k & 1, k & 2), SPMV3_THREADS,
+                                                          CG_BATCH_SMEM));
+    fit = per_sm >= 1;
+  }
+  cg->k34_batch = fit;
   return 0;
+}
+
+// SCS_B200_CG_BATCH_KERNEL=0 runs every CG iteration as its three kernels (A/B runs); read once
+static std::atomic<int> g_cg_batch{-1};
+extern "C" void scs_b200_set_cg_batch_kernel(int on) { g_cg_batch = on ? 1 : 0; }
+static bool cg_batch_enabled() {
+  if (g_cg_batch < 0) {
+    const char *e = getenv("SCS_B200_CG_BATCH_KERNEL");
+    g_cg_batch = (e && atoi(e) == 0) ? 0 : 1;
+  }
+  return g_cg_batch == 1;
+}
+// the views of the reordered pair when the batch kernel can run this workspace's CG loop
+static bool cg_batch_ready(const B200Cg *cg, B200FlagView *A, B200FlagView *At) {
+  return cg->k34_batch && cg->nranks == 1 && cg->P == nullptr && cg->A_cg != nullptr && cg->At_cg != nullptr &&
+         cg->d_ry_cg != nullptr && b200_spmv_flag_view(cg->A_cg, A) == 0 && b200_spmv_flag_view(cg->At_cg, At) == 0;
+}
+static void k1_operand(const B200Cg *cg, bool re, B200SpmvArgs &a);
+static void k2_operand(const B200Cg *cg, bool re, B200SpmvArgs &a);
+// `iters` CG iterations as one cooperative launch of k_cg_batch; the caller holds the K34 token
+static cudaError_t cg_batch_launch(B200Cg *cg, const B200FlagView &A, const B200FlagView &At, double *d_x, int iters,
+                                   unsigned long long *stamps) {
+  B200CgBatchArgs a;
+  memset(&a, 0, sizeof(a));
+  a.x = d_x; a.r = cg->d_r; a.p = cg->d_p; a.Gp = cg->d_Gp; a.tmp = cg->d_tmp; a.M = cg->d_M;
+  B200SpmvArgs k;
+  memset(&k, 0, sizeof(k));
+  k1_operand(cg, true, k);
+  a.d1 = k.d_d; a.dmask1 = k.d_dmask; a.dform1 = k.dform;
+  k2_operand(cg, true, k);
+  a.d2 = k.d_d; a.dform2 = k.dform;
+  a.ctl = cg->d_ctl; a.partials = cg->d_partials; a.counter = cg->d_counter; a.bar = cg->d_counter + 8;
+  a.seq = (int *)cg->d_counter + 9;
+  a.g34 = k34_grid(cg->n);
+  a.stamps = stamps;
+  int grid = (a.g34 + 1) / 2;
+  if (A.grid > grid) grid = A.grid;
+  if (At.grid > grid) grid = At.grid;
+  cudaLaunchConfig_t cfg;
+  memset(&cfg, 0, sizeof(cfg));
+  cfg.gridDim = dim3(grid);
+  cfg.blockDim = dim3(SPMV3_THREADS);
+  cfg.dynamicSmemBytes = CG_BATCH_SMEM;
+  cfg.stream = (cudaStream_t)b200_stream();
+  cudaLaunchAttribute at[1];
+  at[0].id = cudaLaunchAttributeCooperative;
+  at[0].val.cooperative = 1;
+  cfg.attrs = at;
+  cfg.numAttrs = 1;
+  return cudaLaunchKernelEx(&cfg, cg_batch_fn(A.packed != 0, At.packed != 0), cg->n, iters, A, At, a);
 }
 
 // fused: K3 and K4 as k_cg_update_p (the caller holds the token when its grid has more than one block)
@@ -1187,7 +1616,8 @@ static int cg_iteration(B200Cg *cg, double *d_x, bool fused) {
 // another thread
 extern "C" int b200_cg_one_iteration(B200Cg *cg, double *d_x) { return cg_iteration(cg, d_x, cg->k34_fused != 0); }
 
-// The fused kernel's grid barrier under concurrency. k_cg_update_p needs all of its blocks resident at once; setup
+// The fused kernel's grid barrier under concurrency (k_cg_batch's barriers likewise: it runs only under the token).
+// k_cg_update_p needs all of its blocks resident at once; setup
 // checks that against the whole GPU. Two such grids on two streams could each get part of the SMs and wait for each
 // other until the spin gives up. So a KKT solve whose fused grid has more than one block runs it only while it holds
 // this process-wide token, taken with a try-lock (never a wait) at the start of b200_cg_solve and given back once the
@@ -1339,6 +1769,39 @@ extern "C" int b200_cg_time_kernels(B200Cg *cg, double *d_x, int reps, double *o
   return rc;
 }
 
+// The batch kernel's phases (scripts/prof_cg_batch.py): one launch of `reps` genuine iterations with the globaltimer
+// stamps of block 0. out_ms[0..3] = average per iteration of the K1 phase, the K2 phase, the update up to its beta
+// wait and the p update, each with the barrier or wait that ends it; out_ms[4] = the launch (CUDA events) per iteration.
+// -1 when the workspace cannot run the batch kernel. Timing only: it must not overlap a solve of another thread.
+extern "C" int b200_cg_time_batch(B200Cg *cg, double *d_x, int reps, double *out_ms) {
+  B200FlagView A, At;
+  if (reps <= 0 || !cg_batch_ready(cg, &A, &At)) return -1;
+  cudaStream_t st = (cudaStream_t)b200_stream();
+  const size_t bytes = (size_t)reps * 5 * sizeof(unsigned long long);
+  unsigned long long *d_stamps = (unsigned long long *)b200_malloc(bytes);
+  cudaEvent_t ev[2] = {nullptr, nullptr};
+  int rc = -1;
+  std::vector<unsigned long long> h((size_t)reps * 5);
+  if (d_stamps && cudaEventCreate(&ev[0]) == cudaSuccess && cudaEventCreate(&ev[1]) == cudaSuccess &&
+      cudaEventRecord(ev[0], st) == cudaSuccess && cg_batch_launch(cg, A, At, d_x, reps, d_stamps) == cudaSuccess &&
+      cudaEventRecord(ev[1], st) == cudaSuccess && cudaStreamSynchronize(st) == cudaSuccess &&
+      cudaMemcpy(h.data(), d_stamps, bytes, cudaMemcpyDeviceToHost) == cudaSuccess) {
+    b200_count_launch(1);
+    float ms = 0.f;
+    cudaEventElapsedTime(&ms, ev[0], ev[1]);
+    for (int k = 0; k < 4; ++k) out_ms[k] = 0.0;
+    for (int r = 0; r < reps; ++r)
+      for (int k = 0; k < 4; ++k) out_ms[k] += (double)(long long)(h[(size_t)r * 5 + k + 1] - h[(size_t)r * 5 + k]) * 1e-6;
+    for (int k = 0; k < 4; ++k) out_ms[k] /= reps;
+    out_ms[4] = ms / reps;
+    rc = 0;
+  }
+  for (auto e : ev)
+    if (e) cudaEventDestroy(e);
+  b200_free(d_stamps);
+  return rc;
+}
+
 extern "C" double b200_cg_iter_alg_bytes(const B200Cg *cg, double *per_kernel) {
   const double nnz = (double)b200_spmv_nnz(cg->A), n = cg->n, m = cg->m;
   const bool re = cg->A_cg != nullptr && cg->At_cg != nullptr && cg->d_ry_cg != nullptr;
@@ -1398,8 +1861,8 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
   b200_count_launch(1);
   CUDA_OK(cudaGetLastError());
 
-  // main loop in batches. An iteration enqueued after `done` costs 3 or 4 empty launches (~12 us), a
-  // host poll costs a ~40 us bubble: the first batch is the hint, the previous count of a solve of the same kind
+  // main loop in batches. An iteration enqueued after `done` costs 3 or 4 empty launches (~12 us; nothing in the batch
+  // kernel), a host poll costs a ~40 us bubble: the first batch is the hint, the previous count of a solve of the same kind
   // (host/linsys_b200.c), plus a 6 % margin (consecutive ADMM iterations need nearly the same number of CG steps),
   // later batches are small.
   int batch = its_hint + (its_hint / 16 > 2 ? its_hint / 16 : 2);
@@ -1408,18 +1871,34 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
   const int follow = its_hint / 8 > 8 ? (its_hint / 8 < 256 ? its_hint / 8 : 256) : 8;
   long long enq = 0;
   int polls = 0;
+  // the batch kernel when this workspace can run it and the token is free; without the token the K3 / K4 pair
   K34Token token;
-  const bool fused = cg->k34_fused && (k34_grid(n) == 1 || token.take());
+  B200FlagView vA, vAt;
+  const bool want_batch = cg_batch_enabled() && cg_batch_ready(cg, &vA, &vAt);
+  const bool held = cg->k34_fused && (want_batch || k34_grid(n) > 1) && token.take();
+  bool one_launch = want_batch && held;
+  const bool fused = cg->k34_fused && (k34_grid(n) == 1 || held);
   ++cg->k34_solves[fused ? 0 : 1];
   for (;;) {
-    for (int i = 0; i < batch; ++i)
-      if (cg_iteration(cg, d_b, fused) != 0) return -1;
+    if (one_launch) {
+      const cudaError_t e = cg_batch_launch(cg, vA, vAt, d_b, batch, nullptr);
+      if (e == cudaErrorCooperativeLaunchTooLarge || e == cudaErrorNotSupported) {
+        (void)cudaGetLastError();  // refused: this solve runs the three kernels
+        one_launch = false;
+      } else {
+        CUDA_OK(e);
+        b200_count_launch(1);
+      }
+    }
+    if (!one_launch)
+      for (int i = 0; i < batch; ++i)
+        if (cg_iteration(cg, d_b, fused) != 0) return -1;
     enq += batch;
     CUDA_OK(cudaMemcpyAsync(cg->h_ctl, cg->d_ctl, sizeof(B200CgCtl), cudaMemcpyDeviceToHost, st));
     CUDA_OK(cudaStreamSynchronize(st));
     if (cg->h_ctl->pad[0]) {
       b200_set_error(cg->nranks > 1 ? "peer-memory wait timed out in k_cg_finish_p2p"
-                                    : "grid barrier wait timed out in k_cg_update_p",
+                                    : "grid barrier wait timed out in k_cg_update_p or k_cg_batch",
                      cudaErrorUnknown, __FILE__, __LINE__);
       return -1;
     }
@@ -1432,6 +1911,7 @@ extern "C" int b200_cg_solve(B200Cg *cg, double *d_b, const double *d_s, double 
     else batch = batch < 128 ? batch * 2 : 256;
   }
   token.give_back();  // the last fused launch has finished: the host has seen the stream drain
+  if (one_launch) ++cg->k34_batch_solves;
   if (shard_x_active(cg) && !cg->h_ctl->skip) {
     // sharded-x mode: every rank owns a slice of x; all ranks need all of it for the back-substitution
     std::vector<int> xoff((size_t)cg->nranks + 1);

@@ -19,6 +19,7 @@
 // per extra row vector read by the epilogue).
 #include "../common.cuh"
 #include "../dev_api.h"
+#include "../spmv_flag.cuh"
 #include <mutex>
 #include <stdlib.h>
 #include <string.h>
@@ -43,35 +44,6 @@ struct B200Spmv {
   int borrows;       // 1: d_rowptr / d_vals / d_wt3 / d_cta_begin3 belong to another operator (renumbered-columns view)
   unsigned char *d_idx24;  // the packed index stream (b200_spmv_pack_indices; d_colidx is then NULL), or NULL
 };
-
-// random 8-byte gather of the dense vector: read-only path, optionally without L1 allocation
-__device__ __forceinline__ double gather_ld(const double *p) {
-#ifdef SPMV_GATHER_NOALLOC
-  double r;
-  asm volatile("ld.global.nc.L1::no_allocate.f64 %0, [%1];" : "=d"(r) : "l"(p));
-  return r;
-#else
-  return __ldg(p);
-#endif
-}
-// epilogue; the caller fetches the operands d[row] (dv) and v[row] (vv), the flag kernel EARLY (before the gathers
-// are consumed) so that their latency overlaps the row's chain instead of adding to it
-template <int POST>
-__device__ __forceinline__ void spmv_epilogue(double s, int row, double *__restrict__ y, double dv, double vv,
-                                              double &dot_acc) {
-  double out = s;
-  if (POST == B200_POST_DIV) {
-    out = s / dv;
-  } else if (POST == B200_POST_MUL) {
-    out = s * dv;
-  } else if (POST == B200_POST_FMA_DOT) {
-    out = fma(dv, vv, s);
-    dot_acc = fma(vv, out, dot_acc);
-  } else if (POST == B200_POST_FMA) {
-    out = fma(dv, vv, s);
-  }
-  y[row] = out;
-}
 
 // Tail of both kernels. Multi-GPU (replicated modes): the last block tells every peer that this rank's partial product
 // is complete; the push mode (B200_HOOK_P2P_ROUTE) needs no signal, every pushed row validates itself. Then, for
@@ -135,24 +107,7 @@ __device__ __forceinline__ void spmv_tail(double dot_acc, double *dot_out, int h
 //     return, so the ring runs ahead of the gather latency.
 // Rows longer than SPMV3_MAXROW entries do not fit a warp-tile: they are cut into balanced pieces
 // (spmv3_piece_end), each a "virtual row" with its own END, and spmv_combine_kernel adds the pieces.
-// defaults: ONE CTA of 768 threads per SM (1 producer + 23 consumer warps), 3 stages = 130 kB of shared
-// memory (within the H100's 227 kB per block), which leaves ~125 kB of the 256 kB L1/shared array to the gathers
-#ifndef SPMV3_THREADS
-#define SPMV3_THREADS 768
-#endif
-#ifndef SPMV3_STAGES
-#define SPMV3_STAGES 3
-#endif
-#ifndef SPMV3_CTAS_PER_SM
-#define SPMV3_CTAS_PER_SM 1
-#endif
-#define SPMV3_NCW (SPMV3_THREADS / 32 - 1)
-#define SPMV3_WT 128
-#define SPMV3_CAP (SPMV3_NCW * SPMV3_WT + 8)
-#define SPMV3_MAXROW 124
-// the kernel forms stream positions up to stored + 128 in 32-bit int (kb = (k0 & ~3) + 4 * lane, ka + cnt)
-#define SPMV3_MAX_STORED B200_MAX_STORED
-
+// The ring's geometry and the per-stage work of producer and consumers: spmv_flag.cuh.
 static size_t spmv3_smem_bytes() {
   return (size_t)SPMV3_STAGES * (SPMV3_CAP * 12 + SPMV3_NCW * 16) + 2 * SPMV3_STAGES * 8 + 64 * 8 +
          (size_t)SPMV3_NCW * SPMV3_WT * 8;
@@ -199,23 +154,6 @@ __host__ __device__ __forceinline__ unsigned spmv3_same_sum_phases(int len, int 
   return (1u << (6 - len < 4 ? 6 - len : 4)) - 1u;
 }
 
-// Packed index stream of the CG loop's operators (an operator with at most 2^22 columns): 3 bytes per entry, the
-// column in bits 0..21, END in bit 22, SKIP in bit 23. The one encode / decode of that format; decode gives back the
-// int32 entry (flags in bits 31 / 30) bit for bit.
-#define SPMV3_IDX24_MAXCOLS (1 << 22)
-__host__ __device__ __forceinline__ unsigned spmv3_idx24_encode(int v) {
-  const unsigned u = (unsigned)v;
-  return (u & 0x3fffffu) | ((u >> 31) & 1u) << 22 | ((u >> 30) & 1u) << 23;
-}
-__host__ __device__ __forceinline__ int spmv3_idx24_decode(unsigned e) {
-  return (int)((e & 0x3fffffu) | ((e >> 22) & 1u) << 31 | ((e >> 23) & 1u) << 30);
-}
-// The packed slice of a stage's entries [ka, ka + cnt) (ka a multiple of 4): a 1-D bulk copy needs a 16-byte aligned
-// address and a length that is a multiple of 16, so it starts at entry ka & ~15 (byte 3 * (ka & ~15)) and its length
-// is rounded up. At most 12 + 5 entries more than the int32 slice, which is still less than 4 * cnt bytes.
-__host__ __device__ __forceinline__ unsigned spmv3_idx24_slice_bytes(int ka, int cnt) {
-  return (unsigned)((3 * (ka + cnt - (ka & ~15)) + 15) & ~15);
-}
 
 
 // IDX24: the index stream is packed (spmv3_idx24_*), else int32
@@ -264,6 +202,7 @@ spmv_flag_kernel(const void *__restrict__ colidx, const double *__restrict__ val
 
   double dot_acc = 0.0;
   int skipped = 0;
+  const Spmv3Ring R = {s_vals, s_idx, s_desc, s_full, s_empty, s_out};
   if (wid == 0) {
     // ------------------------------------------------ producer (one elected lane)
     if (lane == 0) {
@@ -292,16 +231,7 @@ spmv_flag_kernel(const void *__restrict__ colidx, const double *__restrict__ val
           }
           mbar_wait(&s_empty[st], (unsigned)((use - 1) & 1));
         }
-        const unsigned ib = IDX24 ? spmv3_idx24_slice_bytes(ka, cnt) : (unsigned)cnt * 4u;
-        mbar_expect_tx(&s_full[st], (unsigned)cnt * 8u + ib + (unsigned)(SPMV3_NCW * 16));
-        tma_load_1d(s_desc + (size_t)st * SPMV3_NCW, g + (size_t)i * SPMV3_NCW, SPMV3_NCW * 16,
-                    &s_full[st], pol);
-        if (IDX24)
-          tma_load_1d(s_idx + (size_t)st * SPMV3_CAP,
-                      static_cast<const unsigned char *>(colidx) + 3 * (size_t)(ka & ~15), ib, &s_full[st], pol);
-        else
-          tma_load_1d(s_idx + (size_t)st * SPMV3_CAP, static_cast<const int *>(colidx) + ka, ib, &s_full[st], pol);
-        tma_load_1d(s_vals + (size_t)st * SPMV3_CAP, vals + ka, (unsigned)cnt * 8u, &s_full[st], pol);
+        spmv3_issue_stage<IDX24>(R, st, g, i, ka, cnt, colidx, vals, pol);
       }
       if (!waited) {
         pdl_wait();
@@ -321,165 +251,16 @@ spmv_flag_kernel(const void *__restrict__ colidx, const double *__restrict__ val
     // ------------------------------------------------ consumers: one warp-tile per warp per stage
     pdl_wait();
     if (skip != nullptr && *((volatile const int *)skip) != 0) skipped = 1;
-    const int cw = wid - 1;
-    double *ws = s_out + cw * SPMV3_WT;
-    const unsigned FULL = 0xffffffffu;
-    const unsigned lt = (1u << lane) - 1u;
-    const unsigned le = lt | (1u << lane);
-    const int sw = (lane >> 2) & 1;
     // the table forms of d (B200_D_ONE / B200_D_TWO): its values, once per launch
     constexpr bool TAB = POST == B200_POST_MUL || POST == B200_POST_FMA_DOT || POST == B200_POST_FMA;
-    double dt0 = 0.0, dt1 = 0.0;
+    Spmv3Epi E = {x, y, init, init_sign, d, dmask, dform, 0.0, 0.0, v, routed, s_rt_lo, s_rt_dst, hook_val};
     if (TAB && dform != B200_D_VEC) {
-      dt0 = d[0];
-      dt1 = dform == B200_D_TWO ? d[1] : dt0;
+      E.dt0 = d[0];
+      E.dt1 = dform == B200_D_TWO ? d[1] : E.dt0;
     }
-    for (int i = 0; i < (skipped ? 0 : nt); ++i) {
-      const int st = i % SPMV3_STAGES;
-      const unsigned par = (unsigned)((i / SPMV3_STAGES) & 1);
-      mbar_wait(&s_full[st], par);
-      const int4 dsc = s_desc[st * SPMV3_NCW + cw];
-      const int ka = s_desc[st * SPMV3_NCW].y & ~3;
-      const int row0 = dsc.x, k0 = dsc.y, cnt = dsc.z;
-      const int kend = k0 + cnt;
-      const int kb = (k0 & ~3) + 4 * lane;  // global index of this lane's first entry
-      int4 iv = make_int4(0, 0, 0, 0);
-      double2 t0 = make_double2(0.0, 0.0), t1 = make_double2(0.0, 0.0);
-      const bool any = (kb < kend) && (kb + 4 > k0);
-      if (any) {
-        const int e = kb - ka;
-        if (IDX24) {  // 12 bytes from byte 3 * (kb - (ka & ~15)), a multiple of 12: three conflict-free 32-bit LDS
-          const unsigned *wp = reinterpret_cast<const unsigned *>(
-              reinterpret_cast<const unsigned char *>(s_idx + (size_t)st * SPMV3_CAP) + 3 * (kb - (ka & ~15)));
-          const unsigned w0 = wp[0], w1 = wp[1], w2 = wp[2];
-          iv = make_int4(spmv3_idx24_decode(w0 & 0xffffffu), spmv3_idx24_decode(w0 >> 24 | (w1 & 0xffffu) << 8),
-                         spmv3_idx24_decode(w1 >> 16 | (w2 & 0xffu) << 16), spmv3_idx24_decode(w2 >> 8));
-        } else {
-          iv = *reinterpret_cast<const int4 *>(s_idx + (size_t)st * SPMV3_CAP + e);
-        }
-        t0 = *reinterpret_cast<const double2 *>(s_vals + (size_t)st * SPMV3_CAP + e + 2 * sw);
-        t1 = *reinterpret_cast<const double2 *>(s_vals + (size_t)st * SPMV3_CAP + e + 2 - 2 * sw);
-      }
-      const bool v0 = any && (kb >= k0), v1 = any && (kb + 1 >= k0) && (kb + 1 < kend),
-                 v2 = any && (kb + 2 >= k0) && (kb + 2 < kend), v3 = any && (kb + 3 < kend);
-      const bool g0 = v0 && !(iv.x & B200_FLAG_SKIP), g1 = v1 && !(iv.y & B200_FLAG_SKIP),
-                 g2 = v2 && !(iv.z & B200_FLAG_SKIP), g3 = v3 && !(iv.w & B200_FLAG_SKIP);
-      // 4 independent gathers in flight per lane
-      const double x0 = g0 ? gather_ld(&x[iv.x & B200_COLMASK]) : 0.0;
-      const double x1 = g1 ? gather_ld(&x[iv.y & B200_COLMASK]) : 0.0;
-      const double x2 = g2 ? gather_ld(&x[iv.z & B200_COLMASK]) : 0.0;
-      const double x3 = g3 ? gather_ld(&x[iv.w & B200_COLMASK]) : 0.0;
-      // the stage's bytes are in registers (the gather addresses depend on them): hand it back
-      __syncwarp();
-      if (lane == 0) mbar_arrive(&s_empty[st]);
-      if (cnt == 0) continue;  // padding descriptor (warp-uniform)
-      const int nrows_w = dsc.w;
-      // epilogue operands of the first two rounds (rows row0 + lane, row0 + lane + 32): in flight
-      // together with the gathers
-      // (B200_D_TWO: the mask words, at most two per round; the table value is selected at the use)
-      double pd0 = 0.0, pd1 = 0.0, pv0 = 0.0, pv1 = 0.0, pi0 = 0.0, pi1 = 0.0;
-      unsigned pw0 = 0u, pw1 = 0u;
-      {
-        const bool r0ok = lane < nrows_w, r1ok = lane + 32 < nrows_w;
-        if (POST != B200_POST_NONE) {
-          if (!TAB || dform == B200_D_VEC) {
-            if (r0ok) pd0 = d[row0 + lane];
-            if (r1ok) pd1 = d[row0 + lane + 32];
-          } else if (TAB && dform == B200_D_TWO) {
-            if (r0ok) pw0 = dmask[(row0 + lane) >> 5];
-            if (r1ok) pw1 = dmask[(row0 + lane + 32) >> 5];
-          }
-        }
-        if (POST == B200_POST_FMA_DOT || POST == B200_POST_FMA) {
-          if (r0ok) pv0 = v[row0 + lane];
-          if (r1ok) pv1 = v[row0 + lane + 32];
-        }
-        if (init != nullptr) {
-          if (r0ok) pi0 = init[row0 + lane];
-          if (r1ok) pi1 = init[row0 + lane + 32];
-        }
-      }
-
-      const double a0 = sw ? t1.x : t0.x, a1 = sw ? t1.y : t0.y;
-      const double a2 = sw ? t0.x : t1.x, a3 = sw ? t0.y : t1.y;
-      const bool e0 = v0 && (iv.x < 0), e1 = v1 && (iv.y < 0), e2 = v2 && (iv.z < 0), e3 = v3 && (iv.w < 0);
-      const unsigned b0 = __ballot_sync(FULL, e0), b1 = __ballot_sync(FULL, e1);
-      const unsigned b2 = __ballot_sync(FULL, e2), b3 = __ballot_sync(FULL, e3);
-      const unsigned ends = b0 | b1 | b2 | b3;  // lanes in which at least one row ends
-      // row number (within the warp-tile) of the first END of this lane = number of ENDs in the lanes before it
-      int r = __popc(b0 & lt) + __popc(b1 & lt) + __popc(b2 & lt) + __popc(b3 & lt);
-      // open-row segments: the tail of lane h (the last lane <= me in which a row ends) starts the
-      // row that is open when my entries begin
-      const unsigned mle = ends & le;
-      const int h = mle ? 31 - __clz(mle) : 0;
-      const int maxdist = __reduce_max_sync(FULL, lane - h);
-
-      const double p0 = g0 ? __dmul_rn(a0, x0) : 0.0, p1 = g1 ? __dmul_rn(a1, x1) : 0.0;
-      const double p2 = g2 ? __dmul_rn(a2, x2) : 0.0, p3 = g3 ? __dmul_rn(a3, x3) : 0.0;
-      // in-lane sequential sums, restarted after every END (0 + p is exact)
-      double acc = p0;
-      double o0 = acc;
-      if (e0) acc = 0.0;
-      acc = __dadd_rn(acc, p1);
-      double o1 = acc;
-      if (e1) acc = 0.0;
-      acc = __dadd_rn(acc, p2);
-      double o2 = acc;
-      if (e2) acc = 0.0;
-      acc = __dadd_rn(acc, p3);
-      double o3 = acc;
-      if (e3) acc = 0.0;
-      // segmented inclusive scan of the tails (Hillis-Steele, fixed order)
-      double I = acc;
-      for (int dd = 1; dd <= maxdist; dd <<= 1) {
-        const double up = __shfl_up_sync(FULL, I, dd);
-        if (lane - dd >= h) I = __dadd_rn(up, I);
-      }
-      double carry = __shfl_up_sync(FULL, I, 1);
-      if (lane == 0) carry = 0.0;  // warp-tiles hold whole rows: nothing is open at entry 0
-      // the first END of the lane closes the row that was open on entry
-      if (e0) o0 = __dadd_rn(carry, o0);
-      else if (e1) o1 = __dadd_rn(carry, o1);
-      else if (e2) o2 = __dadd_rn(carry, o2);
-      else if (e3) o3 = __dadd_rn(carry, o3);
-      // transpose through the warp's scratch: row sums by row number, then a COALESCED epilogue
-      // (one row per lane and round: full-sector stores of y, one division per row, operands of the
-      // first two rounds were fetched before the gathers were consumed)
-      if (e0) { ws[r] = o0; ++r; }
-      if (e1) { ws[r] = o1; ++r; }
-      if (e2) { ws[r] = o2; ++r; }
-      if (e3) { ws[r] = o3; }
-      __syncwarp();
-#pragma unroll
-      for (int j = 0; j < SPMV3_WT / 32; ++j) {
-        const int rr = lane + 32 * j;
-        if (j * 32 >= nrows_w) break;  // warp-uniform
-        if (rr < nrows_w) {
-          const int row = row0 + rr;
-          double sres = ws[rr];
-          double dv, vv, iv0;
-          unsigned dw;
-          if (j == 0) { dv = pd0; dw = pw0; vv = pv0; iv0 = pi0; }
-          else if (j == 1) { dv = pd1; dw = pw1; vv = pv1; iv0 = pi1; }
-          else {
-            dv = (POST != B200_POST_NONE && (!TAB || dform == B200_D_VEC)) ? d[row] : 0.0;
-            dw = (TAB && dform == B200_D_TWO) ? dmask[row >> 5] : 0u;
-            vv = (POST == B200_POST_FMA_DOT || POST == B200_POST_FMA) ? v[row] : 0.0;
-            iv0 = (init != nullptr) ? init[row] : 0.0;
-          }
-          if (TAB && dform != B200_D_VEC) dv = (dw >> (row & 31)) & 1u ? dt1 : dt0;
-          if (init != nullptr) sres = __dadd_rn(sres, init_sign * iv0);
-          if (routed) {  // push the row to the rank that owns it, as a self-validating 16-byte element
-            int o = 0;
-            while (row >= s_rt_lo[o + 1]) ++o;
-            ll_store(s_rt_dst[o] + 2 * (size_t)(row - s_rt_lo[o]), sres, (unsigned)hook_val);
-          } else {
-            spmv_epilogue<POST>(sres, row, y, dv, vv, dot_acc);
-          }
-        }
-      }
-      __syncwarp();  // the scratch is rewritten by the next warp-tile
-    }
+    for (int i = 0; i < (skipped ? 0 : nt); ++i)
+      spmv3_consume_stage<POST, IDX24, true>(R, i % SPMV3_STAGES, (unsigned)((i / SPMV3_STAGES) & 1), wid - 1, lane,
+                                             E, dot_acc);
   }
 
   if (skipped) return;  // uniform over the CTA: every thread read the same *skip after the predecessor completed
@@ -1227,6 +1008,18 @@ extern "C" int b200_spmv(const B200Spmv *M, const B200SpmvArgs *a) {
 #undef LAUNCH_IDX
   b200_count_launch(1);
   CUDA_OK(cudaGetLastError());
+  return 0;
+}
+extern "C" int b200_spmv_flag_view(const B200Spmv *M, B200FlagView *out) {
+  if (!b200_spmv_can_route(M)) return -1;
+  out->idx = M->d_idx24 != nullptr ? (const void *)M->d_idx24 : (const void *)M->d_colidx;
+  out->vals = M->d_vals;
+  out->wt = M->d_wt3;
+  out->cta_begin = M->d_cta_begin3;
+  out->grid = M->grid;
+  out->packed = M->d_idx24 != nullptr ? 1 : 0;
+  out->partials = M->d_partials;
+  out->counter = M->d_counter;
   return 0;
 }
 // B200_HOOK_P2P_ROUTE needs the one-pass kernel (no virtual rows / combine pass)
